@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- novel-views/sec of the B200 splat rasterizer on BASELINE config C2
+"""bench.py -- novel-views/sec of the H100 splat rasterizer on BASELINE config C2
 (1024x1024, ~500k pixel-aligned Gaussians, fixed novel camera), plus the roofline of the dominant
 kernel, the CPU baseline and the end-to-end (host-buffer) number.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--views V] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--views V] [--impl reference] [--dump-outputs DIR]
 
 A "step" = R passes of the hot path over one batch of V independent synthetic view-pairs per GPU (seeds 1314+k, the C4
 sharding unit); R = ceil(2000 / steps) so that the timed region is >= ~2.5 s of GPU work whatever --steps is (a burst of a
@@ -15,6 +15,9 @@ collective (inference), `scaling: weak`.  `--train-c5` instead times the referen
 --impl reference: the reference has no runnable implementation of this path here (its rasterizer is the
 absent third-party CUDA extension; lib/TaichiRender.py needs taichi + CUDA), so that arm times the CPU
 oracle PORT of the same algorithm on the host cores (the one other place bench.py may execute oracle/).
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the timed path returned in its last step as float32 .npy
+files (see dump_outputs), so that two builds can be compared output for output on the same seeded inputs.
 """
 import argparse
 import json
@@ -41,12 +44,12 @@ def _peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
-    """SM clock + throttle reasons sampled DURING the timed region (NVML; same fields as the nvidia-smi recipe
-    in B200_PROFILING.md: clocks.sm, clocks.max.sm, clocks_event_reasons.*)."""
+    """SM clock + throttle reasons sampled DURING the timed region (NVML; the fields nvidia-smi reports as clocks.sm,
+    clocks.max.sm, clocks_event_reasons.*)."""
 
     def __init__(self, gpu_index, period_s=0.01):
         self.idx, self.period = gpu_index, period_s
@@ -109,7 +112,7 @@ def passes_per_step(steps, override=0):
 
 
 def bench_config(V, R, **extra):
-    """The `config` object: identical in the b200 and the reference arm (VERDICT r1 weak #11)."""
+    """The `config` object: identical in the b200 and the reference arm."""
     cfg = {"workload": WORKLOAD, "views_per_pass_per_gpu": int(V), "passes_per_step": int(R),
            "views_per_step_per_gpu": int(V * R)}
     cfg.update(extra)
@@ -119,7 +122,7 @@ def bench_config(V, R, **extra):
 def _source_hash(kernel="render_forward_kernel"):
     """sha256 over the CODE of a compositing kernel's sources (// comments and whitespace stripped, so a reworded comment
     does not invalidate a capture): stamps profiles/render_forward_traffic.json so that a stale ncu traffic figure is refused
-    instead of silently reported (VERDICT r1 weak #12)."""
+    instead of silently reported."""
     import hashlib
     import re
     h = hashlib.sha256()
@@ -131,18 +134,46 @@ def _source_hash(kernel="render_forward_kernel"):
     return h.hexdigest()
 
 
+TRAFFIC_FILE = os.path.join(ROOT, "profiles", "render_forward_traffic.json")
+
+
 def _traffic(kernel):
-    tp = os.path.join(ROOT, "profiles", "render_forward_traffic.json")
     try:
-        j = json.load(open(tp))
+        j = json.load(open(TRAFFIC_FILE))
     except Exception:
-        return None, "no profiles/render_forward_traffic.json"
+        return None, "no profiles/render_forward_traffic.json (no ncu capture of these kernels)"
     ent = j.get(kernel) if isinstance(j.get(kernel), dict) else (j if kernel == "render_forward_kernel" else None)
     if not ent:
         return None, "kernel not in traffic file"
     if ent.get("source_sha256") != _source_hash(kernel):
         return None, "stale: kernel sources changed since the ncu capture (source_sha256 mismatch)"
     return float(ent["dram_bytes_per_launch"]), ent.get("from", "ncu --set full")
+
+
+DUMP_SAMPLE = 1 << 22          # pixel values of all views in color_sample.npy (16 MB)
+DUMP_RADII = 1 << 20           # radii of all views in radii_sample.npy (4 MB)
+
+
+def dump_outputs(out_dir, colors, radii, num_rendered):
+    """What the timed path returned in its last step, as float32 / float64 .npy files (about 33 MB at 1024^2, whatever the
+    number of views): color_view0 = the whole [3,H,W] image of the first view; color_sample = a fixed, seeded sample
+    (DUMP_SAMPLE values, same indices in every run) of the flattened [V,3,H,W] images of all views; radii_sample = the same
+    kind of sample (DUMP_RADII values) of every view's int32 radii, concatenated; num_rendered = the pair count of each
+    view.  Inputs are seeded, so the same arguments give the same inputs."""
+    import torch
+
+    def sample(flat, n, seed):
+        idx = np.sort(np.random.default_rng(seed).choice(flat.numel(), size=min(n, flat.numel()), replace=False))
+        return flat[torch.from_numpy(idx).to(flat.device)]
+
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"color_view0": colors[0].float().cpu().numpy(),
+              "color_sample": sample(torch.stack(colors).reshape(-1), DUMP_SAMPLE, 1314).float().cpu().numpy(),
+              "radii_sample": sample(torch.cat([r.reshape(-1) for r in radii]), DUMP_RADII, 1315).float().cpu().numpy(),
+              "num_rendered": np.asarray(num_rendered, np.float64)}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20, "output dump exceeds 64 MB"
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def _scenes(n, first_seed):
@@ -230,7 +261,7 @@ def run_reference_arm(args, rank, world):
 
 
 def _corr_section(dev, hbm_peak_gbs):
-    """Volume + pyramid build (fp16 tcgen05 kernel / fp16 + fp32 FFMA kernels) and the fused 4-level lookup, CUDA-event timed."""
+    """Volume + pyramid build (fp16 wgmma kernel / fp16 + fp32 FFMA kernels) and the fused 4-level lookup, CUDA-event timed."""
     import torch
     from gps_gaussian_b200 import _lib
     from gps_gaussian_b200.corr import CorrBlockFast1D
@@ -256,10 +287,10 @@ def _corr_section(dev, hbm_peak_gbs):
     out = {"shape": [B, D, H, W]}
     alg = lambda s: 2 * B * D * H * W * s + 1.875 * B * H * W * W * s          # SURVEY 8d: features in, volume + pyramid out
     with torch.no_grad():
-        out["build_fp16_tcgen05_ms"] = timed(lambda: CorrBlockFast1D(f16[0], f16[1]))
+        out["build_fp16_wgmma_ms"] = timed(lambda: CorrBlockFast1D(f16[0], f16[1]))
         _lib.set_corr_build("ffma")
         out["build_fp16_ffma_ms"] = timed(lambda: CorrBlockFast1D(f16[0], f16[1]))
-        _lib.set_corr_build("tcgen05")
+        _lib.set_corr_build("wgmma")
         out["build_fp32_ffma_ms"] = timed(lambda: CorrBlockFast1D(f32[0], f32[1]))
         blk = CorrBlockFast1D(f16[0], f16[1])
         out["lookup_4level_fp16_ms"] = timed(lambda: blk(coords))
@@ -280,10 +311,10 @@ def _corr_section(dev, hbm_peak_gbs):
     def bwd():
         v0 = CorrBlockFast1D.corr(fa, fb_).squeeze(3)
         torch.autograd.grad(v0, (fa, fb_), gvol)
-    out["build_fwd_bwd_fp16_tcgen05_ms"] = timed(bwd, 20)
+    out["build_fwd_bwd_fp16_wgmma_ms"] = timed(bwd, 20)
     _lib.set_corr_build("ffma")
     out["build_fwd_bwd_fp16_ffma_ms"] = timed(bwd, 20)
-    _lib.set_corr_build("tcgen05")
+    _lib.set_corr_build("wgmma")
     # CPU port beside it (oracle, scalar C, 1 thread) on a bounded sample: 8 of the 128 rows of the same problem
     try:
         from oracle.corr_oracle import CorrOracle
@@ -325,7 +356,7 @@ def _corr_section(dev, hbm_peak_gbs):
         roof = {}
         for key, name, nbytes in (("corr_forward", "corr_lookup_fwd_kernel (fused 4 levels)", b_look),
                                   ("corr_backward", "corr_lookup_bwd_kernel (fused 4 levels)", b_look_bwd),
-                                  ("corr_build", "corr_build_tc_kernel (tcgen05)", alg(2))):
+                                  ("corr_build", "corr_build_tc_kernel (wgmma)", alg(2))):
             if pr.get(key, {}).get("calls"):
                 ms = pr[key]["ms"] / pr[key]["calls"]
                 roof[key] = {"kernel": name, "kernel_ms": ms, "algorithmic_bytes_per_launch": nbytes, "achieved_gbps": nbytes / (ms * 1e-3) / 1e9,
@@ -333,8 +364,8 @@ def _corr_section(dev, hbm_peak_gbs):
         out["kernel_rooflines"] = roof
     except Exception as exc:
         out["kernel_rooflines"] = {"error": repr(exc)[:200]}
-    out["build_fp16_tcgen05_gbps"] = alg(2) / (out["build_fp16_tcgen05_ms"] * 1e-3) / 1e9
-    out["build_fp16_tcgen05_hbm_frac"] = out["build_fp16_tcgen05_gbps"] / hbm_peak_gbs
+    out["build_fp16_wgmma_gbps"] = alg(2) / (out["build_fp16_wgmma_ms"] * 1e-3) / 1e9
+    out["build_fp16_wgmma_hbm_frac"] = out["build_fp16_wgmma_gbps"] / hbm_peak_gbs
     out["note"] = "wall of the Python call (allocation of the 4 level tensors + 1 launch), CUDA events, back-to-back"
     return out
 
@@ -487,14 +518,14 @@ def _train_section(dev, calls, ndup, P, steps, V, peak):
 
 def _c3_section(dev, n_steps=6):
     """BASELINE config C3 on this GPU: the reference's OWN RtStereoHumanModel + loader + train_stage2.py:57-89 step (AMP,
-    GradScaler) from baseline/_ref against the drop-ins, 512^2 sources / 1024^2 render, batch 2 -- plain drop-ins and with
+    GradScaler) from oracle/_ref against the drop-ins, 512^2 sources / 1024^2 render, batch 2 -- plain drop-ins and with
     the GPSG_PATCH fused paths.  Stage split by CUDA events between the statements of the step; rasterizer kernel time from
     the library's own per-kernel events."""
     import tempfile
     import torch
     from gps_gaussian_b200 import _lib, harness, patch, synth_dataset
     if harness.staged_reference() is None:
-        return {"unavailable": "baseline/_ref not staged (build() stages it where /root/reference is mounted)"}
+        return {"unavailable": "oracle/_ref not staged (build() stages it where the original project is checked out)"}
     root = tempfile.mkdtemp(prefix="gpsg_c3_")
     synth_dataset.write_dataset(root, n_train=2, n_val=1, res=512, hr=True)
     out = {"config": "C3: reference RtStereoHumanModel (5 144 408 params), AMP + GradScaler, batch 2, 512^2 stereo pair -> "
@@ -545,7 +576,7 @@ def dict_copy(data):
 
 
 def run_c5(args, rank, world, local_rank):
-    """BASELINE config C5: stage-2 TRAINING data-parallel -- the reference's own model + step from baseline/_ref, 2 stereo
+    """BASELINE config C5: stage-2 TRAINING data-parallel -- the reference's own model + step from oracle/_ref, 2 stereo
     pairs of 1024^2 per GPU (2048^2 novel view, use_hr_img), ONE flat NCCL all-reduce (5 144 408 fp32 = 20.6 MB) between
     backward and unscale_ (train_stage2.py:83-85).  metric: pixels/s of source-pair pixels trained on (16 x 1024^2 per
     step at N=8), plus the exposed all-reduce time (step with all-reduce minus step without)."""
@@ -614,7 +645,7 @@ def run_c5(args, rank, world, local_rank):
         line = {"metric": "stage2_train_source_pixels_per_sec", "value": px / (ms * 1e-3), "unit": "pixels/s", "n_gpus": world,
                 "steps": args.steps, "warmup": max(3, args.warmup), "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "fp16 autocast nets + fp32 rasterizer (reference AMP)", "data": "synthetic",
-                "config": {"workload": f"C5: stage-2 training, reference RtStereoHumanModel from baseline/_ref, 2 pairs/GPU of {res}^2 "
+                "config": {"workload": f"C5: stage-2 training, reference RtStereoHumanModel from oracle/_ref, 2 pairs/GPU of {res}^2 "
                                        f"(render {2 * res}^2), global batch {2 * world}, flat NCCL all-reduce of 5144408 fp32 grads",
                            "fast_paths": "GPSG_PATCH fused paths" if args.patch else "plain drop-ins", "parallelism": f"dp{world}"},
                 "exposed_comm_ms": res_ms["with_allreduce_stages"].get("allreduce"),
@@ -648,6 +679,8 @@ def main():
     ap.add_argument("--train-c5", action="store_true", help="time data-parallel stage-2 training (C5) instead of the render")
     ap.add_argument("--c5-res", type=int, default=1024)
     ap.add_argument("--patch", action="store_true", help="C5: use the GPSG_PATCH fused paths")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the images (and radii) the timed path computed in its last step to DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -728,6 +761,9 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     prof_overlapped = _lib.profile_read()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, [pr.color for pr in planned], [pr.radii[:c.P] for pr, c in zip(planned, calls)],
+                     [pr.status()["num_rendered"] for pr in planned])
     clocks = sampler.stop()
     ms = shard.max_over_ranks(ms, dev)
     # Per-kernel durations for the roofline: with several streams the kernels of different views time-share the SMs, so
@@ -907,7 +943,7 @@ def main():
             "config": bench_config(V, R, P_mean=float(np.mean(P)), N_dup_mean=nd,
                                    parallelism=f"view-pairs sharded over {world} GPU(s); {len(side)} CUDA stream(s) per GPU",
                                    l2=f"{V} distinct scenes per pass, ~{(56 * np.mean(P) + 96 * nd + 20 * hw) / 1e6:.0f} MB touched per "
-                                      "view > 126 MB L2 between reuses",
+                                      "view > 50 MB L2 between reuses",
                                    timed_region_s=ms * 1e-3),
             "roofline": {"bound": "hbm", "kernel": "render_forward_kernel", "achieved": achieved, "peak": peak,
                          "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src,

@@ -2,7 +2,7 @@
 from the valid pixel-aligned Gaussians of both source views into data['novel_view']['img_pred'] [B,3,H,W].
 
 The reference boolean-mask-gathers ten maps per sample (each gather is a `nonzero` + index_select, i.e. a host sync),
-concatenates the two views, rescales the colours and only then calls `render`.  Here the sm_100a rasterizer reads the
+concatenates the two views, rescales the colours and only then calls `render`.  Here the sm_90a rasterizer reads the
 maps in place (`gpsg_rasterize_forward_maps`): invalid pixels are culled inside the projection kernel, colours are
 img*0.5+0.5 on the fly, and the backward writes gradients directly in map layout.  Same signature, same result
 (Gaussian order = lmain pixels then rmain pixels, exactly the order of the reference's gather + concat).
@@ -40,12 +40,12 @@ class _RasterizeMaps(torch.autograd.Function):
         rot, scale = [_f32(rl.detach()), _f32(rr.detach())], [_f32(sl.detach()), _f32(sr.detach())]
         opac = [_f32(ol.detach()), _f32(orr.detach())]
         if valid[1].numel() != S2:
-            raise RuntimeError("pts2render (gpsg_sm100): lmain and rmain pts_valid differ in size")
+            raise RuntimeError("pts2render (gpsg): lmain and rmain pts_valid differ in size")
         for t, n in ((xyz, 3), (img, 3), (rot, 4), (scale, 3), (opac, 1)):
             if any(u.numel() != n * S2 for u in t):
-                raise RuntimeError("pts2render (gpsg_sm100): map shapes do not match pts_valid")
+                raise RuntimeError("pts2render (gpsg): map shapes do not match pts_valid")
         if any(u.device != dev for t in (valid, xyz, img, rot, scale, opac) for u in t):
-            raise RuntimeError("pts2render (gpsg_sm100): all source-view maps must live on one CUDA device")
+            raise RuntimeError("pts2render (gpsg): all source-view maps must live on one CUDA device")
         H, W = int(settings.image_height), int(settings.image_width)
         color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((2 * S2,), dtype=torch.int32, device=dev)
@@ -115,7 +115,7 @@ class _RasterizeMapsBatch(torch.autograd.Function):
         for b in range(B):
             st = settings_list[b]
             if int(st.image_height) != H or int(st.image_width) != W:
-                raise RuntimeError("pts2render (gpsg_sm100): all samples of a batch must render at one resolution")
+                raise RuntimeError("pts2render (gpsg): all samples of a batch must render at one resolution")
             vl, xl, il, rl, sl, ol, vr, xr, ir_, rr, sr, orr = maps[12 * b:12 * b + 12]
             S2 = int(vl.numel())
             valid = [vl.contiguous().view(torch.uint8), vr.contiguous().view(torch.uint8)]
@@ -123,12 +123,12 @@ class _RasterizeMapsBatch(torch.autograd.Function):
             rot, scale = [_f32(rl.detach()), _f32(rr.detach())], [_f32(sl.detach()), _f32(sr.detach())]
             opac = [_f32(ol.detach()), _f32(orr.detach())]
             if valid[1].numel() != S2:
-                raise RuntimeError("pts2render (gpsg_sm100): lmain and rmain pts_valid differ in size")
+                raise RuntimeError("pts2render (gpsg): lmain and rmain pts_valid differ in size")
             for t, n in ((xyz, 3), (img, 3), (rot, 4), (scale, 3), (opac, 1)):
                 if any(u.numel() != n * S2 for u in t):
-                    raise RuntimeError("pts2render (gpsg_sm100): map shapes do not match pts_valid")
+                    raise RuntimeError("pts2render (gpsg): map shapes do not match pts_valid")
             if any(u.device != dev for t in (valid, xyz, img, rot, scale, opac) for u in t):
-                raise RuntimeError("pts2render (gpsg_sm100): all source-view maps must live on one CUDA device")
+                raise RuntimeError("pts2render (gpsg): all source-view maps must live on one CUDA device")
             radii = torch.empty((2 * S2,), dtype=torch.int32, device=dev)
             ptrs = (_ptrs(valid), _ptrs(xyz), _ptrs(img), _ptrs(rot), _ptrs(scale), _ptrs(opac))
             _lib.begin_alloc(dev)

@@ -1,4 +1,4 @@
-"""ctypes binding of libgpsg_sm100.so (the C ABI declared in include/gpsg.h).
+"""ctypes binding of libgpsg_sm90.so (the C ABI declared in include/gpsg.h).
 
 There is NO fallback: if the shared library is missing this module raises at import time --
 a product path that silently ran on the CPU oracle or on eager PyTorch would void every parity
@@ -9,7 +9,7 @@ import os
 import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "libgpsg_sm100.so")
+LIB_PATH = os.path.join(_HERE, "lib", "libgpsg_sm90.so")
 
 
 class GpsgError(RuntimeError):
@@ -42,7 +42,7 @@ ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} not found: the CUDA extension is not built. Run `python gps-gaussian_b200/build.py` "
-        "(nvcc, sm_100a). There is deliberately no CPU / PyTorch fallback.")
+        "(nvcc, sm_90a). There is deliberately no CPU / PyTorch fallback.")
 
 lib = C.CDLL(LIB_PATH)
 
@@ -176,8 +176,8 @@ lib.gpsg_set_corr_build.restype = _i
 lib.gpsg_set_corr_build.argtypes = [_i]
 
 
-def set_corr_build(kind="tcgen05"):
-    """'tcgen05' (default: tensor-core kernels for fp16 volumes when the shape fits) or 'ffma'."""
+def set_corr_build(kind="wgmma"):
+    """'wgmma' (default: tensor-core kernels for fp16 volumes when the shape fits) or 'ffma'."""
     check(lib.gpsg_set_corr_build(1 if kind == "ffma" else 0), "gpsg_set_corr_build")
 
 

@@ -1,8 +1,8 @@
-"""Build libgpsg_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libgpsg_sm90.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python gps-gaussian_b200/build.py [--force] [--verbose]
 
-Output: gps-gaussian_b200/lib/libgpsg_sm100.so (git-ignored; travels to the GPU box with gpurun).
+Output: gps-gaussian_b200/lib/libgpsg_sm90.so (git-ignored build product).
 raster_preprocess.cu is compiled with -fmad=false (see its header): the fp32 op order that decides
 radii / tile rectangles must not be FMA-contracted.
 """
@@ -15,9 +15,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "lib")
-LIB = os.path.join(LIBDIR, "libgpsg_sm100.so")
+LIB = os.path.join(LIBDIR, "libgpsg_sm90.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
           "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 SOURCES = {

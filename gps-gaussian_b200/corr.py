@@ -2,7 +2,7 @@
 `CorrSampler` (autograd.Function over `corr_sampler.forward/backward`) and `CorrBlockFast1D(fmap1, fmap2,
 num_levels=4, radius=4)` with `__call__(coords[B,2,H,W]) -> [B, num_levels*(2r+1), H, W]`.
 
-Same names, ctor kwargs and results; the work is done by sm_100a kernels:
+Same names, ctor kwargs and results; the work is done by sm_90a kernels:
   * ctor: ONE fused launch builds the all-pairs volume, applies 1/sqrt(D) and pools the whole pyramid
     (reference: batched GEMM + divide + 3 avg_pool2d + reshape copies);
   * call: ONE fused launch looks up all levels and writes the concatenated [B,36,H,W] tensor
@@ -55,7 +55,7 @@ class _BuildPyramid(torch.autograd.Function):
     @staticmethod
     def forward(ctx, fmap1, fmap2, levels):
         if fmap1.dtype not in _DT or fmap2.dtype != fmap1.dtype or not fmap1.is_cuda:
-            raise RuntimeError("CorrBlockFast1D (gpsg_sm100): fmaps must be CUDA fp16/fp32 tensors of one dtype")
+            raise RuntimeError("CorrBlockFast1D (gpsg): fmaps must be CUDA fp16/fp32 tensors of one dtype")
         f1, f2 = fmap1.detach().contiguous(), fmap2.detach().contiguous()
         B, D, H, W1 = f1.shape
         W2 = f2.shape[3]
@@ -78,7 +78,7 @@ class _BuildPyramid(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         # Chain of avg_pool2d([1,2]) folded back to level 0 (cheap elementwise torch ops), then the two contractions
-        # dF1 = F2 g^T, dF2 = F1 g in one sm_100a kernel each (gpsg_corr_build_backward).
+        # dF1 = F2 g^T, dF2 = F1 g in one sm_90a kernel each (gpsg_corr_build_backward).
         f1, f2 = ctx.saved_tensors
         B, D, H, W1 = f1.shape
         W2 = f2.shape[3]
@@ -149,7 +149,7 @@ class _LookupPyramid(torch.autograd.Function):
 class CorrBlockFast1D:
     def __init__(self, fmap1, fmap2, num_levels=4, radius=4):
         if num_levels > 4:
-            raise ValueError("CorrBlockFast1D (gpsg_sm100): at most 4 pyramid levels")
+            raise ValueError("CorrBlockFast1D (gpsg): at most 4 pyramid levels")
         self.num_levels = num_levels
         self.radius = radius
         self._vols = _BuildPyramid.apply(fmap1, fmap2, num_levels)

@@ -11,7 +11,7 @@
 
 namespace gpsg {
 
-// 0 = tcgen05 / TMEM kernels for fp16 volumes when the shape fits (default), 1 = always the FFMA kernels.  Process-wide; set
+// 0 = wgmma tensor-core kernels for fp16 volumes when the shape fits (default), 1 = always the FFMA kernels.  Process-wide; set
 // through gpsg_set_corr_build() (tests and bench.py compare the two formulations) -- the environment variable GPSG_CORR_BUILD
 // is only read ONCE, for the initial value (r1 called getenv on every launch).
 static std::atomic<int> g_corr_build_mode{-1};
@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(256) corr_build_kernel(int B, int D, int H, in
 int launch_corr_build(int dtype, int B, int D, int H, int W1, int W2, const void* f1, const void* f2, void* v0, void* v1,
                       void* v2, void* v3, int levels, cudaStream_t stream) {
     if ((int64_t)B * H * W1 * W2 == 0) return GPSG_OK;
-    {   // fp16 (stage-2 AMP) volumes go to the tcgen05 kernel (corr_tc.cu) when the shape fits; gpsg_set_corr_build(1) / GPSG_CORR_BUILD=ffma at start-up opts out
+    {   // fp16 (stage-2 AMP) volumes go to the wgmma kernel (corr_tc.cu) when the shape fits; gpsg_set_corr_build(1) / GPSG_CORR_BUILD=ffma at start-up opts out
         void* lv[4] = {v0, v1, v2, v3};
         if (corr_build_mode() == 0 && corr_build_tc_supported(dtype, D, W1, W2, f1, f2, lv, levels))
             return launch_corr_build_tc(B, D, H, W1, W2, f1, f2, v0, v1, v2, v3, levels, stream);
@@ -431,7 +431,7 @@ __global__ void __launch_bounds__(256) corr_build_bwd_kernel(int D, int H, int N
 int launch_corr_build_bwd(int dtype, int B, int D, int H, int W1, int W2, const void* f1, const void* f2, const void* g,
                           void* df1, void* df2, cudaStream_t stream) {
     if ((int64_t)B * D * H * W1 * W2 == 0) return GPSG_OK;
-    {   // fp16: tcgen05 kernels (corr_tc.cu) when the shape fits; gpsg_set_corr_build(1) / GPSG_CORR_BUILD=ffma at start-up opts out
+    {   // fp16: wgmma kernels (corr_tc.cu) when the shape fits; gpsg_set_corr_build(1) / GPSG_CORR_BUILD=ffma at start-up opts out
         if (corr_build_mode() == 0 && corr_build_bwd_tc_supported(dtype, D, W1, W2, f1, f2, g, df1, df2))
             return launch_corr_build_bwd_tc(B, D, H, W1, W2, f1, f2, g, df1, df2, stream);
     }

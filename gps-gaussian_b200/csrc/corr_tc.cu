@@ -1,22 +1,22 @@
-// corr_tc.cu -- the fp16 correlation-volume build on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a only.
+// corr_tc.cu -- the fp16 correlation-volume build on the Hopper tensor cores (warpgroup MMA, wgmma), sm_90a.
 //
 // Same contract as corr_build_kernel<__half> in corr.cu (reference core/corr.py:53-61 under stage-2 AMP: volume =
 // einsum('aijk,aijh->ajkh', f1, f2) / sqrt(D), then the avg_pool2d([1,2]) pyramid of core/corr.py:36-42, every level
 // rounded to fp16 like the torch op chain).  Per (b, h) the volume is the GEMM  C[x, y] = sum_d F1[d, x] * F2[d, y]:
-// M = W1 (tiles of 128), N = W2 (<= 128), K = D.  Both operands are "MN-major" in the UMMA sense -- the feature maps
-// are [B, D, H, W] with W contiguous, so for a fixed (b, h) the M (resp. N) index is the contiguous one -- which
-// tcgen05.mma.kind::f16 accepts directly (instruction-descriptor a_major = b_major = 1): no transpose anywhere.
+// M = W1 (tiles of 128), N = W2 (<= 128), K = D.  Both operands are "MN-major" -- the feature maps are [B, D, H, W] with
+// W contiguous, so for a fixed (b, h) the M (resp. N) index is the contiguous one -- which wgmma accepts directly for
+// fp16 (imm-trans-a = imm-trans-b = 1): no transpose anywhere.
 //
-// One CTA (256 threads) per (M tile, b, h):
+// One CTA (256 threads = two warpgroups) per (M tile, b, h):
 //   1. all warps copy the [D x 128] / [D x N] operand panels global -> shared in 16-byte chunks, placing them in the
 //      no-swizzle canonical layout (8 x 8 "core matrices" of 128 contiguous bytes: 8 K rows x 16 B of 8 MN elements;
 //      MN-adjacent cores 128 B apart (SBO), K-adjacent core groups one panel row of cores apart (LBO));
-//   2. ONE thread issues D/16 tcgen05.mma (UMMA 128 x N x 16, fp32 accumulate in TMEM) and a tcgen05.commit on an
-//      mbarrier;
-//   3. all 8 warps read their TMEM quadrant back with tcgen05.ld (32 lanes x 16 columns per instruction; thread = one
-//      volume row x, 16 consecutive y), scale / round / pool down the pyramid in registers and store 16-byte vectors.
-// 98 KB of shared memory and 128 TMEM columns per CTA at D = 192: two CTAs per SM, so one CTA's loads overlap the
-// other's MMA + epilogue.  HBM-bound by design: 2*D*W*2 B in, 1.875*W1*W2*2 B out per (b, h).
+//   2. warpgroup g issues D/16 x N/16 wgmma.m64n16k16 for volume rows 64g .. 64g+63, fp32 accumulators in registers;
+//   3. the accumulators are scaled / rounded to fp16 into a shared-memory tile (which reuses the operand panels), and
+//      thread = one volume row x then reads 16 consecutive y, pools down the pyramid in registers and stores 16-byte
+//      vectors (a warp writes 32 full rows of every level).
+// 96 KB of shared memory per CTA at D = 192, N = 128: two CTAs per SM, so one CTA's loads overlap the other's MMA +
+// epilogue.  HBM-bound by design: 2*D*W*2 B in, 1.875*W1*W2*2 B out per (b, h).
 #include "gpsg_internal.cuh"
 #include "tma_bulk.cuh"
 
@@ -27,42 +27,60 @@ namespace gpsg {
 namespace {
 
 constexpr int kTcThreads = 256;
-constexpr int kTcM = 128;              // UMMA M (rows of the volume per CTA)
-constexpr uint32_t kTmemCols = 128;    // power of two >= N
+constexpr int kTcM = 128;              // volume rows per CTA: warpgroup g owns rows 64g .. 64g+63
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// shared-memory matrix descriptor, no swizzle (layout_type 0), version 1 (Blackwell); offsets in 16-byte units
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// shared-memory matrix descriptor (sm_90 GMMA), no swizzle (layout type 0); address and offsets in 16-byte units
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= 1ull << 46;
     return d;
 }
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 16] (+)= A[64 x 16] B[16 x 16], fp16 in, fp32 accumulate; TA / TB = 1: the operand is MN-major in shared memory
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, int accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB)
         : "memory");
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accesses of the accumulators across the asynchronous MMAs that own them
+template <int NC>
+__device__ __forceinline__ void fence_acc(float (&acc)[NC][8]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) asm volatile("" : "+f"(acc[c][i])::"memory");
+}
+
+// acc[c] = A x B[:, 16c .. 16c+15] for c < nch over ksteps K-steps of 16.  a0 / b0: shared addresses of this warpgroup's
+// A rows and of the B panel; A's K-adjacent core groups are 2048 B apart, B's lbo_b; MN-adjacent cores 128 B apart.
+template <int TA, int TB, int NC>
+__device__ __forceinline__ void warpgroup_mma(float (&acc)[NC][8], uint32_t a0, uint32_t b0, uint32_t lbo_b, int ksteps,
+                                              int nch) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
+    fence_acc(acc);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    for (int s = 0; s < ksteps; ++s) {
+        const uint64_t da = gmma_desc(a0 + (uint32_t)s * 2u * 2048u, 2048u, 128u);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+            if (c < nch)
+                wgmma_m64n16k16<TA, TB>(acc[c], da, gmma_desc(b0 + (uint32_t)s * 2u * lbo_b + (uint32_t)c * 256u, lbo_b, 128u),
+                                        s > 0);
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    fence_acc(acc);
 }
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, uint32_t src_bytes) {
@@ -81,6 +99,20 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
     const __half2 h = __halves2half2(__float2half_rn(a), __float2half_rn(b));
     return *reinterpret_cast<const uint32_t*>(&h);
 }
+__device__ __forceinline__ void unpack8(uint4 u, float* v) {
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+        v[2 * i] = f.x;
+        v[2 * i + 1] = f.y;
+    }
+}
+
+// Accumulator fragment of wgmma m64nNk16 (fp32): thread (warp w of the warpgroup, lane l) holds, per 16-column chunk,
+// rows 16w + l/4 (+8) and columns 2(l%4) (+1) (+8): element i -> row + 8*((i>>1)&1), column 8*(i>>2) + 2(l%4) + (i&1).
+__device__ __forceinline__ int frag_row(int i, int lane, int warp_in_wg) { return 16 * warp_in_wg + (lane >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int i, int lane) { return 8 * (i >> 2) + 2 * (lane & 3) + (i & 1); }
 
 __global__ void __launch_bounds__(kTcThreads) corr_build_tc_kernel(int D, int H, int W1, int W2,
                                                                    const __half* __restrict__ f1,
@@ -88,8 +120,6 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_tc_kernel(int D, int H,
                                                                    __half* __restrict__ v1, __half* __restrict__ v2,
                                                                    __half* __restrict__ v3, int levels, float div) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(8) uint64_t bar;
-    __shared__ uint32_t tmem_slot;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int x_base = blockIdx.x * kTcM;
     const int b = blockIdx.y / H, h = blockIdx.y % H;
@@ -97,17 +127,6 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_tc_kernel(int D, int H,
     const int KC = D >> 3;                                      // K core groups
     uint8_t* sA = smem;                                         // [KC][16 cores][128 B]
     uint8_t* sB = smem + (size_t)KC * 2048;                     // [KC][NB cores][128 B]
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                     "r"(kTmemCols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 32) {
-        mbar_init(&bar, 1);
-        mbar_fence_init();
-    }
 
     // ---- operand panels -> shared, canonical no-swizzle MN-major layout --------------------------------------------
     // a warp moves one K core group (8 d rows) x 4 chunks of 8 elements: lanes 0-7 -> rows of chunk 0 (128 contiguous
@@ -118,7 +137,7 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_tc_kernel(int D, int H,
     const __half* g2 = f2 + (size_t)b * D * plane2 + (size_t)h * W2;
     const int cl = lane >> 3, dl = lane & 7;
     // cp.async (LDGSTS): every thread puts all of its 16-byte copies in flight before waiting on any of them -- the whole
-    // 2*D*W*2-byte panel pair is outstanding at once (register-staged loads stalled on the scoreboard after 4).
+    // 2*D*W*2-byte panel pair is outstanding at once.
     for (int it = warp; it < KC * 4; it += kTcThreads / 32) {
         const int kc = it >> 2, c = (it & 3) * 4 + cl;
         const bool in = x_base + c * 8 < W1;                      // ragged last M tile: zero-fill (src-size 0)
@@ -131,106 +150,91 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_tc_kernel(int D, int H,
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
 
-    // ---- MMA: one thread, D/16 instructions of 128 x N x 16 ------------------------------------------------------------
-    if (tid == 0) {
-        // instruction descriptor: D fp32 (bits 4-5 = 1), A/B fp16 (0), A and B MN-major (bits 15, 16), N>>3 at 17, M>>4 at 24
-        const uint32_t idesc = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(W2 >> 3) << 17) | ((uint32_t)(kTcM >> 4) << 24);
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-        const uint32_t lbo_b = (uint32_t)NB * 128u;
-        for (int s = 0; s < (D >> 4); ++s) {
-            const uint64_t da = umma_desc(a0 + (uint32_t)s * 2u * 2048u, 2048u, 128u);
-            const uint64_t db = umma_desc(b0 + (uint32_t)s * 2u * lbo_b, lbo_b, 128u);
-            umma_f16(tmem, da, db, idesc, s > 0 ? 1u : 0u);
+    // ---- MMA: warpgroup wg computes volume rows 64 wg .. 64 wg + 63, all N columns --------------------------------------
+    const int wg = warp >> 2, wwg = warp & 3;
+    float acc[8][8];
+    warpgroup_mma<1, 1>(acc, smem_u32(sA) + (uint32_t)wg * 1024u, smem_u32(sB), (uint32_t)NB * 128u, D >> 4, W2 >> 4);
+    __syncthreads();                                             // both warpgroups are done reading the panels
+
+    // ---- epilogue 1: scale + round to fp16 into a [128][W2 + 8] tile over the panels (row pad: conflict-free stores) ----
+    const float rdiv = __frcp_rn(div);
+    const int ld = W2 + 8;
+    __half* S = reinterpret_cast<__half*>(smem);
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        if (c < (W2 >> 4)) {
+#pragma unroll
+            for (int i = 0; i < 8; i += 2) {
+                const int r = wg * 64 + frag_row(i, lane, wwg), col = c * 16 + frag_col(i, lane);
+                // einsum result in fp16, then the division in fp16
+                *reinterpret_cast<uint32_t*>(S + r * ld + col) =
+                    pack2(div_rn_fast(rh(acc[c][i]), div, rdiv), div_rn_fast(rh(acc[c][i + 1]), div, rdiv));
+            }
         }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar))
-                     : "memory");
     }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
+    __syncthreads();
 
-    // ---- epilogue: TMEM -> registers -> scale / round / pool -> global -------------------------------------------------
-    const int quad = warp & 3;                                  // TMEM lanes 32*quad .. +31 belong to this warp
-    const int x = x_base + quad * 32 + lane;
+    // ---- epilogue 2: thread = one volume row x, 16-column batches -> pool -> global -------------------------------------
+    const int xr = tid & (kTcM - 1);
+    const int x = x_base + xr;
     const size_t row = ((size_t)b * H + h) * W1 + x;
     const int Wl1 = W2 >> 1, Wl2 = W2 >> 2, Wl3 = W2 >> 3;
-    const float rdiv = __frcp_rn(div);
-    for (int j = warp >> 2; j < (W2 >> 4); j += 2) {            // 16-column batches, split between the two warp sets
-        float acc[16];
-        __syncwarp();                                            // tcgen05.ld is .sync.aligned: whole warp, converged
-        tmem_ld16(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(j * 16), acc);
-        if (x < W1) {
-        float q0[16], q1[8], q2[4], q3[2];
+    if (x < W1) {
+        for (int j = warp >> 2; j < (W2 >> 4); j += 2) {        // 16-column batches, split between the two warp sets
+            const uint4* src = reinterpret_cast<const uint4*>(S + xr * ld + j * 16);
+            const uint4 u0 = src[0], u1 = src[1];
+            float q0[16], q1[8], q2[4], q3[2];
+            unpack8(u0, q0);
+            unpack8(u1, q0 + 8);
+            uint4* o0 = reinterpret_cast<uint4*>(v0 + row * W2 + j * 16);
+            o0[0] = u0;
+            o0[1] = u1;
+            if (levels > 1) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) q0[i] = rh(div_rn_fast(rh(acc[i]), div, rdiv));   // einsum result in fp16, then the division in fp16
-        uint4* o0 = reinterpret_cast<uint4*>(v0 + row * W2 + j * 16);
-        o0[0] = make_uint4(pack2(q0[0], q0[1]), pack2(q0[2], q0[3]), pack2(q0[4], q0[5]), pack2(q0[6], q0[7]));
-        o0[1] = make_uint4(pack2(q0[8], q0[9]), pack2(q0[10], q0[11]), pack2(q0[12], q0[13]), pack2(q0[14], q0[15]));
-        if (levels > 1) {
+                for (int i = 0; i < 8; ++i) q1[i] = rh((q0[2 * i] + q0[2 * i + 1]) * 0.5f);
+                *reinterpret_cast<uint4*>(v1 + row * Wl1 + j * 8) =
+                    make_uint4(pack2(q1[0], q1[1]), pack2(q1[2], q1[3]), pack2(q1[4], q1[5]), pack2(q1[6], q1[7]));
+            }
+            if (levels > 2) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) q1[i] = rh((q0[2 * i] + q0[2 * i + 1]) * 0.5f);
-            *reinterpret_cast<uint4*>(v1 + row * Wl1 + j * 8) =
-                make_uint4(pack2(q1[0], q1[1]), pack2(q1[2], q1[3]), pack2(q1[4], q1[5]), pack2(q1[6], q1[7]));
-        }
-        if (levels > 2) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) q2[i] = rh((q1[2 * i] + q1[2 * i + 1]) * 0.5f);
-            *reinterpret_cast<uint2*>(v2 + row * Wl2 + j * 4) = make_uint2(pack2(q2[0], q2[1]), pack2(q2[2], q2[3]));
-        }
-        if (levels > 3) {
-            q3[0] = rh((q2[0] + q2[1]) * 0.5f);
-            q3[1] = rh((q2[2] + q2[3]) * 0.5f);
-            *reinterpret_cast<uint32_t*>(v3 + row * Wl3 + j * 2) = pack2(q3[0], q3[1]);
-        }
+                for (int i = 0; i < 4; ++i) q2[i] = rh((q1[2 * i] + q1[2 * i + 1]) * 0.5f);
+                *reinterpret_cast<uint2*>(v2 + row * Wl2 + j * 4) = make_uint2(pack2(q2[0], q2[1]), pack2(q2[2], q2[3]));
+            }
+            if (levels > 3) {
+                q3[0] = rh((q2[0] + q2[1]) * 0.5f);
+                q3[1] = rh((q2[2] + q2[3]) * 0.5f);
+                *reinterpret_cast<uint32_t*>(v3 + row * Wl3 + j * 2) = pack2(q3[0], q3[1]);
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemCols) : "memory");
 }
 
 // =====================================================================================================================
 // Backward of the build on the tensor cores (fp16): per (b, h), with g = d(loss)/d(level-0 volume) [W1 x W2],
 //   dF1[d, x] = sum_y g[x, y] F2[d, y] / sqrt(D)        A_MN = false:  M = x, N = d, K = y;  A = g rows (K-major)
 //   dF2[d, y] = sum_x g[x, y] F1[d, x] / sqrt(D)        A_MN = true :  M = y, N = d, K = x;  A = g columns (MN-major)
-// computed transposed (C^T[m, d]) so that M is the 128-wide volume axis and N = D (a multiple of 16 up to 256, which
-// M = 64/128 UMMA shapes accept); B = the other feature map's [D x K] panel, K-contiguous (K-major) in both cases.
+// computed transposed (C^T[m, d]) so that M is the 128-wide volume axis (two warpgroups of 64 rows) and N = D (a multiple
+// of 16 up to 256); B = the other feature map's [D x K] panel, K-contiguous (K-major) in both cases.
 // Shared layout: the same 128-byte core matrices as the forward -- K-major cores hold 8 MN rows x 16 B of 8 K elements.
-// Thread = one TMEM lane = one m; its 16-column batches are 16 different d planes of the output, so a warp stores 64
-// contiguous bytes per (d, 32 m).
+// The fp16 results go through a [D][128 + 8] shared tile (over the panels), so that a warp stores 512 contiguous bytes
+// of one d plane of the output.
 // =====================================================================================================================
 template <bool A_MN>
 __global__ void __launch_bounds__(kTcThreads) corr_build_bwd_tc_kernel(int D, int H, int W1, int W2,
                                                                        const __half* __restrict__ fmap,
                                                                        const __half* __restrict__ g,
-                                                                       __half* __restrict__ dfmap, float div,
-                                                                       uint32_t tmem_cols) {
+                                                                       __half* __restrict__ dfmap, float div) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(8) uint64_t bar;
-    __shared__ uint32_t tmem_slot;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int b = blockIdx.y / H, h = blockIdx.y % H;
     const int Kdim = A_MN ? W1 : W2, Mdim = A_MN ? W2 : W1;
-    const int KC = ((Kdim + 15) & ~15) >> 3;                    // K core groups, K padded to the UMMA K of 16 with zeros
+    const int KC = ((Kdim + 15) & ~15) >> 3;                    // K core groups, K padded to the MMA K of 16 with zeros
     const int m_base = blockIdx.x * kTcM;
     const int NB = D >> 3;
     uint8_t* sA = smem;                                         // [KC][16 M cores][128 B]
     uint8_t* sB = smem + (size_t)KC * 2048;                     // [KC][NB N cores][128 B]
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                     "r"(tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 32) {
-        mbar_init(&bar, 1);
-        mbar_fence_init();
-    }
     const __half* gbh = g + ((size_t)b * H + h) * W1 * W2;
     const int cl = lane >> 3, dl = lane & 7;
     const int KCg = (KC + 3) >> 2;
@@ -263,45 +267,47 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_bwd_tc_kernel(int D, in
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
-    if (tid == 0) {
-        const uint32_t idesc = (1u << 4) | (A_MN ? (1u << 15) : 0u) | ((uint32_t)(D >> 3) << 17) | ((uint32_t)(kTcM >> 4) << 24);
-        const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-        const uint32_t lbo_b = (uint32_t)NB * 128u;
-        for (int s = 0; s < (KC >> 1); ++s) {
-            const uint64_t da = umma_desc(a0 + (uint32_t)s * 2u * 2048u, 2048u, 128u);
-            const uint64_t db = umma_desc(b0 + (uint32_t)s * 2u * lbo_b, lbo_b, 128u);
-            umma_f16(tmem, da, db, idesc, s > 0 ? 1u : 0u);
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar))
-                     : "memory");
-    }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
-    const int quad = warp & 3;
-    const int m = m_base + quad * 32 + lane;
+
+    const int wg = warp >> 2, wwg = warp & 3;
+    float acc[16][8];
+    warpgroup_mma<A_MN ? 1 : 0, 0>(acc, smem_u32(sA) + (uint32_t)wg * 1024u, smem_u32(sB), (uint32_t)NB * 128u, KC >> 1, D >> 4);
+    __syncthreads();                                             // both warpgroups are done reading the panels
+
     const float rdiv = __frcp_rn(div);
-    __half* o = dfmap + ((size_t)b * D * H + h) * Mdim + m;     // + d * H * Mdim
-    const size_t dplane = (size_t)H * Mdim;
-    for (int j = warp >> 2; j < (D >> 4); j += 2) {
-        float acc[16];
-        __syncwarp();
-        tmem_ld16(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(j * 16), acc);
-        if (m < Mdim) {
+    constexpr int ld = kTcM + 8;
+    __half* S = reinterpret_cast<__half*>(smem);                 // [D][ld]: S[d][m - m_base]
 #pragma unroll
-            for (int i = 0; i < 16; ++i) o[(size_t)(j * 16 + i) * dplane] = __float2half_rn(div_rn_fast(acc[i], div, rdiv));
+    for (int c = 0; c < 16; ++c) {
+        if (c < (D >> 4)) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+                S[(c * 16 + frag_col(i, lane)) * ld + wg * 64 + frag_row(i, lane, wwg)] =
+                    __float2half_rn(div_rn_fast(acc[c][i], div, rdiv));
         }
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
+    __half* o = dfmap + ((size_t)b * D * H + h) * Mdim + m_base;    // + d * H * Mdim
+    const size_t dplane = (size_t)H * Mdim;
+    for (int it = tid; it < D * (kTcM / 8); it += kTcThreads) {
+        const int d = it >> 4, m8 = (it & 15) * 8;
+        if (m_base + m8 < Mdim)
+            *reinterpret_cast<uint4*>(o + (size_t)d * dplane + m8) = *reinterpret_cast<const uint4*>(S + d * ld + m8);
+    }
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// dynamic shared memory: the operand panels, or the fp16 result tile that later reuses them, whichever is larger
+size_t fwd_smem_bytes(int D, int W2) {
+    const size_t panels = (size_t)D * 256 + (size_t)D * W2 * 2, tile = (size_t)kTcM * (W2 + 8) * 2;
+    return panels > tile ? panels : tile;
+}
+size_t bwd_smem_bytes(int D, int Kdim) {
+    const size_t kc = (size_t)((Kdim + 15) & ~15) >> 3;
+    const size_t panels = kc * (2048 + (size_t)D * 16), tile = (size_t)D * (kTcM + 8) * 2;
+    return panels > tile ? panels : tile;
+}
 
 }  // namespace
 
@@ -309,7 +315,7 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) ==
 bool corr_build_tc_supported(int dtype, int D, int W1, int W2, const void* f1, const void* f2, void* const* v, int levels) {
     if (dtype != 1) return false;
     if (D < 16 || (D & 15) || W1 < 8 || (W1 & 7) || W2 < 16 || (W2 & 15) || W2 > 128) return false;
-    if ((size_t)D * 256 + (size_t)D * W2 * 2 > 200 * 1024) return false;
+    if (fwd_smem_bytes(D, W2) > 200 * 1024) return false;
     if (!aligned16(f1) || !aligned16(f2)) return false;
     for (int l = 0; l < levels && l < 4; ++l)
         if (!aligned16(v[l])) return false;
@@ -318,7 +324,7 @@ bool corr_build_tc_supported(int dtype, int D, int W1, int W2, const void* f1, c
 
 int launch_corr_build_tc(int B, int D, int H, int W1, int W2, const void* f1, const void* f2, void* v0, void* v1, void* v2,
                          void* v3, int levels, cudaStream_t stream) {
-    const size_t smem = (size_t)D * 256 + (size_t)D * W2 * 2;
+    const size_t smem = fwd_smem_bytes(D, W2);
     GPSG_CUDA(cudaFuncSetAttribute(corr_build_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     dim3 grid((W1 + kTcM - 1) / kTcM, B * H);
     GPSG_REQUIRE(grid.y <= 65535, "corr build: B*H too large");
@@ -333,25 +339,22 @@ bool corr_build_bwd_tc_supported(int dtype, int D, int W1, int W2, const void* f
                                  const void* d1, const void* d2) {
     if (dtype != 1) return false;
     if (D < 16 || (D & 15) || D > 256 || W1 < 8 || (W1 & 7) || W2 < 16 || (W2 & 15) || W2 > 128) return false;
-    const size_t kc1 = (size_t)((W2 + 15) & ~15) >> 3, kc2 = (size_t)((W1 + 15) & ~15) >> 3;
-    if (kc1 * (2048 + (size_t)D * 16) > 200 * 1024 || kc2 * (2048 + (size_t)D * 16) > 200 * 1024) return false;
+    if (bwd_smem_bytes(D, W2) > 200 * 1024 || bwd_smem_bytes(D, W1) > 200 * 1024) return false;
     return aligned16(f1) && aligned16(f2) && aligned16(g) && aligned16(d1) && aligned16(d2);
 }
 
 int launch_corr_build_bwd_tc(int B, int D, int H, int W1, int W2, const void* f1, const void* f2, const void* g, void* df1,
                              void* df2, cudaStream_t stream) {
-    const uint32_t cols = D <= 32 ? 32u : D <= 64 ? 64u : D <= 128 ? 128u : 256u;
     const float div = sqrtf((float)D);
-    const size_t kc1 = (size_t)((W2 + 15) & ~15) >> 3, kc2 = (size_t)((W1 + 15) & ~15) >> 3;
-    const size_t smem1 = kc1 * (2048 + (size_t)D * 16), smem2 = kc2 * (2048 + (size_t)D * 16);
+    const size_t smem1 = bwd_smem_bytes(D, W2), smem2 = bwd_smem_bytes(D, W1);
     GPSG_REQUIRE((size_t)B * H <= 65535, "corr build backward: B*H too large");
     GPSG_CUDA(cudaFuncSetAttribute(corr_build_bwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
     GPSG_CUDA(cudaFuncSetAttribute(corr_build_bwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
     corr_build_bwd_tc_kernel<false><<<dim3((W1 + kTcM - 1) / kTcM, B * H), kTcThreads, smem1, stream>>>(
-        D, H, W1, W2, (const __half*)f2, (const __half*)g, (__half*)df1, div, cols);
+        D, H, W1, W2, (const __half*)f2, (const __half*)g, (__half*)df1, div);
     GPSG_LAUNCH_CHECK();
     corr_build_bwd_tc_kernel<true><<<dim3(1, B * H), kTcThreads, smem2, stream>>>(D, H, W1, W2, (const __half*)f1,
-                                                                                (const __half*)g, (__half*)df2, div, cols);
+                                                                                (const __half*)g, (__half*)df2, div);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

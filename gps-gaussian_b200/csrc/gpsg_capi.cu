@@ -1,4 +1,4 @@
-// gpsg_capi.cu -- the extern "C" boundary of libgpsg_sm100.so (declared in include/gpsg.h).
+// gpsg_capi.cu -- the extern "C" boundary of libgpsg_sm90.so (declared in include/gpsg.h).
 // Host-side orchestration only; kernels live in raster_*.cu / corr.cu.
 #include <cstdarg>
 #include <cstdio>
@@ -193,7 +193,7 @@ using namespace gpsg;
 extern "C" {
 
 GPSG_API const char* gpsg_last_error(void) { return g_err; }
-int gpsg_version(void) { return 100; }
+int gpsg_version(void) { return 90; }
 
 // The exact (one host read) forward in two halves, so that a BATCH of samples needs one host synchronisation in total
 // (lib/GaussianRender.py:8 loops over the samples; upstream synchronises once per sample to read num_rendered):

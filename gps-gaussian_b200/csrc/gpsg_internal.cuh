@@ -1,4 +1,4 @@
-// gpsg_internal.cuh -- shared declarations of libgpsg_sm100.so (sm_100a only).
+// gpsg_internal.cuh -- shared declarations of libgpsg_sm90.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -182,7 +182,7 @@ int launch_unproject_bwd(int B, int S, const float* depth, const float* mask, in
                          const float* extr, int extr_rows, const float* ref_intr, const float* Tf_x,
                          const float* dL_dxyz, const float* dL_ddepth, float* dL_dflow, cudaStream_t stream);
 // corr.cu
-int corr_build_mode();            // 0 = tcgen05 when possible, 1 = FFMA kernels
+int corr_build_mode();            // 0 = wgmma when possible, 1 = FFMA kernels
 void set_corr_build_mode(int m);
 int launch_corr_fwd(int dtype, int B, int H, int W1, int W2, const void* vol, int64_t sb, int64_t sh, int64_t sw1,
                     const float* coords, int64_t csb, int r, void* out, cudaStream_t stream);

@@ -9,7 +9,7 @@ namespace gpsg {
 
 constexpr int kBwdChunk = 64;   // Gaussians per ring stage
 #ifndef GPSG_BWD_STAGES
-#define GPSG_BWD_STAGES 8       // ring depth / CTAs per SM of the backward kernel (compile-time knobs; sweep in the kernel header)
+#define GPSG_BWD_STAGES 8       // ring depth / CTAs per SM of the backward kernel (compile-time knobs)
 #endif
 #ifndef GPSG_BWD_BLOCKS
 #define GPSG_BWD_BLOCKS 4
@@ -19,7 +19,7 @@ constexpr int kBwdWarps = 4;    // consumer warps per CTA: 16 x 8 pixels (half a
 // ---------------------------------------------------------------------------------------------------------------------
 // A.6: pixel-major replay + GAUSSIAN-major reduction.
 // (A first formulation reduced the 9 per-pixel products of every survivor across the warp with a butterfly reduce-scatter and
-// spent ~2/3 of its instructions doing so: 443 us at C2 against 304 us for this one -- removed in round 2.)  Here the
+// spent most of its instructions doing so; it was slower than this one and was removed.)  Here the
 // sequential part (per pixel, back to front: alpha, T, the running colour) only produces the two scalars every gradient
 // term is linear in,  s = G * opacity * dL/dalpha  and  w = alpha * T,  and parks them in shared memory, one row of 32 pixels
 // per surviving Gaussian.  Once kQ = 16 rows are parked the roles flip: lane (j, h) owns Gaussian j and pixel rows
@@ -29,7 +29,7 @@ constexpr int kBwdWarps = 4;    // consumer warps per CTA: 16 x 8 pixels (half a
 // 128-bit vector reductions (`REDG.E.ADD.F32x4`, sm_90+) into a packed per-Gaussian accumulator row of 12 floats
 //   acc[id] = { (S s dx, S s dy, S s dx^2, S s dx dy), (S s dy^2, S s, S w g_r, S w g_g), (S w g_b, -, -, -) }:
 // one v4 RED from the lower half-warp, one v4 + one scalar RED from the upper -- 3 L2 reduction sectors per (warp,
-// Gaussian) instead of 9 (ncu r1: 16.4 M RED sectors = 526 MB of L2 traffic against 47 MB algorithmic).
+// Gaussian) instead of 9.
 // Rows are padded to 33 floats: conflict-free both when a pixel-lane writes column `lane` of row `slot` and when
 // Gaussian-lanes read `row j, column p`.
 // The per-pixel replay is branch-free in its state: an inactive (pixel, Gaussian) pair is replayed with G = 0, hence
@@ -49,10 +49,9 @@ struct __align__(16) BwdWarpBuf {
 // (as the forward does front to back), so the replay loop walks fixed shared-memory addresses two survivors per iteration:
 // no find-first-set / mask update / index arithmetic per survivor, and the loads, the conic polynomial and the ex2 of the
 // second survivor are issued before the first one's dependent transmittance / colour chain (the r1 loop had one survivor in
-// flight).  Ring + park buffers + queues = 51 KB > the 48 KB static limit: dynamic shared memory, 4 CTAs / SM, 8-stage ring
-// (measured at C2: <8 stages,4 CTAs> 251-254 us, <6,4> 266, <6,5> 254, <5,5> 267, <4,5> 280, <3,5> 294, <4,6> 298, <10,4> 299
-// (3 CTAs): depth of the ring -- how far a fast warp may run ahead of the slowest of its CTA -- matters more than a fifth or
-// sixth CTA; r1's one-survivor loop with scalar REDs: 304).
+// flight).  Ring + park buffers + queues = 51 KB > the 48 KB static limit: dynamic shared memory, 4 CTAs / SM (4 x 51 KB fits
+// the 228 KB of an H100 SM), 8-stage ring: the depth of the ring -- how far a fast warp may run ahead of the slowest of its
+// CTA -- is what the stage count trades against CTAs per SM.
 // ---------------------------------------------------------------------------------------------------------------------
 struct __align__(16) BwdQueue {
     float4 X[34];      // (mean x, mean y, Gaussian id bits, list position bits)

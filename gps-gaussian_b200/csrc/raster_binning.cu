@@ -1,7 +1,7 @@
 // raster_binning.cu -- tile binning (SURVEY.md Appendix A.3; upstream rasterizer_impl.cu:
 // InclusiveSum -> duplicateWithKeys -> SortPairs -> identifyTileRanges).
 //
-// B200 redesign of the last step: after the sort, one pass gathers every pair's render parameters
+// Redesign of the last step: after the sort, one pass gathers every pair's render parameters
 // into three tile-contiguous float4 "slab" arrays, so the compositing kernels stream each tile's
 // list with 1-D TMA bulk copies instead of chasing point_list[] indirections, and the backward
 // re-uses the same slabs.  The same pass detects tile boundaries (identifyTileRanges).
@@ -330,6 +330,8 @@ __global__ void __launch_bounds__(256, BIG ? 1 : 4) tile_sort_gather_kernel(cons
     }
 }
 
+constexpr int kBigTileCTAs = 132;   // one CTA per SM of an H100 for the few overlong tile lists
+
 int launch_tile_sort_gather(const Camera& cam, int P, uint32_t max_count, const GaussianSrc& colors, GeomState g,
                             BinningState b, ImageState im, cudaStream_t stream) {
     int id_bits = 1;
@@ -338,7 +340,7 @@ int launch_tile_sort_gather(const Camera& cam, int P, uint32_t max_count, const 
     tile_sort_gather_kernel<false><<<tiles, 256, 0, stream>>>(colors, g, b, im, id_bits);
     GPSG_LAUNCH_CHECK();
     if (max_count > kBigTile) {   // exact mode passes the real maximum; planned mode passes kMaxTileSort (always launch)
-        tile_sort_gather_kernel<true><<<min(tiles, 148), 256, 0, stream>>>(colors, g, b, im, id_bits);
+        tile_sort_gather_kernel<true><<<min(tiles, kBigTileCTAs), 256, 0, stream>>>(colors, g, b, im, id_bits);
         GPSG_LAUNCH_CHECK();
     }
     return GPSG_OK;

@@ -38,9 +38,9 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
     __shared__ uint32_t sh_cnt[kBoxBins];
     __shared__ int s_bb[4];
     __shared__ int s_last;
-    // (r2: staging the CTA's [256,3] position / scale triples through shared memory with 192 coalesced 128-bit loads was
-    //  measured SLOWER -- 29.1 vs 27.0 us at C2: the per-thread 12-byte-stride loads hit L1 for two of every three sectors
-    //  and the kernel is bound by its fp32 chain without FMA and the histogram, not by load instructions.  The quaternion,
+    // (Staging the CTA's [256,3] position / scale triples through shared memory with 192 coalesced 128-bit loads was tried
+    //  and was slower: the per-thread 12-byte-stride loads hit L1 for two of every three sectors and the kernel is bound by
+    //  its fp32 chain without FMA and the histogram, not by load instructions.  The quaternion,
     //  a natural 16-byte row, is loaded as one float4 in src_geom.)
     if (threadIdx.x == 0) { s_bb[0] = 0x7fffffff; s_bb[1] = 0x7fffffff; s_bb[2] = 0; s_bb[3] = 0; }
     for (int t = threadIdx.x; t < kBoxBins; t += blockDim.x) sh_cnt[t] = 0u;

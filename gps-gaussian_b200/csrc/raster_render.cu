@@ -1,67 +1,48 @@
 // raster_render.cu -- per-tile front-to-back alpha compositing (SURVEY.md Appendix A.4; upstream
 // forward.cu::renderCUDA, behind reference gaussian_renderer/__init__.py:54-62).
 //
-// B200 design (not upstream's):
+// Design (not upstream's):
 //  * a tile's sorted Gaussians are three contiguous float4 slabs (raster_binning.cu) streamed into a shared
 //    memory ring by a producer lane with 1-D TMA bulk copies (slab_ring.cuh); consumer warps never block on
 //    each other (no per-batch __syncthreads);
 //  * a CTA is half a tile (16x8 pixels, 4 consumer warps + 1 producer warp) -> 2x more, smaller work units for
-//    the 148 SMs; a warp covers an 8x4 pixel block;
+//    the 132 SMs of an H100; a warp covers an 8x4 pixel block;
 //  * warp-cooperative culling: for every 32 staged Gaussians each lane tests ONE Gaussian's conservative
 //    alpha>=1/255 bounding box against the warp's block; a ballot gives the survivors and only those are
 //    evaluated by the 32 pixels.  Skipped entries are exactly entries every lane would `continue` on, so the
 //    result is unchanged (n_contrib counts list positions, not evaluations);
 //  * the survivors of each 32-entry group are compacted (rank = popc of the ballot below the lane) into a per-warp
 //    shared-memory queue, so the evaluation loop walks fixed addresses, 8 survivors per unrolled iteration, instead of
-//    find-first-set + index arithmetic per survivor (38 -> 27 SASS instructions per survivor, XU pipe 42 % -> 17 %);
-//  * (r2) the queue is pair-interleaved and the conic polynomial / opacity product of TWO survivors of the same pixel run
-//    as packed fp32 (FADD2 / FMUL2 / FFMA2): 27 -> 21.5 SASS instructions per survivor, bit-identical images;
-//  * (r2) tiles are taken longest list first (tile_order from the tile scan): 122 -> 108 us at C2;
-//  * (r2, tried and NOT kept) a persistent grid (148 x 8 CTAs, atomic cursor over tile_order, ONE ring running across tiles
-//    with the producer lane prefetching the next tile's slabs, tile descriptors through a 2-slot mbarrier mailbox) rendered
-//    bit-identical images but was slower: 114.7 us without the saturation early-out, 118.9 us with an early-out + drain
-//    protocol, against 107.2 us for one CTA per half tile.  The start-up chain it removes (~7 % of the stall samples) is
-//    outweighed by what it adds: consumers of the next tile still wait behind the slowest warp of the current one through
-//    the shared ring, every tile costs two more barrier round trips, and the loop-carried state spills at 48 registers.
+//    find-first-set + index arithmetic per survivor (fewer instructions per survivor, less load on the XU pipe);
+//  * the queue is pair-interleaved (one LDS.128 lands the same field of two survivors) and the conic polynomial /
+//    opacity product of TWO survivors of the same pixel are evaluated side by side, so their loads and ex2 overlap;
+//  * tiles are taken longest list first (tile_order from the tile scan), so the longest lists do not start last;
+//  * (tried and NOT kept) a persistent grid (atomic cursor over tile_order, ONE ring running across tiles with the producer
+//    lane prefetching the next tile's slabs) rendered bit-identical images but was slower than one CTA per half tile:
+//    consumers of the next tile still wait behind the slowest warp of the current one through the shared ring, every tile
+//    costs two more barrier round trips, and the loop-carried state spills at 48 registers.
 //  * the conic arrives pre-scaled into the log2 domain, so alpha = o * ex2(p) with p a 5-op polynomial.
 #include "gpsg_internal.cuh"
 #include "slab_ring.cuh"
 
 namespace gpsg {
 
-// ---- packed fp32 (Blackwell `*.f32x2`, SASS FADD2 / FMUL2 / FFMA2): one issue slot does the same IEEE operation on two
-// independent values held in an aligned register pair.  Used across TWO SURVIVORS of the same pixel (their conic polynomials
-// are independent; only the transmittance blend is sequential), so the 8x4 cull block is unchanged -- the r1 attempt packed
-// two PIXELS per lane, which coarsened the culling and lost (profiles/microbench/README.md).
-__device__ __forceinline__ unsigned long long pk2(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void upk2(unsigned long long v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ unsigned long long mul2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
+// ---- two survivors of the same pixel evaluated side by side: their conic polynomials are independent (only the
+// transmittance blend is sequential), so both are computed as a pair of values with explicitly rounded IEEE operations in
+// the order the single-survivor formula uses.  `_rn` intrinsics keep nvcc from contracting a mul + add into an FMA, so
+// the result does not depend on how the compiler schedules the pair.
+struct f2p { float a, b; };
+__device__ __forceinline__ f2p pk2(float lo, float hi) { return {lo, hi}; }
+__device__ __forceinline__ void upk2(f2p v, float& lo, float& hi) { lo = v.a; hi = v.b; }
+__device__ __forceinline__ f2p sub2(f2p x, f2p y) { return {__fsub_rn(x.a, y.a), __fsub_rn(x.b, y.b)}; }
+__device__ __forceinline__ f2p mul2(f2p x, f2p y) { return {__fmul_rn(x.a, y.a), __fmul_rn(x.b, y.b)}; }
+__device__ __forceinline__ f2p fma2(f2p x, f2p y, f2p z) { return {__fmaf_rn(x.a, y.a, z.a), __fmaf_rn(x.b, y.b, z.b)}; }
 
 constexpr int kFwdChunk = 64;   // Gaussians per ring stage (3 x 1 KB)
 constexpr int kFwdStages = 6;   // 6 x 3 KB ring + 5.4 KB of survivor queues = 23.9 KB: still 9 CTAs / SM
 constexpr int kFwdWarps = 4;    // consumer warps per CTA: 16 x 8 pixels
 
-// 8 CTAs / SM (48 registers): measured best of {7, 8, 9} CTAs x {1, 2, 4}-pair unrolling (profiles/microbench/README.md)
+// 8 CTAs / SM (48 registers; 8 x 23.9 KB of shared memory also fits the 228 KB of an H100 SM)
 __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel(const __grid_constant__ Camera cam,
                                                                             const float4* __restrict__ slabA,
                                                                             const float4* __restrict__ slabB,
@@ -74,8 +55,8 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
     __shared__ SlabRing<kFwdChunk, kFwdStages> ring;
     // per consumer warp: queue of the (at most 32) entries of the current 32-entry group that survive the warp's cull,
     // + 1 pad slot.  Zero-initialised so that a pad / stale slot is always finite data with a defined (non-contributing) result.
-    // PACKED: pair-interleaved queue -- pair p = survivors (2p, 2p+1): QP[k][p] = (xA,xB,yA,yB), (bxA,bxB,byA,byB),
-    // (bzA,bzB,oA,oB), (rA,rB,gA,gB), (bA,bB,posA,posB): every LDS.128 lands two register pairs ready for f32x2 operands.
+    // Pair-interleaved queue -- pair p = survivors (2p, 2p+1): QP[k][p] = (xA,xB,yA,yB), (bxA,bxB,byA,byB),
+    // (bzA,bzB,oA,oB), (rA,rB,gA,gB), (bA,bB,posA,posB): every LDS.128 lands the same two fields of both survivors.
     __shared__ float4 qp[kFwdWarps][5][17];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -106,7 +87,7 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
     const float wx0 = (float)bx0, wx1 = (float)(bx0 + 7), wy0 = (float)by0, wy1 = (float)(by0 + 3);
 
     float4 (*__restrict__ QP)[17] = qp[warp];
-    const unsigned long long pixfx2 = pk2(pixfx, pixfx), pixfy2 = pk2(pixfy, pixfy);
+    const f2p pixfx2 = pk2(pixfx, pixfx), pixfy2 = pk2(pixfy, pixfy);
     const unsigned lt_mask = (1u << lane) - 1u;
 
     bool done = !inside;
@@ -157,10 +138,10 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
                     for (int i = 0; i < cnt; i += 2) {
                         const int pr = i >> 1;
                         const float4 v0 = QP[0][pr], v1 = QP[1][pr], v2 = QP[2][pr], v3 = QP[3][pr], v4 = QP[4][pr];
-                        const unsigned long long dx2 = sub2(pk2(v0.x, v0.y), pixfx2), dy2 = sub2(pk2(v0.z, v0.w), pixfy2);
+                        const f2p dx2 = sub2(pk2(v0.x, v0.y), pixfx2), dy2 = sub2(pk2(v0.z, v0.w), pixfy2);
                         // p = log2e * power = bz*dy*dy + (bx*dx + by*dy)*dx, same operation order as the scalar kernel
-                        const unsigned long long t2 = fma2(pk2(v1.x, v1.y), dx2, mul2(pk2(v1.z, v1.w), dy2));
-                        const unsigned long long p2 = fma2(mul2(pk2(v2.x, v2.y), dy2), dy2, mul2(t2, dx2));
+                        const f2p t2 = fma2(pk2(v1.x, v1.y), dx2, mul2(pk2(v1.z, v1.w), dy2));
+                        const f2p p2 = fma2(mul2(pk2(v2.x, v2.y), dy2), dy2, mul2(t2, dx2));
                         float pA, pB;
                         upk2(p2, pA, pB);
                         float aA, aB;

@@ -4,8 +4,8 @@
 // ring of shared-memory stages with 1-D TMA bulk copies; each stage has a `full` transaction barrier (armed by
 // the producer, completed by the TMA bytes) and an `empty` barrier (one arrival per consumer warp).  Consumer
 // warps therefore never synchronise with each other: a warp whose pixels reject most of a stage simply runs
-// ahead, up to kStages stages, instead of idling at a block barrier (ncu on the block-barrier version:
-// barrier stalls were the top stall reason, 8.9 warps per issued instruction).
+// ahead, up to kStages stages, instead of idling at a block barrier (in a block-barrier version barrier stalls were
+// the top stall reason).
 #pragma once
 #include "tma_bulk.cuh"
 
@@ -59,7 +59,7 @@ __device__ __forceinline__ void ring_produce(SlabRing<CHUNK, STAGES>& r, int nba
         if (b >= STAGES) {
             const uint32_t par = (uint32_t)(((b / STAGES) - 1) & 1);
             // hardware-suspended wait (<= 1 us per try); consumers that are all done stop arriving, so the flag is
-            // re-checked whenever a try times out.  (r1 polled with nanosleep(128): 3-7 M loop iterations per launch.)
+            // re-checked whenever a try times out.
             while (!mbar_try_wait_hint(&r.empty[s], par, 1000u)) {
                 if (*(volatile int*)&r.done_warps >= consumer_warps) { stop = true; break; }
             }

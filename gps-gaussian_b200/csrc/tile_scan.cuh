@@ -12,8 +12,8 @@ constexpr uint32_t kBigTile = 2048;
 
 // Also emits `tile_order`: all tile ids, longest list first (64 buckets of 32 pairs; order inside a bucket is arbitrary).
 // The compositing kernels take their tile from this list, so the long tiles start first and the short / empty ones fill
-// the tail of the grid (longest-processing-time-first: ~2.4 waves of very unequal half-tile CTAs otherwise leave the SMs
-// idle at the end -- ncu r1: issue slots busy 78 % of active cycles but 66 % of elapsed).
+// the tail of the grid (longest-processing-time-first: several waves of very unequal half-tile CTAs otherwise leave the SMs
+// idle at the end).
 __device__ __forceinline__ uint32_t order_bucket(uint32_t c) { return 63u - min(63u, (c + 31u) >> 5); }
 
 __device__ __forceinline__ void tile_scan_block(int tiles, const ImageState& im, uint32_t capacity) {

@@ -1,5 +1,5 @@
 // tma_bulk.cuh -- minimal inline-PTX wrappers for 1-D TMA bulk copies (cp.async.bulk, SASS: UBLKCP) and the
-// mbarrier transaction barrier they complete on (sm_90+/sm_100a).  No CUTLASS dependency.
+// mbarrier transaction barrier they complete on (sm_90+).  No CUTLASS dependency.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,8 +32,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Same, but the hardware may keep the thread suspended for up to `ns` nanoseconds while the phase is incomplete (it is woken
 // as soon as the phase completes).  A software poll loop (try_wait + nanosleep + flag check + branch, ~7 instructions per
-// iteration) in the slab producers cost 20 % (forward) / 26 % (backward) of ALL executed warp instructions of the two
-// issue-bound compositing kernels (ncu r2, profiles/r2_prof_*_summary.md); with the hint an iteration is rare.
+// iteration) in the slab producers made up a large share of ALL executed warp instructions of the two compositing kernels;
+// with the hint an iteration is rare.
 __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t ns) {
     uint32_t ok;
     asm volatile(

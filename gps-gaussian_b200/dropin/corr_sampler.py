@@ -1,4 +1,4 @@
-"""Drop-in `corr_sampler` for GPS-Gaussian, backed by libgpsg_sm100.so (sm_100a).
+"""Drop-in `corr_sampler` for GPS-Gaussian, backed by libgpsg_sm90.so (sm_90a).
 
 Put `gps-gaussian_b200/dropin` on PYTHONPATH and the UNMODIFIED reference imports this module at
 core/corr.py:5-8 instead of princeton-vl/RAFT-Stereo's `sampler` extension (SURVEY.md Appendix B).
@@ -23,14 +23,14 @@ _DT = {torch.float32: 0, torch.float16: 1}
 
 def _check(volume, coords):
     if not volume.is_cuda:
-        raise RuntimeError("corr_sampler (gpsg_sm100): volume must be a CUDA tensor")
+        raise RuntimeError("corr_sampler (gpsg): volume must be a CUDA tensor")
     if volume.dtype not in _DT:
-        raise RuntimeError(f"corr_sampler (gpsg_sm100): unsupported volume dtype {volume.dtype}")
+        raise RuntimeError(f"corr_sampler (gpsg): unsupported volume dtype {volume.dtype}")
     if volume.dim() != 4 or coords.dim() != 4:
-        raise RuntimeError("corr_sampler (gpsg_sm100): volume must be [B,H,W1,W2] and coords [B,C,H,W1]")
+        raise RuntimeError("corr_sampler (gpsg): volume must be [B,H,W1,W2] and coords [B,C,H,W1]")
     B, H, W1, _ = volume.shape
     if coords.shape[0] != B or coords.shape[2] != H or coords.shape[3] != W1:
-        raise RuntimeError("corr_sampler (gpsg_sm100): coords shape does not match volume")
+        raise RuntimeError("corr_sampler (gpsg): coords shape does not match volume")
 
 
 def _coords_x(coords):

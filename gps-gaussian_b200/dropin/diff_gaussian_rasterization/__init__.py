@@ -1,4 +1,4 @@
-"""Drop-in `diff_gaussian_rasterization` for GPS-Gaussian, backed by libgpsg_sm100.so (sm_100a).
+"""Drop-in `diff_gaussian_rasterization` for GPS-Gaussian, backed by libgpsg_sm90.so (sm_90a).
 
 Put `gps-gaussian_b200/dropin` on PYTHONPATH and the UNMODIFIED reference imports this module at
 gaussian_renderer/__init__.py:14 instead of the third-party extension
@@ -113,7 +113,7 @@ class _RasterizeGaussians(torch.autograd.Function):
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings):
         if not means3D.is_cuda:
-            raise RuntimeError("diff_gaussian_rasterization (gpsg_sm100): means3D must be a CUDA tensor")
+            raise RuntimeError("diff_gaussian_rasterization (gpsg): means3D must be a CUDA tensor")
         dev = means3D.device
         P = int(means3D.shape[0])
         H, W = int(raster_settings.image_height), int(raster_settings.image_width)
@@ -129,10 +129,10 @@ class _RasterizeGaussians(torch.autograd.Function):
         for name, t, k in (("opacities", op, 1), ("scales", sc, 3), ("rotations", ro, 4), ("colors_precomp", col, 3),
                            ("cov3D_precomp", cp, 6)):
             if t is not None and (t.numel() != k * P or t.device != dev):
-                raise RuntimeError(f"diff_gaussian_rasterization (gpsg_sm100): {name} must hold {P} x {k} values on {dev}, "
+                raise RuntimeError(f"diff_gaussian_rasterization (gpsg): {name} must hold {P} x {k} values on {dev}, "
                                    f"got shape {tuple(t.shape)} on {t.device}")
         if shs is not None and (shs.dim() != 3 or shs.shape[0] != P or shs.shape[2] != 3 or shs.device != dev):
-            raise RuntimeError(f"diff_gaussian_rasterization (gpsg_sm100): shs must be [{P}, M, 3] on {dev}")
+            raise RuntimeError(f"diff_gaussian_rasterization (gpsg): shs must be [{P}, M, 3] on {dev}")
         color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((P,), dtype=torch.int32, device=dev)
         num_rendered = C.c_int32(0)

@@ -1,5 +1,5 @@
 """Imported by Python at start-up when `gps-gaussian_b200/dropin` is on PYTHONPATH.  Does nothing unless GPSG_PATCH=1, in
-which case the reference's `core.corr.CorrBlockFast1D` / `lib.GaussianRender.pts2render` are rebound to the fused sm_100a
+which case the reference's `core.corr.CorrBlockFast1D` / `lib.GaussianRender.pts2render` are rebound to the fused sm_90a
 paths right after the reference imports those modules (see gps_gaussian_b200/patch.py and INTEGRATION.md)."""
 import os
 import sys

@@ -1,6 +1,6 @@
 """Mirror of reference gaussian_renderer/__init__.py:17-67 -- `render(data, idx, pts_xyz, pts_rgb,
 rotations, scales, opacity, bg_color)` with the same argument meaning and return value
-([3,H,W] image; radii dropped), wired to the sm_100a rasterizer.
+([3,H,W] image; radii dropped), wired to the sm_90a rasterizer.
 
 Differences that are invisible to the caller: the zero `screenspace_points` tensor is only created
 when a gradient is being recorded (it exists upstream solely so autograd can return a means2D

@@ -1,34 +1,30 @@
 """Run the UNMODIFIED reference scripts and model against the drop-ins (BASELINE config C3; VERDICT r1 item N1).
 
-The reference tree is staged once, byte for byte, into the git-ignored `baseline/_ref/` by `__graft_entry__.build()`
-(it travels to the GPU box with the snapshot like the built `.so`; it is never committed and nothing in the product
-imports it).  Everything here is harness: it builds the reference's own `RtStereoHumanModel`, feeds it the synthetic
+The original project's tree is staged, byte for byte, into the git-ignored `oracle/_ref/` by the oracle recipe
+(`oracle/build.py`, run by `__graft_entry__.build()` where a checkout of the original project exists); it is never
+committed and nothing in the product imports it.  Where nothing was staged the C3 tests skip and the bench block reports
+itself unavailable.  Everything here is harness: it builds the reference's own `RtStereoHumanModel`, feeds it the synthetic
 dataset through the reference's own `StereoHumanDataset`, and executes the optimisation step of
-/root/reference/train_stage2.py:57-89 -- with `gps-gaussian_b200/dropin` providing `diff_gaussian_rasterization`,
+the reference's train_stage2.py:57-89 -- with `gps-gaussian_b200/dropin` providing `diff_gaussian_rasterization`,
 `corr_sampler` and `yacs`.  Used by tests/test_c3_gpu.py and bench.py's `train_c3` block.
 """
 import os
 import shutil
+import stat
 import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 DROPIN = os.path.join(HERE, "dropin")
-REF_SRC = "/root/reference"
-REF_STAGED = os.path.join(ROOT, "baseline", "_ref")
+REF_STAGED = os.path.join(ROOT, "oracle", "_ref")           # staged by oracle/build.py
 
 
-def stage_reference(force=False):
-    """Copy /root/reference (read-only, only present in the build container) to baseline/_ref. Returns the staged path,
-    or None when neither the source nor an earlier staging exists."""
-    marker = os.path.join(REF_STAGED, "train_stage2.py")
-    if os.path.isdir(REF_SRC) and (force or not os.path.exists(marker)):
-        if os.path.isdir(REF_STAGED):
-            shutil.rmtree(REF_STAGED)
-        os.makedirs(os.path.dirname(REF_STAGED), exist_ok=True)
-        shutil.copytree(REF_SRC, REF_STAGED, ignore=shutil.ignore_patterns(".git", "__pycache__", "*.pyc"))
-    return REF_STAGED if os.path.exists(marker) else None
+def make_writable(root):
+    """Give the owner write permission on every directory and file under root."""
+    for d, _, files in os.walk(root):
+        for p in [d] + [os.path.join(d, f) for f in files]:
+            os.chmod(p, os.stat(p).st_mode | stat.S_IWUSR)
 
 
 def staged_reference():
@@ -39,7 +35,7 @@ def add_reference_to_path():
     """dropin first (so `diff_gaussian_rasterization`, `corr_sampler`, `yacs` resolve to ours), then the staged tree."""
     ref = staged_reference()
     if ref is None:
-        raise FileNotFoundError("baseline/_ref is not staged: run __graft_entry__.build() where /root/reference is mounted")
+        raise FileNotFoundError("oracle/_ref is not staged: run __graft_entry__.build() where the original project is checked out")
     for p in (ref, DROPIN, ROOT):
         if p in sys.path:
             sys.path.remove(p)
@@ -69,10 +65,11 @@ def make_workdir(path, data_root, **cfg):
     cwd and write experiments/ into it) with our config/stage2.yaml in place of the placeholder one."""
     ref = staged_reference()
     if ref is None:
-        raise FileNotFoundError("baseline/_ref is not staged")
+        raise FileNotFoundError("oracle/_ref is not staged")
     if os.path.isdir(path):
         shutil.rmtree(path)
     shutil.copytree(ref, path)
+    make_writable(path)                 # a read-only checkout keeps its modes through the copies
     with open(os.path.join(path, "config", "stage2.yaml"), "w") as f:
         f.write(stage2_yaml(data_root, **cfg))
     return path
@@ -88,9 +85,24 @@ def script_env(patch=False, extra=None):
     return env
 
 
+# Runs a script as __main__ (unmodified), then shuts down the DataLoader iterators it left alive before the interpreter
+# does.  train_stage2.py keeps iterators with pin-memory threads on its trainer object until exit; left to interpreter
+# finalization, such a daemon thread may be inside torch's C++ code when Python 3.12 ends it by a forced unwind, which aborts
+# the process ("terminate called without an active exception") after the script itself has finished.
+# `_shutdown_workers()` is what the iterator runs when it is released: it stops and joins the pin-memory thread and the
+# worker processes.
+SCRIPT_RUNNER = ("import gc, runpy, sys\n"
+                 "sys.argv = sys.argv[1:]\n"
+                 "runpy.run_path(sys.argv[0], run_name='__main__')\n"
+                 "from torch.utils.data.dataloader import _MultiProcessingDataLoaderIter\n"
+                 "for o in gc.get_objects():\n"
+                 "    if isinstance(o, _MultiProcessingDataLoaderIter):\n"
+                 "        o._shutdown_workers()\n")
+
+
 def run_script(workdir, script, args=(), patch=False, timeout=900):
-    """python <script> in the working copy with only dropin/ on PYTHONPATH. Returns CompletedProcess."""
-    return subprocess.run([sys.executable, script] + list(args), cwd=workdir, env=script_env(patch), text=True,
+    """python <script> in the working copy with only dropin/ on PYTHONPATH (through SCRIPT_RUNNER). Returns CompletedProcess."""
+    return subprocess.run([sys.executable, "-c", SCRIPT_RUNNER, script] + list(args), cwd=workdir, env=script_env(patch), text=True,
                           capture_output=True, timeout=timeout)
 
 

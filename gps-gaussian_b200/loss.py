@@ -1,4 +1,4 @@
-"""Mirror of the photometric part of reference lib/loss.py:35-72 and its use at train_stage2.py:70-72, on sm_100a.
+"""Mirror of the photometric part of reference lib/loss.py:35-72 and its use at train_stage2.py:70-72, on sm_90a.
 
 `l1_loss(network_output, gt)`, `ssim(img1, img2, window_size=11, size_average=True)` keep the reference signatures;
 `fused_l1_ssim(img, gt, w_l1=0.8, w_ssim=0.2)` is the whole expression `0.8*Ll1 + 0.2*(1 - ssim)` in one forward and one
@@ -23,9 +23,9 @@ def _dev(t):
 
 def _check_inputs(img, gt):
     if not (img.is_cuda and gt.is_cuda):
-        raise RuntimeError("gpsg_sm100 loss: CUDA tensors required (no CPU fallback)")
+        raise RuntimeError("gpsg loss: CUDA tensors required (no CPU fallback)")
     if img.shape != gt.shape or img.dim() < 2:
-        raise RuntimeError(f"gpsg_sm100 loss: shape mismatch {tuple(img.shape)} vs {tuple(gt.shape)}")
+        raise RuntimeError(f"gpsg loss: shape mismatch {tuple(img.shape)} vs {tuple(gt.shape)}")
 
 
 class _L1SSIM(torch.autograd.Function):
@@ -94,7 +94,7 @@ def l1_loss(network_output, gt):
 def ssim(img1, img2, window_size=11, size_average=True):
     """reference lib/loss.py:52-72 (the only window the reference ever uses is the default 11 / sigma 1.5)."""
     if window_size != 11:
-        raise NotImplementedError("gpsg_sm100 ssim: window_size is fixed to 11 (reference default, lib/loss.py:52)")
+        raise NotImplementedError("gpsg ssim: window_size is fixed to 11 (reference default, lib/loss.py:52)")
     if size_average:
         return 1.0 - _L1SSIM.apply(img1, img2, 0.0, 1.0)[0]
     if img1.dim() != 4:

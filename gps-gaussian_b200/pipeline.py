@@ -1,7 +1,7 @@
 """Host-buffer front end: render novel views whose Gaussians live in (pinned) HOST memory.
 
 The reference moves a sample to the GPU with blocking `.cuda()` copies and then renders (train_stage2.py:155-157,
-test_view_interp.py:55-59).  On a B200 the render itself takes ~0.3 ms while the 28 MB of per-view inputs take
+test_view_interp.py:55-59).  On an H100 the render itself takes ~0.3 ms while the 28 MB of per-view inputs take
 ~0.5 ms over PCIe, so the copies must overlap the compute: three CUDA streams (H2D, compute, D2H) and
 double-buffered device staging slots; the render is the unchanged reference-signature call
 `gaussian_renderer.render(data, idx, pts_xyz, pts_rgb, rotations, scales, opacity, bg_color)`.

@@ -37,7 +37,7 @@ def init(backend=None, device=None):
 def allreduce_grads(params, bucket=None):
     """Data-parallel gradient averaging for stage-2 training (BASELINE config C5): ONE flat fp32 bucket, SUM all-reduce,
     divide by the world size, written back in place -- issued between `scaler.scale(loss).backward()` and
-    `scaler.unscale_()` exactly where /root/reference/train_stage2.py:83-85 needs it (clip_grad_norm_ then sees the global
+    `scaler.unscale_()` exactly where the reference's train_stage2.py:83-85 needs it (clip_grad_norm_ then sees the global
     gradient and GradScaler's found-inf is identical on every rank).  5 144 408 fp32 values = 20.6 MB for the reference's
     stage-2 model.  Parameters without a gradient (the reference's unused 1/16 and 1/32 GRUs) are skipped on every rank
     alike.  `bucket`: optional reusable flat tensor.  Returns the flat bucket (averaged)."""

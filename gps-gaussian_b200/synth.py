@@ -12,7 +12,7 @@ shapes, value ranges and matrix conventions are the ones the real pipeline feeds
                                                      (reference lib/utils.py:87-109)
   * value ranges: unit quaternion, scale<=0.01, opacity in (0,1), rgb in [0,1]
                                                      (reference lib/gs_parm_network.py:72-78, lib/GaussianRender.py:30)
-Nothing here reads /root/reference.
+Nothing here reads the original project.
 """
 import math
 

@@ -1,5 +1,5 @@
 """Fused unprojection in front of the rasterizer -- mirror of reference lib/network.py:64-69 (`flow2gsparms`, first
-loop) built on lib/utils.py:87-119 (`flow2depth`, `depth2pc`): flow -> depth -> xyz + pts_valid in ONE sm_100a kernel
+loop) built on lib/utils.py:87-119 (`flow2depth`, `depth2pc`): flow -> depth -> xyz + pts_valid in ONE sm_90a kernel
 (and one for the backward), instead of ~12 elementwise / bmm torch kernels with repeat/cat copies."""
 import ctypes as C
 
@@ -12,13 +12,13 @@ class _Unproject(torch.autograd.Function):
     @staticmethod
     def forward(ctx, flow_pred, mask, intr, extr, ref_intr, tf_x):
         if not flow_pred.is_cuda:
-            raise RuntimeError("unproject (gpsg_sm100): flow_pred must be a CUDA tensor")
+            raise RuntimeError("unproject (gpsg): flow_pred must be a CUDA tensor")
         dev = flow_pred.device
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
         flow, m, K, E, Kr, tf = f32(flow_pred), f32(mask), f32(intr), f32(extr), f32(ref_intr), f32(tf_x).reshape(-1)
         B, _, S, S2 = flow.shape
         if S != S2 or m.shape[0] != B or m.shape[-1] != S or E.shape[-1] != 4 or E.shape[-2] < 3:
-            raise RuntimeError("unproject (gpsg_sm100): unexpected input shapes")
+            raise RuntimeError("unproject (gpsg): unexpected input shapes")
         depth = torch.empty((B, 1, S, S), dtype=torch.float32, device=dev)
         xyz = torch.empty((B, S * S, 3), dtype=torch.float32, device=dev)
         valid = torch.empty((B, S * S), dtype=torch.bool, device=dev)

@@ -1,5 +1,5 @@
 /*
- * gpsg.h -- C ABI of libgpsg_sm100.so: the B200 (sm_100a) splat rasterizer and 1-D stereo
+ * gpsg.h -- C ABI of libgpsg_sm90.so: the H100 (sm_90a) splat rasterizer and 1-D stereo
  * correlation sampler behind GPS-Gaussian's hot path.
  *
  * The reference has no native code of its own; its FFI for this path is the pybind surface of
@@ -201,7 +201,7 @@ GPSG_API int gpsg_corr_sampler_backward(int device, void* stream, int dtype, int
 /* ---- fused forms of the correlation block (reference core/corr.py:31-61), used by the mirrored CorrBlockFast1D ----
  * gpsg_corr_build_pyramid: fmap1[B,D,H,W1], fmap2[B,D,H,W2] (contiguous, dtype 0=fp32 1=fp16) ->
  *   vol[l][B,H,W1,W2>>l], l < levels<=4 : einsum/sqrt(D) then avg_pool2d([1,2]) per level, each level rounded to dtype.
- *   fp16 with D%16==0, D<=256, W1%8==0, W2%16==0, W2<=128 and 16-byte aligned pointers runs on tcgen05/TMEM (csrc/corr_tc.cu),
+ *   fp16 with D%16==0, D<=256, W1%8==0, W2%16==0, W2<=128 and 16-byte aligned pointers runs on the wgmma tensor-core kernel (csrc/corr_tc.cu),
  *   anything else on the FFMA kernel (csrc/corr.cu); same rounding chain, results agree to one fp16 ulp.  The environment
  *   variable GPSG_CORR_BUILD=ffma forces the FFMA kernels (tests compare the two).
  * gpsg_corr_lookup_pyramid_forward: all levels of CorrBlockFast1D.__call__ in one launch -> out[B, levels*(2r+1), H, W1]
@@ -249,7 +249,7 @@ GPSG_API int gpsg_l1_ssim_backward(int device, void* stream, int planes, int H, 
  * reset), calls[i] and the number of kernel launches[i]; it returns the number of stages (names via
  * gpsg_profile_stage_name) and resets the accumulators.  Process-wide (autograd runs backward nodes on its own thread).  on = 2 counts launches only (no events: nothing is
  * inserted into the streams, for timed regions that should only be counted). */
-/* fp16 correlation-volume build / backward: 0 = tcgen05 + TMEM kernels when the shape fits (default), 1 = FFMA kernels.
+/* fp16 correlation-volume build / backward: 0 = wgmma tensor-core kernels when the shape fits (default), 1 = FFMA kernels.
  * Process-wide switch for comparing the two formulations (tests, bench.py); GPSG_CORR_BUILD=ffma sets the initial value. */
 GPSG_API int gpsg_set_corr_build(int mode);
 GPSG_API int gpsg_profile_enable(int on);

@@ -8,7 +8,7 @@
  *     (princeton-vl/RAFT-Stereo sampler/sampler_kernel.cu, un-pinned, absent here) is restated
  *     from SURVEY.md Appendix B.
  * Pinned against the in-repo PyTorch twin `CorrBlock1D` (reference core/corr.py:110-156) imported
- * from /root/reference: golden vectors in tests/golden/corr_*.npz (generator: tests/golden/make_corr_golden.py).
+ * from the original project: golden vectors in tests/golden/corr_*.npz (generator: tests/golden/make_corr_golden.py).
  */
 #include <stdlib.h>
 #include <string.h>

@@ -6,7 +6,7 @@
  * gaussian_renderer/__init__.py:14,36-62; inputs assembled at
  * lib/GaussianRender.py:5-39).  The arithmetic itself lives in the un-vendored,
  * un-pinned third-party extension graphdeco-inria/diff-gaussian-rasterization
- * (pre-`antialiasing` API, ~commit 59f5f77) which is ABSENT from /root/reference
+ * (pre-`antialiasing` API, ~commit 59f5f77) which is ABSENT from the original project's tree
  * and from this image.  This file therefore restates the PUBLISHED algorithm as
  * specified in SURVEY.md Appendix A (A.2 preprocess, A.3 binning, A.4 render,
  * A.6 render-backward, A.7 cov2D-backward, A.8 preprocess-backward).
@@ -17,7 +17,7 @@
  *   autograd restatement (oracle/raster_torch64.py) -- see tests/test_oracle_*.py.
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
- * reference legs may load this library.  The product (libgpsg_sm100.so) never does.
+ * reference legs may load this library.  The product (libgpsg_sm90.so) never does.
  *
  * Built twice by oracle/build.py:
  *   -DREAL=float  -ffp-contract=off  -> liboracle_f32.so  (fp32, fixed op order:

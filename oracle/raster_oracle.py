@@ -5,7 +5,7 @@ cpu_baseline / `--impl reference` legs of bench.py may import this module.
 
 The oracle restates SURVEY.md Appendix A (the published algorithm of
 graphdeco-inria/diff-gaussian-rasterization, pre-antialiasing API, which the reference calls at
-gaussian_renderer/__init__.py:36-62 and which is absent from /root/reference).
+gaussian_renderer/__init__.py:36-62 and which is absent from the original project's tree).
 PARITY UNPINNED against the real extension -- see the header of gpsg_oracle.c.
 """
 import ctypes as C

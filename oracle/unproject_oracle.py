@@ -2,7 +2,7 @@
 
 Restates reference lib/utils.py:112-119 (flow2depth) and :87-109 (depth2pc) as used by lib/network.py:64-69.
 PINNED by tests/golden/unproject_golden.npz, which tests/golden/make_unproject_golden.py produced by calling the
-reference's own functions (imported from /root/reference in the build container), incl. autograd gradients."""
+reference's own functions (imported from a checkout of the original project), incl. autograd gradients."""
 import numpy as np
 
 

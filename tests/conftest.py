@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "gps-gaussian_b200", "dropin")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 box with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -22,7 +22,7 @@ def pytest_collection_modifyitems(config, items):
         has_cuda = False
     if has_cuda:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200); run with -m gpu on the GPU box")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100); run with -m gpu on the GPU box")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
@@ -30,7 +30,7 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def built_lib():
-    """Build (if stale) and return the path of libgpsg_sm100.so; nvcc cross-compiles without a GPU."""
+    """Build (if stale) and return the path of libgpsg_sm90.so; nvcc cross-compiles without a GPU."""
     import importlib.util
     spec = importlib.util.spec_from_file_location("_gpsg_build", os.path.join(ROOT, "gps-gaussian_b200", "build.py"))
     mod = importlib.util.module_from_spec(spec)

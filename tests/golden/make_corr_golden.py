@@ -1,6 +1,6 @@
 """Generate tests/golden/corr_golden.npz from the REFERENCE's own PyTorch correlation block.
 
-Run in the build container (needs /root/reference; the GPU box does not have it):
+Run with GPSG_REFERENCE naming a checkout of the original project:
     python tests/golden/make_corr_golden.py
 It imports `CorrBlock1D` from reference core/corr.py:110-156 -- the in-repo twin of the CUDA
 `CorrBlockFast1D`/`corr_sampler` path (README.md:34: same results) -- runs it on seeded inputs on the CPU in
@@ -12,7 +12,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["GPSG_REFERENCE"])
 from core.corr import CorrBlock1D  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))

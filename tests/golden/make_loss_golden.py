@@ -1,14 +1,14 @@
 """Generate tests/golden/loss_golden.npz from the REFERENCE's own lib/loss.py (l1_loss, ssim) and the combination of
 train_stage2.py:70-72, on the CPU in float64 and float32, with autograd gradients w.r.t. the rendered image.
 
-Run in the build container (needs /root/reference):  python tests/golden/make_loss_golden.py"""
+Run with GPSG_REFERENCE naming a checkout of the original project:  python tests/golden/make_loss_golden.py"""
 import os
 import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["GPSG_REFERENCE"])
 from lib.loss import gaussian, l1_loss, ssim  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))

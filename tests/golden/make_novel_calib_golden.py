@@ -1,6 +1,6 @@
 """Generate tests/golden/novel_calib_golden.npz from the REFERENCE's own get_novel_calib (lib/utils.py:8-54).
 
-Run in the build container (needs /root/reference + scipy):  python tests/golden/make_novel_calib_golden.py
+Run with GPSG_REFERENCE naming a checkout of the original project (+ scipy):  python tests/golden/make_novel_calib_golden.py
 The reference ends with five `.cuda()` copies; there is no GPU here, so `torch.Tensor.cuda` is shimmed to the identity
 for the duration of the call (the values are unaffected).  Cases: the benchmark's ring cameras (22.5 deg apart), random
 rotation pairs up to ~170 deg apart, perturbed intrinsics, `use_hr_img` on/off, non-zero trans / scale."""
@@ -11,7 +11,7 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["GPSG_REFERENCE"])
 from lib.utils import get_novel_calib  # noqa: E402
 from scipy.spatial.transform import Rotation as Rot  # noqa: E402
 

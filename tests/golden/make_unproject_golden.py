@@ -1,6 +1,6 @@
 """Generate tests/golden/unproject_golden.npz from the REFERENCE's own flow2depth / depth2pc.
 
-Run in the build container (needs /root/reference):  python tests/golden/make_unproject_golden.py
+Run with GPSG_REFERENCE naming a checkout of the original project:  python tests/golden/make_unproject_golden.py
 Imports lib/utils.py:87-119 and replays lib/network.py:64-69 (flow2gsparms) on seeded fp64 inputs on the CPU;
 stores inputs, depth, xyz, pts_valid and the autograd gradient d(loss)/d(flow_pred) for a random d(loss)/d(xyz)."""
 import os
@@ -9,7 +9,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["GPSG_REFERENCE"])
 from lib.utils import depth2pc, flow2depth  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))

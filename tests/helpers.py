@@ -18,8 +18,7 @@ tested value sits within rounding distance of its threshold.  `RasterOracle.marg
              is > 95 % of a C2 scene and agrees to ~1e-6.  Against the fp64 oracle the fp32 rounding of the projected
              means (6e-5 px at 1000-px coordinates => 1e-4 relative on alpha) must be inside eps, so eps_alpha = 1e-3 there
              and `clean` shrinks; the bound on each class is the same.
-The counts are appended to $GPSG_PARITY_LOG (json lines) when that variable is set; profiles/r2_parity_counts.jsonl is
-such a log from the B200.
+The counts are appended to $GPSG_PARITY_LOG (json lines) when that variable is set.
 """
 import json
 import os

@@ -25,15 +25,19 @@ def test_both_arms_print_the_same_config():
     assert a["views_per_step_per_gpu"] == 8 * 100 and "model" not in a
 
 
-def test_traffic_stamp_matches_code_not_comments():
+def test_traffic_stamp_matches_code_not_comments(tmp_path, monkeypatch):
     h = bench._source_hash("render_forward_kernel")
     assert re.fullmatch(r"[0-9a-f]{64}", h) and h != bench._source_hash("render_backward_q_kernel")
-    with open(os.path.join(ROOT, "profiles", "render_forward_traffic.json")) as f:
-        j = json.load(f)
-    for kernel in ("render_forward_kernel", "render_backward_q_kernel"):
-        val, src = bench._traffic(kernel)
-        if j[kernel]["source_sha256"] == bench._source_hash(kernel):
-            assert val == j[kernel]["dram_bytes_per_launch"] and 3e7 < val < 3e8         # tens of MB per launch at C2
-        else:                                                                             # kernel code changed since the capture:
-            assert val is None and src.startswith("stale")                                # refused, never silently reported
+    # a capture file with one entry stamped with the current code and one stamped with other code
+    j = {"render_forward_kernel": {"source_sha256": h, "dram_bytes_per_launch": 5.0e7},
+         "render_backward_q_kernel": {"source_sha256": "0" * 64, "dram_bytes_per_launch": 9.0e7}}
+    tf = tmp_path / "render_forward_traffic.json"
+    tf.write_text(json.dumps(j))
+    monkeypatch.setattr(bench, "TRAFFIC_FILE", str(tf))
+    val, src = bench._traffic("render_forward_kernel")
+    assert val == j["render_forward_kernel"]["dram_bytes_per_launch"]                  # stamp matches the code: reported
+    val, src = bench._traffic("render_backward_q_kernel")                               # kernel code changed since the capture:
+    assert val is None and src.startswith("stale")                                      # refused, never silently reported
     assert bench._traffic("no_such_kernel")[0] is None
+    monkeypatch.setattr(bench, "TRAFFIC_FILE", str(tmp_path / "absent.json"))
+    assert bench._traffic("render_forward_kernel")[0] is None                           # no capture: nothing reported

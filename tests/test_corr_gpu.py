@@ -1,4 +1,4 @@
-"""GPU parity of the sm_100a correlation sampler: golden vectors from the reference's CorrBlock1D,
+"""GPU parity of the sm_90a correlation sampler: golden vectors from the reference's CorrBlock1D,
 the CPU oracle at larger sizes, fp16 volumes (stage-2 AMP), edge cases.  Through the drop-in
 `corr_sampler` module (== C-ABI via ctypes)."""
 import os
@@ -174,7 +174,7 @@ def test_build_backward_kernel_vs_fp64_contractions(dtype, tol, shape):
 @pytest.mark.parametrize("shape", [(2, 192, 6, 128, 128), (1, 64, 3, 152, 48), (1, 32, 2, 264, 128), (1, 256, 2, 64, 64),
                                    (1, 16, 1, 8, 16)])
 def test_fp16_tcgen05_build_matches_ffma_kernel_and_oracle(shape):
-    """fp16 volumes take the tcgen05/TMEM kernel (corr_tc.cu); GPSG_CORR_BUILD=ffma forces the FFMA kernel.  Both follow the
+    """fp16 volumes take the wgmma kernel (corr_tc.cu); GPSG_CORR_BUILD=ffma forces the FFMA kernel.  Both follow the
     same rounding chain, so every pyramid level agrees to one fp16 ulp of the level's magnitude (different fp32 summation
     order), and both match the fp64 oracle on the quantised inputs.  Shapes: ragged M tiles (W1 = 152, 264), N < 128."""
     from gps_gaussian_b200.corr import CorrBlockFast1D
@@ -187,7 +187,7 @@ def test_fp16_tcgen05_build_matches_ffma_kernel_and_oracle(shape):
     try:
         ff = [v.clone() for v in CorrBlockFast1D(f1, f2, num_levels=4, radius=4).corr_pyramid]
     finally:
-        _lib.set_corr_build("tcgen05")
+        _lib.set_corr_build("wgmma")
     pyr = CorrOracle("f64").pyramid(f1.float().cpu().numpy(), f2.float().cpu().numpy(), 4)
     for l in range(4):
         a, b = tc[l].squeeze(3).float(), ff[l].squeeze(3).float()
@@ -213,7 +213,7 @@ def test_tcgen05_build_falls_back_for_unsupported_shapes():
 @pytest.mark.parametrize("shape", [(2, 192, 4, 128, 128), (1, 64, 2, 152, 48), (1, 32, 2, 264, 128), (1, 256, 1, 64, 64),
                                    (1, 16, 1, 8, 16), (1, 48, 3, 72, 112)])
 def test_fp16_tcgen05_build_backward_matches_ffma_kernel_and_fp64(shape):
-    """gpsg_corr_build_backward in fp16: tcgen05 kernels (K-major and MN-major g operand) vs the FFMA kernels
+    """gpsg_corr_build_backward in fp16: wgmma kernels (K-major and MN-major g operand) vs the FFMA kernels
     (GPSG_CORR_BUILD=ffma) vs fp64 contractions; ragged M tiles and K padded to 16 (W1 = 152, 264, 72, 8)."""
     import ctypes as C
     from gps_gaussian_b200 import _lib
@@ -237,7 +237,7 @@ def test_fp16_tcgen05_build_backward_matches_ffma_kernel_and_fp64(shape):
     try:
         ff = run()
     finally:
-        _lib.set_corr_build("tcgen05")
+        _lib.set_corr_build("wgmma")
     r1 = torch.einsum("bhxy,bdhy->bdhx", g.double(), f2.double()) / D ** 0.5
     r2 = torch.einsum("bhxy,bdhx->bdhy", g.double(), f1.double()) / D ** 0.5
     for a, b_, ref in ((tc[0], ff[0], r1), (tc[1], ff[1], r2)):

@@ -19,7 +19,7 @@ def test_library_exports_every_declared_symbol(built_lib):
         assert hasattr(lib, name), name
     from gps_gaussian_b200 import _lib
     assert set(_lib.EXPORTED) == declared
-    assert _lib.lib.gpsg_version() == 100
+    assert _lib.lib.gpsg_version() == 90
 
 
 def test_settings_struct_layout_matches_header(built_lib):

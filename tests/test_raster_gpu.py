@@ -1,4 +1,4 @@
-"""GPU parity tests of the sm_100a rasterizer against the CPU oracle (run with -m gpu on the B200).
+"""GPU parity tests of the sm_90a rasterizer against the CPU oracle (run with -m gpu on an H100).
 
 Bars (BASELINE.md section 2): tile indices (radii, tiles_touched, offsets, sorted keys + point list, ranges) bit-exact;
 RGB <= 1e-4 abs (except threshold-flip pixels, see test_oracle_cpu.test_f32_and_f64_oracles_agree);

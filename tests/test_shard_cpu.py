@@ -75,7 +75,9 @@ def _ddp_worker(rank, ws, port, out):
     params = list(m.parameters()) + list(unused.parameters())
     bucket = shard.allreduce_grads(params)
     gn = torch.nn.utils.clip_grad_norm_([p for p in params if p.grad is not None], 1e9)
-    out.put((rank, [p.grad.clone() / 1024.0 for p in m.parameters()], float(gn) / 1024.0, int(bucket.numel()),
+    # numpy arrays travel by value: a torch tensor on the queue is shared through a file descriptor, which is gone once
+    # this process has exited
+    out.put((rank, [(p.grad / 1024.0).numpy() for p in m.parameters()], float(gn) / 1024.0, int(bucket.numel()),
              all(p.grad is None for p in unused.parameters())))
     shard.finalize()
 
@@ -102,5 +104,5 @@ def test_allreduce_grads_world2_equals_single_process_batch2():
     for rank, grads, gn, nb, unused_none in res:
         assert nb == n_params and unused_none            # one flat bucket over exactly the parameters that have gradients
         for a, b in zip(grads, want):
-            assert torch.allclose(a, b, rtol=1e-5, atol=1e-7)
+            assert torch.allclose(torch.from_numpy(a), b, rtol=1e-5, atol=1e-7)
     assert abs(res[0][2] - res[1][2]) < 1e-9             # same global norm on both ranks => same clipping decision

@@ -1,5 +1,5 @@
 """Fused unprojection (reference lib/utils.py:87-119 via lib/network.py:64-69): oracle vs the reference's golden
-vectors on CPU; the sm_100a kernels vs golden + oracle on the GPU."""
+vectors on CPU; the sm_90a kernels vs golden + oracle on the GPU."""
 import os
 
 import numpy as np

@@ -10,7 +10,7 @@ so oracle/gpsg_oracle.c is "parity unpinned" (DESIGN.md section 2).  Run this sc
     cd RAFT-Stereo/sampler && python setup.py install
 
 succeeded -- with THIS repository's `gps-gaussian_b200/dropin` NOT on PYTHONPATH -- and commit the files it writes to
-tests/golden/.  tests/test_reference_vectors.py then pins (i) the CPU oracle and (ii) the sm_100a kernels to the real
+tests/golden/.  tests/test_reference_vectors.py then pins (i) the CPU oracle and (ii) the sm_90a kernels to the real
 extension's outputs: radii bit-exact, RGB <= 1e-4, gradients <= 1e-3 rel (BASELINE.json north_star), sampler <= 1e-6.
 
     python tools/dump_reference_vectors.py [--out tests/golden] [--device cuda:0]
