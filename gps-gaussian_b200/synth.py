@@ -175,10 +175,25 @@ def gather_valid(views):
     return {k: np.ascontiguousarray(np.concatenate(v, 0)) for k, v in out.items()}
 
 
+def _intrinsics(K, width, height, focal, principal):
+    """K with the focal lengths (fx, fy) and / or principal point (cx, cy) replaced where given; real captures have
+    fx != fy and non-square images (the reference reads both from the calibration, lib/human_loader.py:216-225)."""
+    K = K.copy()
+    if focal is not None:
+        K[0, 0], K[1, 1] = focal
+    if principal is not None:
+        K[0, 2], K[1, 2] = principal
+    elif (width, height) != (None, None):
+        K[0, 2], K[1, 2] = 0.5 * width, 0.5 * height
+    return K
+
+
 def stereo_pair_scene(src_res=1024, render_res=None, seed=SEED, ratio=0.5, body_radius=0.425, bg=(0.0, 0.0, 0.0),
-                      keep_maps=False):
+                      keep_maps=False, width=None, height=None, focal=None, principal=None):
     """BASELINE C2/C4 unit: two source views at +-11.25 deg -> ~P pixel-aligned Gaussians + the novel camera.
-    Returns the flat rasterizer inputs exactly as gaussian_renderer.render() receives them."""
+    Returns the flat rasterizer inputs exactly as gaussian_renderer.render() receives them.  `width` / `height` (default
+    `render_res`), `focal` = (fx, fy) and `principal` = (cx, cy) shape the novel camera only: the source maps stay
+    src_res x src_res.  A non-square image without `principal` puts the principal point at its centre."""
     render_res = render_res or src_res
     views = [source_view_maps(src_res, -11.25, seed * 2 + 0, body_radius),
              source_view_maps(src_res, +11.25, seed * 2 + 1, body_radius)]
@@ -186,30 +201,39 @@ def stereo_pair_scene(src_res=1024, render_res=None, seed=SEED, ratio=0.5, body_
     K0, K1 = views[0]["K"].copy(), views[1]["K"].copy()
     K0[:2] *= scale
     K1[:2] *= scale
-    cam = novel_camera(K0, views[0]["E"], K1, views[1]["E"], render_res, render_res, ratio)
+    W, H = width or render_res, height or render_res
+    K0, K1 = (_intrinsics(K, width, height, focal, principal) for K in (K0, K1))
+    cam = novel_camera(K0, views[0]["E"], K1, views[1]["E"], W, H, ratio)
     g = gather_valid(views)
     sc = dict(means3D=g["xyz"], colors=g["rgb"], opacity=g["opacity"], scales=g["scale"], rots=g["rot"],
               view=cam["world_view_transform"], proj=cam["full_proj_transform"], campos=cam["camera_center"],
-              tanfovx=math.tan(cam["FovX"] * 0.5), tanfovy=math.tan(cam["FovY"] * 0.5), W=render_res, H=render_res,
+              tanfovx=math.tan(cam["FovX"] * 0.5), tanfovy=math.tan(cam["FovY"] * 0.5), W=W, H=H,
               bg=np.asarray(bg, np.float32), cam=cam)
     if keep_maps:
         sc["views"] = views
     return sc
 
 
-def random_cube_scene(P=10_000, res=256, seed=SEED, bg=(0.0, 0.0, 0.0), spread=1.0, scale_mul=1.0):
-    """BASELINE C1: P Gaussians uniform in a `spread`-m cube centred on the look-at point, novel cam at angle 0."""
+def random_cube_scene(P=10_000, res=256, seed=SEED, bg=(0.0, 0.0, 0.0), spread=1.0, scale_mul=1.0, width=None, height=None,
+                      focal=None, principal=None, scale_modifier=1.0):
+    """BASELINE C1: P Gaussians uniform in a `spread`-m cube centred on the look-at point, novel cam at angle 0.
+    `width` / `height` (default `res`), `focal` = (fx, fy) and `principal` = (cx, cy) override the ring camera's image
+    and intrinsics (a non-square image without `principal` puts the principal point at its centre); `scale_modifier` is
+    passed to the rasterizer with the scene."""
     rng = np.random.default_rng(seed)
     K0, E0 = ring_camera(-11.25, res)
     K1, E1 = ring_camera(+11.25, res)
-    cam = novel_camera(K0, E0, K1, E1, res, res, 0.5)
+    W, H = width or res, height or res
+    K0, K1 = (_intrinsics(K, width, height, focal, principal) for K in (K0, K1))
+    cam = novel_camera(K0, E0, K1, E1, W, H, 0.5)
     xyz = (rng.uniform(-0.5, 0.5, (P, 3)) * spread + np.array([0.0, 0.85, 0.0])).astype(np.float32)
     zc = (np.concatenate([xyz, np.ones((P, 1), np.float32)], 1) @ cam["world_view_transform"])[:, 2]
     rot, scale, opacity, rgb = _attrs(rng, P, np.maximum(zc, 0.3) / np.float32(K0[0, 0]))
     scale = np.minimum(scale * np.float32(scale_mul), np.float32(0.01 * max(1.0, scale_mul)))
     return dict(means3D=xyz, colors=rgb, opacity=opacity, scales=scale, rots=rot, view=cam["world_view_transform"],
                 proj=cam["full_proj_transform"], campos=cam["camera_center"], tanfovx=math.tan(cam["FovX"] * 0.5),
-                tanfovy=math.tan(cam["FovY"] * 0.5), W=res, H=res, bg=np.asarray(bg, np.float32), cam=cam)
+                tanfovy=math.tan(cam["FovY"] * 0.5), W=W, H=H, bg=np.asarray(bg, np.float32), cam=cam,
+                scale_modifier=scale_modifier)
 
 
 def corr_inputs(B=2, D=192, H=64, W=64, seed=SEED, dtype=np.float32):

@@ -26,9 +26,20 @@ def _rotmat(q):
     return R.reshape(-1, 3, 3)
 
 
-def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0):
+def cov3d(scales, rots, scale_mod=1.0):
+    """Sigma3D = R diag(mod*s)^2 R^T as the 6 upper-triangle entries [P,6] (xx, xy, xz, yy, yz, zz)."""
+    R = _rotmat(rots)
+    N = R @ torch.diag_embed(scales * scale_mod)
+    S = N @ N.transpose(1, 2)
+    return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], -1)
+
+
+def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0, cov3D=None, denom_eps=0.0):
     """st: state dict of RasterOracle('f64').forward (supplies view/proj/camera + the discrete binning).
-    Tensor args: fp64 torch tensors (requires_grad as desired).  Returns image [3,H,W] fp64."""
+    Tensor args: fp64 torch tensors (requires_grad as desired).  `cov3D` [P,6] (see `cov3d`), when given, replaces the
+    scale/rotation covariance, as cov3D_precomp does; one symmetric off-diagonal entry stands for both Sigma_ab and Sigma_ba.
+    `denom_eps` > 0 scales the gradient through the conic by det^2 / (det^2 + denom_eps) without changing the image: the
+    regulariser of the hand-written backward's 1/(det^2 + 1e-7).  Returns image [3,H,W] fp64."""
     i = st["inputs"]
     W, H = st["W"], st["H"]
     dt = torch.float64
@@ -44,10 +55,9 @@ def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0):
     pw = 1.0 / (ph[:, 3] + float(np.float32(0.0000001)))
     ndc = ph[:, :2] * pw[:, None]
     pix = torch.stack([((ndc[:, 0] + 1.0) * W - 1.0) * 0.5, ((ndc[:, 1] + 1.0) * H - 1.0) * 0.5], 1)
-    R = _rotmat(rots)
-    S = torch.diag_embed(scales * scale_mod)
-    N = R @ S
-    Sigma = N @ N.transpose(1, 2)
+    c6 = cov3d(scales, rots, scale_mod) if cov3D is None else cov3D
+    Sigma = torch.stack([c6[:, 0], c6[:, 1], c6[:, 2], c6[:, 1], c6[:, 3], c6[:, 4], c6[:, 2], c6[:, 4], c6[:, 5]], -1)
+    Sigma = Sigma.reshape(-1, 3, 3)
     limx, limy = float(np.float32(1.3)) * tanx, float(np.float32(1.3)) * tany
     tz = t[:, 2]
     rx, ry = t[:, 0] / tz, t[:, 1] / tz
@@ -63,6 +73,10 @@ def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0):
     k03 = float(np.float32(0.3))
     a, b, c = cov[:, 0, 0] + k03, cov[:, 0, 1], cov[:, 1, 1] + k03
     det = a * c - b * b
+    if denom_eps:
+        k = (det * det / (det * det + denom_eps)).detach()
+        a, b, c = ((k * v + ((1 - k) * v).detach()) for v in (a, b, c))
+        det = a * c - b * b
     conx, cony, conz = c / det, -b / det, a / det
     op = opacity.reshape(-1)
 

@@ -43,6 +43,20 @@ def oracle_forward(sc, dtype="f32", nthreads=8, render=True):
                         nthreads=nthreads, render=render)
 
 
+def near_plane_scene(sc, seed=0):
+    """`sc` with its Gaussians moved to view-space depths on both sides of the z = 0.2 cull plane (some a relative 1e-7 or
+    less from it, some exactly on it), inside the field of view.  Returns (scene, view-space z in fp64)."""
+    rng = np.random.default_rng(seed)
+    P = sc["means3D"].shape[0]
+    d = np.concatenate([[0.0, 1e-8, -1e-8, 3e-8, -3e-8, 1e-7, -1e-7], rng.choice([-1, 1], P) * 10.0 ** rng.uniform(-7, 0, P)])
+    z = np.clip(0.2 + d[:P], 0.01, None)
+    E = sc["cam"]["E"]
+    xy = rng.uniform(-0.4, 0.4, (P, 2)) * np.array([sc["tanfovx"], sc["tanfovy"]]) * z[:, None]
+    X = ((np.concatenate([xy, z[:, None]], 1) - E[:, 3]) @ E[:, :3]).astype(np.float32)
+    z_view = X.astype(np.float64) @ E[2, :3] + E[2, 3]             # of the fp32-rounded positions
+    return dict(sc, means3D=X), z_view
+
+
 def rel_err(a, b):
     """max |a-b| / max|b|  (normalised max error; b is the reference)."""
     a = np.asarray(a, np.float64); b = np.asarray(b, np.float64)
@@ -106,7 +120,7 @@ def grad_err(got, want):
 
 
 GRAD_KEYS = (("dL_dmeans3D", "dL_dmeans3D"), ("dL_dcolors", "dL_dcolors"), ("dL_dopacity", "dL_dopacity"),
-             ("dL_dscales", "dL_dscales"), ("dL_drots", "dL_drots"), ("dL_dmeans2D", "dL_dmean2D"))
+             ("dL_dscales", "dL_dscales"), ("dL_drots", "dL_drots"), ("dL_dmeans2D", "dL_dmean2D"), ("dL_dcov3D", "dL_dcov3D"))
 
 
 def assert_grad_parity(tag, sc, got, base, final_T, n_contrib, g, dtypes=("f32", "f64"), keys=GRAD_KEYS):

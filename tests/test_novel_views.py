@@ -60,16 +60,19 @@ def test_synth_novel_camera_agrees_with_batched_calib():
         assert abs(a["FovX"] - float(b["FovX"][0, 0])) < 1e-6
 
 
-def _pair_data(res, seeds):
+def _pair_data(res, seeds, width=None, height=None, fy_scale=1.0):
+    """Source maps res x res; the novel view width x height (default res), fy of the source intrinsics scaled by fy_scale."""
     datas = []
     for seed in seeds:
         sc = synth.stereo_pair_scene(res, keep_maps=True, seed=seed)
-        d = {"novel_view": {"width": torch.tensor([res]), "height": torch.tensor([res])}}
+        d = {"novel_view": {"width": torch.tensor([width or res]), "height": torch.tensor([height or res])}}
         for name, vw in zip(("lmain", "rmain"), sc["views"]):
             T = lambda a: torch.tensor(a).cuda()[None]
+            K = vw["K"].copy()
+            K[1, 1] *= fy_scale
             d[name] = {"img": T(vw["img"]), "pts_valid": torch.tensor(vw["valid"]).cuda()[None], "xyz": T(vw["xyz"]),
                        "rot_maps": T(vw["rot_maps"]), "scale_maps": T(vw["scale_maps"]), "opacity_maps": T(vw["opacity_maps"]),
-                       "intr": torch.tensor(vw["K"], dtype=torch.float32).cuda()[None],
+                       "intr": torch.tensor(K, dtype=torch.float32).cuda()[None],
                        "extr": torch.tensor(vw["E"], dtype=torch.float32).cuda()[None]}
         datas.append(d)
     data = {"novel_view": {k: torch.cat([d["novel_view"][k] for d in datas]) for k in datas[0]["novel_view"]}}
@@ -79,17 +82,21 @@ def _pair_data(res, seeds):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("streams,mode", [(1, "compact"), (3, "compact"), (2, "maps")])
-def test_cached_novel_view_sweep_equals_per_ratio_calib_plus_pts2render(streams, mode):
-    """test_view_interp.py:39-47 restructured: one cache, all ratios, no gather / sync -- bit-identical to the loop."""
+@pytest.mark.parametrize("streams,mode,cam", [(1, "compact", {}), (3, "compact", {}), (2, "maps", {}),
+                                              (2, "compact", dict(width=160, height=96, fy_scale=1.15)),
+                                              (2, "maps", dict(width=96, height=160, fy_scale=0.85))],
+                         ids=["1-compact", "3-compact", "2-maps", "2-compact-160x96", "2-maps-96x160"])
+def test_cached_novel_view_sweep_equals_per_ratio_calib_plus_pts2render(streams, mode, cam):
+    """test_view_interp.py:39-47 restructured: one cache, all ratios, no gather / sync -- bit-identical to the loop.
+    Also with a non-square novel view and source intrinsics with fx != fy."""
     from gps_gaussian_b200.GaussianRender import pts2render
     from gps_gaussian_b200.novel_views import NovelViewRenderer
     res, ratios = 128, [0.1, 0.3, 0.5, 0.7, 0.9]
-    data = _pair_data(res, (21, 22))
+    data = _pair_data(res, (21, 22), **cam)
     opt = OPTS["plain"]
     bg = [0.05, 0.1, 0.2]
     sweep = NovelViewRenderer(data, opt, bg, streams=streams, mode=mode).render(ratios)
-    assert sweep.shape == (2, len(ratios), 3, res, res)
+    assert sweep.shape == (2, len(ratios), 3, cam.get("height", res), cam.get("width", res))
     for r, ratio in enumerate(ratios):
         d = novel_calib.get_novel_calib(data, opt, ratio=ratio)
         ref = pts2render(d, bg)["novel_view"]["img_pred"]

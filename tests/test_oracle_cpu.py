@@ -51,6 +51,46 @@ def test_single_isotropic_gaussian_closed_form():
         assert np.abs(st["color"][ch] - want).max() < 2e-4       # det-normalised conic vs exact var: ~1e-5
 
 
+def test_anisotropic_camera_matches_the_pinhole_model():
+    """External truth for a camera with fx != fy, W != H and an off-centre principal point, from its K and E alone (none of
+    the three restatements): means2D is the pinhole projection K [R|t] X minus the half pixel of ndc2pix, and inside the
+    1.3 tanfov guard band inverse(conic) - 0.3 I = J Sigma3D J^T, with J the central-difference Jacobian of that projection
+    and Sigma3D = R diag(scale_modifier * s)^2 R^T.  The guard band clamps t.x and t.y separately, so a Gaussian clamped
+    in x only keeps the exact yy entry and one clamped in y only the exact xx entry.  This pins focal_x / focal_y and the
+    two clamps without trusting the written-out Jacobian."""
+    from scipy.spatial.transform import Rotation
+    sc = synth.random_cube_scene(3000, 64, spread=3.0, scale_mul=8.0, width=120, height=48, focal=(70.0, 52.0),
+                                 principal=(66.0, 20.0), scale_modifier=1.3, seed=19)
+    _, st = oracle_forward(sc, "f64")
+    K, E = sc["cam"]["K"], sc["cam"]["E"]
+
+    def pinhole(X):
+        pc = X @ E[:, :3].T + E[:, 3]
+        return np.stack([K[0, 0] * pc[..., 0] / pc[..., 2] + K[0, 2], K[1, 1] * pc[..., 1] / pc[..., 2] + K[1, 2]], -1)
+
+    X = sc["means3D"].astype(np.float64)
+    vis = st["radii"] > 0
+    assert np.abs(st["means2D"][vis] - (pinhole(X[vis]) - 0.5)).max() < 1e-4          # fp32 rounding of view / proj
+    h = 1e-5
+    J = np.stack([(pinhole(X + h * e) - pinhole(X - h * e)) / (2 * h) for e in np.eye(3)], -1)          # [P,2,3]
+    q = sc["rots"].astype(np.float64)
+    R = Rotation.from_quat(q[:, [1, 2, 3, 0]]).as_matrix()                                             # (r,x,y,z) unit
+    s = sc["scales"].astype(np.float64) * sc["scale_modifier"]
+    cov2 = J @ (R * (s * s)[:, None, :]) @ np.swapaxes(R, 1, 2) @ np.swapaxes(J, 1, 2)
+    co = st["conic_opacity"][:, :3]
+    inv = np.linalg.inv(np.stack([co[:, 0], co[:, 1], co[:, 1], co[:, 2]], -1).reshape(-1, 2, 2)[vis]) - 0.3 * np.eye(2)
+    cov2 = cov2[vis]
+    err = np.abs(inv - cov2) / np.abs(cov2).max((1, 2))[:, None, None]
+    pc = X[vis] @ E[:, :3].T + E[:, 3]
+    over = [np.abs(pc[:, k] / pc[:, 2]) - np.float32(1.3) * sc[f"tanfov{a}"] for k, a in ((0, "x"), (1, "y"))]
+    inside_x, inside_y = over[0] < -1e-6, over[1] < -1e-6
+    only_x, only_y = (over[0] > 1e-6) & inside_y, (over[1] > 1e-6) & inside_x
+    assert only_x.sum() > 10 and only_y.sum() > 10 and (inside_x & inside_y).sum() > 1000
+    assert err[inside_x & inside_y].max() < 1e-5
+    assert err[only_x, 1, 1].max() < 1e-5 and err[only_y, 0, 0].max() < 1e-5
+    assert err[only_x, 0, 0].max() > 1e-2 and err[only_y, 1, 1].max() > 1e-2        # and the clamp does act
+
+
 def test_front_to_back_order_and_bg():
     sc, _ = _single_gaussian_scene(opacity=0.99)
     # second, farther Gaussian of another colour exactly behind the first
@@ -67,22 +107,59 @@ def test_front_to_back_order_and_bg():
     assert c[0] > 0.9 and c[1] < 0.08                            # near (red) dominates
 
 
-@pytest.mark.parametrize("res,P,spread,mul", [(64, 600, 0.45, 3.0), (48, 300, 0.3, 6.0)])
-def test_backward_matches_fp64_autograd(res, P, spread, mul):
-    from oracle.raster_torch64 import render_autograd
-    sc = synth.random_cube_scene(P, res, spread=spread, scale_mul=mul, bg=(0.2, 0.5, 0.7), seed=7)
+# anisotropic, non-square, off-centre cameras (fx != fy, W != H) and scale_modifier != 1
+ANISO = dict(wide=dict(width=96, height=40, focal=(80.0, 60.0), principal=(50.0, 17.0)),
+             tall=dict(width=40, height=100, focal=(50.0, 70.0), principal=(18.0, 55.0), scale_modifier=1.7),
+             small=dict(width=72, height=56, focal=(64.0, 64.0), principal=(30.0, 30.0), scale_modifier=0.6))
+
+
+@pytest.mark.parametrize("res,P,spread,mul,kw,precomp", [
+    pytest.param(64, 600, 0.45, 3.0, {}, False, id="64-600-0.45-3.0"),
+    pytest.param(64, 600, 0.45, 3.0, {}, True, id="64-600-0.45-3.0-precomp"),
+    pytest.param(48, 300, 0.3, 6.0, {}, False, id="48-300-0.3-6.0"),
+    pytest.param(48, 300, 0.3, 6.0, {}, True, id="48-300-0.3-6.0-precomp"),
+    pytest.param(64, 600, 0.6, 2.0, ANISO["wide"], False, id="wide"),
+    pytest.param(64, 600, 0.6, 2.0, ANISO["wide"], True, id="wide-precomp"),
+    pytest.param(64, 600, 0.6, 2.0, ANISO["tall"], False, id="tall"),
+    pytest.param(64, 600, 0.6, 2.0, ANISO["tall"], True, id="tall-precomp"),
+    pytest.param(64, 600, 0.6, 2.0, ANISO["small"], False, id="small"),
+    pytest.param(64, 600, 0.6, 2.0, ANISO["small"], True, id="small-precomp"),
+])
+def test_backward_matches_fp64_autograd(res, P, spread, mul, kw, precomp):
+    """The hand-written backward against fp64 autograd, incl. dL_dcov3D: on the scale/rotation path (Sigma3D an
+    intermediate of the autograd graph) and on the cov3D_precomp path (Sigma3D a leaf, no scale/rotation chain)."""
+    from oracle.raster_torch64 import cov3d, render_autograd
+    sc = synth.random_cube_scene(P, res, spread=spread, scale_mul=mul, bg=(0.2, 0.5, 0.7), seed=7, **kw)
+    mod = sc["scale_modifier"]
     o, st = oracle_forward(sc, "f64")
-    T = lambda a: torch.tensor(np.asarray(a, np.float64), requires_grad=True)
-    m, c, op, s, r = T(sc["means3D"]), T(sc["colors"]), T(sc["opacity"]), T(sc["scales"]), T(sc["rots"])
-    img = render_autograd(st, m, c, op, s, r)
-    assert np.abs(img.detach().numpy() - st["color"]).max() < 1e-12
+    cov3D = st["cov3D"].copy()
+    if precomp:
+        o, pre = oracle_forward(dict(sc, cov3D_precomp=cov3D, scales=None, rots=None), "f64")
+        assert np.array_equal(pre["radii"], st["radii"])
+        st = pre
     g = np.random.default_rng(0).standard_normal(st["color"].shape)
-    (img * torch.tensor(g)).sum().backward()
     gr = o.backward(st, g)
-    for name, a, b in (("means3D", m.grad, gr["dL_dmeans3D"]), ("colors", c.grad, gr["dL_dcolors"]),
-                       ("opacity", op.grad.reshape(-1), gr["dL_dopacity"]), ("scales", s.grad, gr["dL_dscales"]),
-                       ("rots", r.grad, gr["dL_drots"])):
-        assert rel_err(b, a.numpy()) < 1e-6, name                 # 1e-7 eps in 1/(denom^2+1e-7) is the floor
+    for denom_eps in (0.0, 1e-7):
+        T = lambda a: torch.tensor(np.asarray(a, np.float64), requires_grad=True)
+        m, c, op, s, r = T(sc["means3D"]), T(sc["colors"]), T(sc["opacity"]), T(sc["scales"]), T(sc["rots"])
+        if precomp:
+            cov = T(cov3D)
+        else:
+            cov = cov3d(s, r, mod)
+            cov.retain_grad()
+        img = render_autograd(st, m, c, op, s, r, scale_mod=mod, cov3D=cov, denom_eps=denom_eps)
+        assert np.abs(img.detach().numpy() - st["color"]).max() < 1e-12
+        (img * torch.tensor(g)).sum().backward()
+        checks = [("means3D", m.grad, gr["dL_dmeans3D"]), ("colors", c.grad, gr["dL_dcolors"]),
+                  ("opacity", op.grad.reshape(-1), gr["dL_dopacity"]), ("cov3D", cov.grad, gr["dL_dcov3D"])]
+        if not precomp:
+            checks += [("scales", s.grad, gr["dL_dscales"]), ("rots", r.grad, gr["dL_drots"])]
+        # The true derivative (denom_eps = 0) differs from the backward's 1/(denom^2 + 1e-7) by a relative 1e-7/denom^2,
+        # which grows as splats shrink: 1.7e-6 at scale_modifier 0.6.  With the same regulariser in the autograd graph the
+        # two agree to 1e-12 in every case, so the regulariser is the whole difference.
+        tol = 1e-12 if denom_eps else (3e-6 if mod < 1 else 1e-6)
+        for name, a, b in checks:
+            assert rel_err(b, a.numpy()) < tol, (name, denom_eps)
 
 
 def test_backward_matches_fp64_autograd_with_independent_binning():
@@ -144,7 +221,11 @@ def test_threshold_margins_explain_every_f32_f64_compositing_difference():
 
 
 @pytest.mark.parametrize("P,res,kw", [(3000, 128, dict(seed=3)), (4000, 250, dict(spread=0.6, scale_mul=4.0, bg=(0.3, 0.6, 0.9), seed=11)),
-                                      (2000, 130, dict(spread=3.0, seed=11)), (10_000, 256, dict())])
+                                      (2000, 130, dict(spread=3.0, seed=11)), (10_000, 256, dict()),
+                                      (2500, 64, dict(spread=0.6, scale_mul=2.0, seed=3, **ANISO["wide"])),
+                                      (2500, 64, dict(spread=0.6, scale_mul=2.0, seed=3, **ANISO["tall"])),
+                                      (3000, 64, dict(spread=3.0, scale_mul=8.0, seed=19, width=120, height=48,
+                                                      focal=(70.0, 52.0), principal=(66.0, 20.0), scale_modifier=1.3))])
 def test_independent_numpy_restatement_agrees_with_the_c_oracle(P, res, kw):
     """oracle/raster_independent.py takes only the raw call arguments (no state of gpsg_oracle.c): culling, radii, tile
     counts, the sorted 64-bit keys, point list and tile ranges must be IDENTICAL to the C oracle's fp64 build, the image,
@@ -181,20 +262,30 @@ def test_non_finite_inputs_are_culled_in_both_restatements():
 
 def test_independent_restatement_randomised_sweep():
     """Seeded sweep over image size, point count, spread, splat size, background: the two restatements (C, scalar chains;
-    numpy, matrix form + global argsort) must agree on every integer output and on the image to 1e-11."""
+    numpy, matrix form + global argsort) must agree on every integer output and on the image to 1e-11.  Every scene is
+    also rendered through a second camera with width and height drawn independently (one 12 px wide: a single tile
+    column; one 9 px tall), fx != fy, an off-centre principal point and a scale_modifier != 1."""
     from oracle import raster_independent as ri
     rng = np.random.default_rng(77)
+    cam_rng = np.random.default_rng(78)
+    sizes = [(12, 180), (230, 9)] + [tuple(int(v) for v in cam_rng.integers(8, 300, 2)) for _ in range(8)]   # grid_x == 1, H < 16
     for k in range(10):
         res = int(rng.integers(24, 220))
         P = int(rng.integers(1, 2500))
-        sc = synth.random_cube_scene(P, res, spread=float(rng.uniform(0.2, 2.5)), scale_mul=float(rng.uniform(0.5, 8.0)),
-                                     bg=tuple(rng.uniform(0, 1, 3)), seed=int(rng.integers(1 << 30)))
-        _, a = oracle_forward(sc, "f64")
-        b = ri.forward_scene(sc)
-        assert np.array_equal(a["radii"], b["radii"]) and np.array_equal(a["tiles_touched"], b["tiles_touched"]), k
-        assert np.array_equal(a["keys"], b["keys"]) and np.array_equal(a["vals"], b["point_list"]), k
-        assert np.array_equal(a["ranges"], b["ranges"]) and np.array_equal(a["n_contrib"], b["n_contrib"]), k
-        assert np.abs(a["color"] - b["color"]).max() < 1e-11 and np.abs(a["final_T"] - b["final_T"]).max() < 1e-11, k
+        kw = dict(spread=float(rng.uniform(0.2, 2.5)), scale_mul=float(rng.uniform(0.5, 8.0)), bg=tuple(rng.uniform(0, 1, 3)),
+                  seed=int(rng.integers(1 << 30)))
+        W, H = sizes[k]
+        fx = 0.8 * math.sqrt(W * H) * cam_rng.uniform(0.7, 1.4)
+        aniso = dict(width=W, height=H, focal=(fx, fx * cam_rng.uniform(0.6, 1.6)),
+                     principal=(W * cam_rng.uniform(0.3, 0.7), H * cam_rng.uniform(0.3, 0.7)),
+                     scale_modifier=cam_rng.uniform(0.5, 2.0))
+        for sc in (synth.random_cube_scene(P, res, **kw), synth.random_cube_scene(P, res, **kw, **aniso)):
+            _, a = oracle_forward(sc, "f64")
+            b = ri.forward_scene(sc)
+            assert np.array_equal(a["radii"], b["radii"]) and np.array_equal(a["tiles_touched"], b["tiles_touched"]), k
+            assert np.array_equal(a["keys"], b["keys"]) and np.array_equal(a["vals"], b["point_list"]), k
+            assert np.array_equal(a["ranges"], b["ranges"]) and np.array_equal(a["n_contrib"], b["n_contrib"]), k
+            assert np.abs(a["color"] - b["color"]).max() < 1e-11 and np.abs(a["final_T"] - b["final_T"]).max() < 1e-11, k
 
 
 def test_binning_invariants():
@@ -224,6 +315,20 @@ def test_empty_and_culled():
     assert np.allclose(st["color"], sc["bg"][:, None, None]) and np.all(st["final_T"] == 1)
     o = RasterOracle("f32")
     assert not o.mark_visible(sc["means3D"], sc["view"]).any()
+
+
+def test_mark_visible_at_the_near_plane():
+    """mark_visible is the preprocess's z > 0.2 cull: points on both sides of view-space z = 0.2 (further than fp32 rounding
+    from it) get the expected mask in both precisions, and no Gaussian it marks absent is rendered."""
+    from helpers import near_plane_scene
+    sc, z = near_plane_scene(synth.random_cube_scene(2000, 64, seed=5, **ANISO["wide"]))
+    far = np.abs(z - 0.2) > 1e-5
+    assert (far & (z > 0.2)).sum() > 500 and (far & (z < 0.2)).sum() > 500
+    for dt in ("f32", "f64"):
+        present = RasterOracle(dt).mark_visible(sc["means3D"], sc["view"])
+        assert np.array_equal(present[far], z[far] > 0.2), dt
+        _, st = oracle_forward(sc, dt, render=False)
+        assert (st["radii"] > 0).sum() > 500 and not (st["radii"] > 0)[~present].any(), dt
 
 
 def test_taichi_splat_restatement():

@@ -18,6 +18,10 @@ from helpers import (GRAD_TOL, RGB_TOL, assert_grad_parity, assert_image_parity,
 
 pytestmark = pytest.mark.gpu
 
+# non-square images with fx != fy and an off-centre principal point (synth.random_cube_scene keywords)
+WIDE = dict(width=250, height=40, focal=(240.0, 190.0), principal=(118.0, 23.0))
+TALL = dict(width=40, height=250, focal=(150.0, 260.0), principal=(21.0, 130.0))
+
 
 def _run(sc):
     from gps_gaussian_b200.introspect import RasterCall
@@ -65,15 +69,24 @@ def test_c1_forward_parity():
     _assert_forward_parity(synth.random_cube_scene(10_000, 256), tag="C1")
 
 
-@pytest.mark.parametrize("res,P,spread,mul,bg", [
-    (250, 4000, 0.6, 4.0, (0.3, 0.6, 0.9)),      # image not a multiple of 16, coloured bg, fat splats
-    (64, 300, 0.3, 12.0, (1.0, 1.0, 1.0)),       # splats covering many tiles; saturating pixels (T<1e-4 stop)
-    (130, 2000, 3.0, 1.0, (0.0, 0.0, 0.0)),      # wide cloud: many off-screen / frustum-clamped Gaussians
-    (64, 4500, 0.35, 1.5, (0.0, 0.0, 0.0)),      # 2-3.4k pairs per tile: the 16-keys-per-thread in-CTA sort variant
-    (48, 30000, 0.25, 1.0, (0.0, 0.0, 0.0)),     # > 4096 pairs in a tile: automatic fallback to the global radix path
-])
-def test_forward_parity_edge_shapes(res, P, spread, mul, bg):
-    sc = synth.random_cube_scene(P, res, spread=spread, scale_mul=mul, bg=bg, seed=11)
+@pytest.mark.parametrize("res,P,spread,mul,bg,cam", [
+    (250, 4000, 0.6, 4.0, (0.3, 0.6, 0.9), {}),  # image not a multiple of 16, coloured bg, fat splats
+    (64, 300, 0.3, 12.0, (1.0, 1.0, 1.0), {}),   # splats covering many tiles; saturating pixels (T<1e-4 stop)
+    (130, 2000, 3.0, 1.0, (0.0, 0.0, 0.0), {}),  # wide cloud: many off-screen / frustum-clamped Gaussians
+    (64, 4500, 0.35, 1.5, (0.0, 0.0, 0.0), {}),  # 2-3.4k pairs per tile: the 16-keys-per-thread in-CTA sort variant
+    (48, 30000, 0.25, 1.0, (0.0, 0.0, 0.0), {}), # > 4096 pairs in a tile: automatic fallback to the global radix path
+    # non-square, fx != fy, off-centre principal point: the two image axes enter every stage separately
+    (64, 3000, 0.6, 4.0, (0.3, 0.6, 0.9), dict(WIDE, scale_modifier=0.7)),   # ragged in both axes, splats shrunk
+    (64, 3000, 0.6, 4.0, (0.0, 0.0, 0.0), dict(TALL, scale_modifier=1.6)),   # ~2.5k pairs in a tile, splats grown
+    (64, 2000, 0.6, 2.0, (0.2, 0.2, 0.2), dict(width=16, height=300, focal=(60.0, 300.0), principal=(8.0, 140.0))),  # grid_x == 1
+    (64, 2000, 0.6, 2.0, (0.0, 0.0, 0.0), dict(width=300, height=8, focal=(300.0, 50.0), principal=(150.0, 4.5))),   # H < 16
+    (64, 30000, 0.25, 1.0, (0.0, 0.0, 0.0), dict(width=64, height=40, focal=(45.0, 38.0), principal=(30.0, 21.0))),  # > 4096 in a tile
+    (64, 3000, 3.0, 5.0, (0.0, 0.0, 0.0), dict(width=120, height=48, focal=(70.0, 52.0), principal=(66.0, 20.0),
+                                               scale_modifier=1.3)),          # frustum-clamped in x only and in y only
+], ids=["250-4000-0.6-4.0-bg0", "64-300-0.3-12.0-bg1", "130-2000-3.0-1.0-bg2", "64-4500-0.35-1.5-bg3", "48-30000-0.25-1.0-bg4",
+        "250x40-mod0.7", "40x250-mod1.6", "16x300", "300x8", "64x40-30000", "120x48-clamp-mod1.3"])
+def test_forward_parity_edge_shapes(res, P, spread, mul, bg, cam):
+    sc = synth.random_cube_scene(P, res, spread=spread, scale_mul=mul, bg=bg, seed=11, **cam)
     _assert_forward_parity(sc)
 
 
@@ -94,7 +107,9 @@ def test_empty_inputs_and_all_culled():
     assert all(float(v.abs().sum()) == 0 for v in g.values() if v is not None)
 
 
-@pytest.mark.parametrize("P,res,kw", [(10_000, 256, dict()), (4000, 250, dict(spread=0.6, scale_mul=4.0, bg=(0.3, 0.6, 0.9), seed=11))])
+@pytest.mark.parametrize("P,res,kw", [(10_000, 256, dict()), (4000, 250, dict(spread=0.6, scale_mul=4.0, bg=(0.3, 0.6, 0.9), seed=11)),
+                                      (3000, 64, dict(spread=0.6, scale_mul=4.0, bg=(0.3, 0.6, 0.9), seed=11, scale_modifier=0.7,
+                                                      **WIDE))])
 def test_device_against_the_independent_numpy_restatement(P, res, kw):
     """The device vs oracle/raster_independent.py (fp64, raw inputs only, no state shared with gpsg_oracle.c).  fp32 vs
     fp64 projection can round a radius / tile rectangle differently, so the comparison is made on the tiles whose lists
@@ -164,15 +179,15 @@ def test_non_finite_inputs_are_culled_not_crashed():
 
 
 def test_cov3d_precomp_path_matches_scale_rot_path():
+    """cov3D_precomp instead of scales / rotations: the same radii as the scale / rotation path, and full forward and
+    backward parity (dL_dcov3D included; no scale / rotation chain, so dL_dscales and dL_drots are zero)."""
     sc = synth.random_cube_scene(3000, 128, seed=5)
     _, ref = oracle_forward(sc, "f32")
-    pre = dict(sc)
-    pre["cov3D_precomp"] = ref["cov3D"].copy()
     # visible Gaussians carry their cov3D; culled ones have zeros there but are culled again anyway
-    pre["scales"] = None; pre["rots"] = None
-    rc = _run(pre)
+    pre = dict(sc, cov3D_precomp=ref["cov3D"].copy(), scales=None, rots=None)
+    rc, _ = _assert_forward_parity(pre, tag="cov3D_precomp")
     assert np.array_equal(_np(rc.radii), ref["radii"])
-    assert np.abs(_np(rc.color) - ref["color"]).max() < 1e-2
+    _assert_backward_parity(pre, seed=1, tag="cov3D_precomp", rc=rc)
 
 
 def test_idempotent_and_deterministic_forward():
@@ -194,7 +209,7 @@ def _assert_backward_parity(sc, seed=0, tag=None, rc=None, ref=None):
     P = sc["means3D"].shape[0]
     assert np.array_equal(_np(st["point_list"]).view(np.uint32), ref["vals"])     # same tile lists => forced replay is exact
     g = np.random.default_rng(seed).standard_normal((3, sc["H"], sc["W"])).astype(np.float32)
-    got = rc.backward(torch.from_numpy(g).cuda(), want_cov3D=False)
+    got = rc.backward(torch.from_numpy(g).cuda(), want_cov3D=True)
     torch.cuda.synchronize()
     assert float(got["dL_dmeans2D"][:, 2].abs().sum()) == 0
     return assert_grad_parity(tag or f"{sc['W']}x{sc['H']}_P{P}", sc, {k: _np(v) for k, v in got.items() if v is not None}, ref,
@@ -205,12 +220,17 @@ def test_c1_backward_parity():
     _assert_backward_parity(synth.random_cube_scene(10_000, 256), tag="C1")
 
 
-@pytest.mark.parametrize("res,P,spread,mul,bg", [
-    (100, 1500, 0.5, 4.0, (0.3, 0.6, 0.9)),      # coloured background term of dL/dalpha, ragged image
-    (64, 300, 0.3, 10.0, (0.0, 0.0, 0.0)),       # heavy overlap, saturated pixels
-])
-def test_backward_parity_edge_shapes(res, P, spread, mul, bg):
-    _assert_backward_parity(synth.random_cube_scene(P, res, spread=spread, scale_mul=mul, bg=bg, seed=13), seed=3)
+@pytest.mark.parametrize("res,P,spread,mul,bg,cam", [
+    (100, 1500, 0.5, 4.0, (0.3, 0.6, 0.9), {}),  # coloured background term of dL/dalpha, ragged image
+    (64, 300, 0.3, 10.0, (0.0, 0.0, 0.0), {}),   # heavy overlap, saturated pixels
+    (64, 1500, 0.6, 4.0, (0.3, 0.6, 0.9), dict(WIDE, scale_modifier=0.7)),   # non-square, fx != fy, splats shrunk
+    (64, 1500, 0.6, 4.0, (0.0, 0.0, 0.0), dict(TALL, scale_modifier=1.6)),   # the transpose, splats grown
+    (64, 1000, 0.6, 2.0, (0.2, 0.2, 0.2), dict(width=300, height=8, focal=(300.0, 50.0), principal=(150.0, 4.5))),   # H < 16
+    (64, 3000, 3.0, 5.0, (0.0, 0.0, 0.0), dict(width=120, height=48, focal=(70.0, 52.0), principal=(66.0, 20.0),
+                                               scale_modifier=1.3)),          # frustum-clamped in x only and in y only
+], ids=["100-1500-0.5-4.0-bg0", "64-300-0.3-10.0-bg1", "250x40-mod0.7", "40x250-mod1.6", "300x8", "120x48-clamp-mod1.3"])
+def test_backward_parity_edge_shapes(res, P, spread, mul, bg, cam):
+    _assert_backward_parity(synth.random_cube_scene(P, res, spread=spread, scale_mul=mul, bg=bg, seed=13, **cam), seed=3)
 
 
 def test_backward_is_linear_in_grad_out():
@@ -228,37 +248,61 @@ def test_backward_is_linear_in_grad_out():
 def test_dropin_autograd_module_matches_capi():
     """The reference-facing path: GaussianRasterizer(...) autograd Function == raw C-ABI results."""
     import diff_gaussian_rasterization as dgr
-    sc = synth.random_cube_scene(5000, 160, seed=6, bg=(0.1, 0.2, 0.3))
-    rc = _run(sc)
-    T = lambda a, rg=True: torch.tensor(a, device="cuda", requires_grad=rg)
-    m, c, op, s, r = T(sc["means3D"]), T(sc["colors"]), T(sc["opacity"]), T(sc["scales"]), T(sc["rots"])
-    m2d = torch.zeros_like(m, requires_grad=True)
+    for cam in ({}, dict(width=200, height=120, focal=(170.0, 140.0), principal=(96.0, 64.0),
+                         scale_modifier=0.8)):
+        sc = synth.random_cube_scene(5000, 160, seed=6, bg=(0.1, 0.2, 0.3), **cam)
+        H, W = sc["H"], sc["W"]
+        rc = _run(sc)
+        T = lambda a, rg=True: torch.tensor(a, device="cuda", requires_grad=rg)
+        m, c, op, s, r = T(sc["means3D"]), T(sc["colors"]), T(sc["opacity"]), T(sc["scales"]), T(sc["rots"])
+        m2d = torch.zeros_like(m, requires_grad=True)
+        rs = dgr.GaussianRasterizationSettings(
+            image_height=H, image_width=W, tanfovx=sc["tanfovx"], tanfovy=sc["tanfovy"],
+            bg=torch.tensor(sc["bg"], device="cuda"), scale_modifier=sc["scale_modifier"],
+            viewmatrix=torch.tensor(sc["view"]), projmatrix=torch.tensor(sc["proj"], device="cuda"),    # host cam, device proj
+            sh_degree=3, campos=torch.tensor(sc["campos"]), prefiltered=False, debug=False)
+        img, radii = dgr.GaussianRasterizer(raster_settings=rs)(means3D=m, means2D=m2d, opacities=op, shs=None,
+                                                                colors_precomp=c, scales=s, rotations=r, cov3D_precomp=None)
+        assert img.shape == (3, H, W) and radii.dtype == torch.int32 and torch.equal(radii, rc.radii)
+        assert torch.equal(img, rc.color)
+        g = torch.randn_like(img)
+        img.backward(g)
+        want = rc.backward(g)
+        assert rel_err(_np(m.grad), _np(want["dL_dmeans3D"])) < 1e-5
+        assert rel_err(_np(s.grad), _np(want["dL_dscales"])) < 1e-5 and rel_err(_np(r.grad), _np(want["dL_drots"])) < 1e-5
+        assert rel_err(_np(op.grad), _np(want["dL_dopacity"])) < 1e-5 and rel_err(_np(c.grad), _np(want["dL_dcolors"])) < 1e-5
+        assert m2d.grad is not None and m2d.grad.shape == (5000, 3)
+        vis = dgr.GaussianRasterizer(raster_settings=rs).markVisible(m.detach())
+        assert vis.dtype == torch.bool and bool(vis.all())
+
+
+def test_mark_visible_matches_the_oracle_at_the_near_plane():
+    """GaussianRasterizer.markVisible == the oracle's fp32 mark_visible bit for bit on points straddling view-space
+    z = 0.2, incl. points within rounding of it; the forward renders no point it marks absent."""
+    import diff_gaussian_rasterization as dgr
+    from helpers import near_plane_scene
+    from oracle.raster_oracle import RasterOracle
+    sc, z = near_plane_scene(synth.random_cube_scene(20_000, 64, seed=5, **WIDE))
+    want = RasterOracle("f32").mark_visible(sc["means3D"], sc["view"])
+    assert 1000 < want.sum() < 19_000
     rs = dgr.GaussianRasterizationSettings(
-        image_height=160, image_width=160, tanfovx=sc["tanfovx"], tanfovy=sc["tanfovy"],
-        bg=torch.tensor(sc["bg"], device="cuda"), scale_modifier=1.0, viewmatrix=torch.tensor(sc["view"]),     # host cam
-        projmatrix=torch.tensor(sc["proj"], device="cuda"), sh_degree=3, campos=torch.tensor(sc["campos"]),     # device proj
-        prefiltered=False, debug=False)
-    img, radii = dgr.GaussianRasterizer(raster_settings=rs)(means3D=m, means2D=m2d, opacities=op, shs=None,
-                                                            colors_precomp=c, scales=s, rotations=r, cov3D_precomp=None)
-    assert img.shape == (3, 160, 160) and radii.dtype == torch.int32 and torch.equal(radii, rc.radii)
-    assert torch.equal(img, rc.color)
-    g = torch.randn_like(img)
-    img.backward(g)
-    want = rc.backward(g)
-    assert rel_err(_np(m.grad), _np(want["dL_dmeans3D"])) < 1e-5
-    assert rel_err(_np(s.grad), _np(want["dL_dscales"])) < 1e-5 and rel_err(_np(r.grad), _np(want["dL_drots"])) < 1e-5
-    assert rel_err(_np(op.grad), _np(want["dL_dopacity"])) < 1e-5 and rel_err(_np(c.grad), _np(want["dL_dcolors"])) < 1e-5
-    assert m2d.grad is not None and m2d.grad.shape == (5000, 3)
-    vis = dgr.GaussianRasterizer(raster_settings=rs).markVisible(m.detach())
-    assert vis.dtype == torch.bool and bool(vis.all())
+        image_height=sc["H"], image_width=sc["W"], tanfovx=sc["tanfovx"], tanfovy=sc["tanfovy"], bg=torch.zeros(3),
+        scale_modifier=1.0, viewmatrix=torch.tensor(sc["view"]), projmatrix=torch.tensor(sc["proj"]), sh_degree=3,
+        campos=torch.tensor(sc["campos"]), prefiltered=False, debug=False)
+    got = _np(dgr.GaussianRasterizer(raster_settings=rs).markVisible(torch.tensor(sc["means3D"], device="cuda")))
+    assert np.array_equal(got, want)
+    rc = _run(sc)
+    assert not (_np(rc.radii) > 0)[~got].any()
 
 
-def _stereo_data(res, requires_grad=False, seed=None):
-    sc = synth.stereo_pair_scene(res, keep_maps=True) if seed is None else synth.stereo_pair_scene(res, keep_maps=True, seed=seed)
+def _stereo_data(res, requires_grad=False, seed=None, **cam_kw):
+    """cam_kw: synth.stereo_pair_scene's novel-camera keywords (width, height, focal, principal)."""
+    sc = synth.stereo_pair_scene(res, keep_maps=True, **cam_kw) if seed is None else \
+        synth.stereo_pair_scene(res, keep_maps=True, seed=seed, **cam_kw)
     cam = sc["cam"]
     data = {"novel_view": {"FovX": torch.tensor([cam["FovX"]], dtype=torch.float64),
                            "FovY": torch.tensor([cam["FovY"]], dtype=torch.float64),
-                           "width": torch.tensor([res]), "height": torch.tensor([res]),
+                           "width": torch.tensor([sc["W"]]), "height": torch.tensor([sc["H"]]),
                            "world_view_transform": torch.tensor(cam["world_view_transform"])[None],
                            "full_proj_transform": torch.tensor(cam["full_proj_transform"])[None],
                            "camera_center": torch.tensor(cam["camera_center"])[None]}}
@@ -273,34 +317,38 @@ def test_mirrored_render_and_pts2render():
     """reference-signature wrappers: pts2render(data, bg_color) (fused map ingest) and the gather -> render(data, idx, ...)
     data flow of the reference give the same image, equal to the oracle on the gathered Gaussians."""
     from gps_gaussian_b200.GaussianRender import pts2render, pts2render_gather
-    res = 128
-    sc, data = _stereo_data(res)
-    out = pts2render(data, [0.0, 0.0, 0.0])["novel_view"]["img_pred"]
-    assert out.shape == (1, 3, res, res)
-    _, ref = oracle_forward(sc, "f32")
-    d = np.abs(_np(out[0]) - ref["color"]).max(0)
-    assert (d > RGB_TOL).mean() < 5e-4 and d.max() < 1e-2
-    out2 = pts2render_gather(data, [0.0, 0.0, 0.0])["novel_view"]["img_pred"]
-    assert torch.equal(out, out2)                 # same Gaussians in the same order -> bit-identical image
+    for cam in ({}, dict(width=160, height=96, focal=(150.0, 120.0), principal=(78.0, 50.0))):
+        res = 128
+        sc, data = _stereo_data(res, **cam)
+        out = pts2render(data, [0.0, 0.0, 0.0])["novel_view"]["img_pred"]
+        assert out.shape == (1, 3, sc["H"], sc["W"])
+        _, ref = oracle_forward(sc, "f32")
+        d = np.abs(_np(out[0]) - ref["color"]).max(0)
+        assert (d > RGB_TOL).mean() < 5e-4 and d.max() < 1e-2
+        out2 = pts2render_gather(data, [0.0, 0.0, 0.0])["novel_view"]["img_pred"]
+        assert torch.equal(out, out2)                 # same Gaussians in the same order -> bit-identical image
 
 
 def test_fused_ingest_gradients_match_gather_path():
     """d(loss)/d(maps) of the fused ingest == autograd through the reference's gather/concat/render data flow."""
     from gps_gaussian_b200.GaussianRender import pts2render, pts2render_gather
-    res = 96
-    g = torch.randn(1, 3, res, res, device="cuda", generator=torch.Generator("cuda").manual_seed(3))
-    grads = []
-    for fn in (pts2render, pts2render_gather):
-        _, data = _stereo_data(res, requires_grad=True, seed=4242)
-        out = fn(data, [0.1, 0.2, 0.3])["novel_view"]["img_pred"]
-        (out * g).sum().backward()
-        grads.append({(v, k): data[v][k].grad for v in ("lmain", "rmain") for k in ("xyz", "img", "rot_maps", "scale_maps", "opacity_maps")})
-    for key in grads[0]:
-        a, b = grads[0][key], grads[1][key]
-        assert a is not None and b is not None and a.shape == b.shape, key
-        scale = max(float(b.abs().max()), 1e-20)
-        per = (a - b).abs().flatten(1).max(0).values / scale if a.dim() > 1 else (a - b).abs() / scale
-        assert int((per > GRAD_TOL).sum()) <= 4 and float(per.max()) < 5e-2, (key, float(per.max()))
+    for cam in ({}, dict(width=72, height=120, focal=(80.0, 100.0), principal=(35.0, 62.0))):
+        res = 96
+        H, W = cam.get("height", res), cam.get("width", res)
+        g = torch.randn(1, 3, H, W, device="cuda", generator=torch.Generator("cuda").manual_seed(3))
+        grads = []
+        for fn in (pts2render, pts2render_gather):
+            _, data = _stereo_data(res, requires_grad=True, seed=4242, **cam)
+            out = fn(data, [0.1, 0.2, 0.3])["novel_view"]["img_pred"]
+            (out * g).sum().backward()
+            grads.append({(v, k): data[v][k].grad for v in ("lmain", "rmain")
+                          for k in ("xyz", "img", "rot_maps", "scale_maps", "opacity_maps")})
+        for key in grads[0]:
+            a, b = grads[0][key], grads[1][key]
+            assert a is not None and b is not None and a.shape == b.shape, key
+            scale = max(float(b.abs().max()), 1e-20)
+            per = (a - b).abs().flatten(1).max(0).values / scale if a.dim() > 1 else (a - b).abs() / scale
+            assert int((per > GRAD_TOL).sum()) <= 4 and float(per.max()) < 5e-2, (key, float(per.max()))
 
 
 def test_c2_full_size_parity_and_properties():
@@ -340,31 +388,33 @@ def test_planned_sync_free_forward_and_cuda_graph():
     bit-identical image / radii to the exact entry point."""
     from gps_gaussian_b200.introspect import to_device
     from gps_gaussian_b200.planned import PlannedRasterizer
-    sc = synth.random_cube_scene(10_000, 256, seed=8, bg=(0.05, 0.1, 0.2))
-    ref = _run(sc)
-    d = to_device(sc)
-    args = (sc, d["means3D"], d["colors"], d["opacity"], d["scales"], d["rots"])
-    pr = PlannedRasterizer(10_000, 256, 256, capacity_pairs=int(ref.num_rendered * 1.25))
-    out = pr.forward(*args)
-    torch.cuda.synchronize()
-    st = pr.status()
-    assert not st["overflow"] and st["num_rendered"] == ref.num_rendered
-    assert torch.equal(out, ref.color) and torch.equal(pr.radii, ref.radii)
-    # overflow: capacity too small -> flagged, nothing written out of bounds, recoverable with grow()
-    small = PlannedRasterizer(10_000, 256, 256, capacity_pairs=ref.num_rendered // 2)
-    small.forward(*args)
-    torch.cuda.synchronize()
-    assert small.status()["overflow"] and not small.ok()
-    small.grow()
-    out2 = small.forward(*args)
-    torch.cuda.synchronize()
-    assert small.ok() and torch.equal(out2, ref.color)
-    # CUDA graph capture + replay
-    pr.capture(*args)
-    pr.color.zero_()
-    pr.replay(); pr.replay()
-    torch.cuda.synchronize()
-    assert pr.ok() and torch.equal(pr.color, ref.color)
+    for cam in ({}, dict(width=256, height=144, focal=(230.0, 190.0), principal=(125.0, 70.0))):
+        sc = synth.random_cube_scene(10_000, 256, seed=8, bg=(0.05, 0.1, 0.2), **cam)
+        H, W = sc["H"], sc["W"]
+        ref = _run(sc)
+        d = to_device(sc)
+        args = (sc, d["means3D"], d["colors"], d["opacity"], d["scales"], d["rots"])
+        pr = PlannedRasterizer(10_000, H, W, capacity_pairs=int(ref.num_rendered * 1.25))
+        out = pr.forward(*args)
+        torch.cuda.synchronize()
+        st = pr.status()
+        assert not st["overflow"] and st["num_rendered"] == ref.num_rendered
+        assert torch.equal(out, ref.color) and torch.equal(pr.radii, ref.radii)
+        # overflow: capacity too small -> flagged, nothing written out of bounds, recoverable with grow()
+        small = PlannedRasterizer(10_000, H, W, capacity_pairs=ref.num_rendered // 2)
+        small.forward(*args)
+        torch.cuda.synchronize()
+        assert small.status()["overflow"] and not small.ok()
+        small.grow()
+        out2 = small.forward(*args)
+        torch.cuda.synchronize()
+        assert small.ok() and torch.equal(out2, ref.color)
+        # CUDA graph capture + replay
+        pr.capture(*args)
+        pr.color.zero_()
+        pr.replay(); pr.replay()
+        torch.cuda.synchronize()
+        assert pr.ok() and torch.equal(pr.color, ref.color)
 
 
 @pytest.mark.parametrize("base_P,rep", [(1500, 3), (120, 40)])
@@ -425,37 +475,48 @@ def test_2048_render_resolution_forward_and_backward():
 
 
 def test_randomised_parity_sweep():
-    """Small randomised sweep (image size, point count, spread, splat size, background): every integer output bit-exact."""
+    """Small randomised sweep (image size, point count, spread, splat size, background): every integer output bit-exact.
+    Each scene is rendered again through a camera with width and height drawn independently, fx != fy, an off-centre
+    principal point and scale_modifier != 1."""
     rng = np.random.default_rng(2024)
+    cam_rng = np.random.default_rng(2025)
     for k in range(8):
         res = int(rng.integers(40, 300))
         P = int(rng.integers(1, 6000))
-        sc = synth.random_cube_scene(P, res, spread=float(rng.uniform(0.2, 2.5)), scale_mul=float(rng.uniform(0.5, 8.0)),
-                                     bg=tuple(rng.uniform(0, 1, 3)), seed=int(rng.integers(1 << 30)))
-        _assert_forward_parity(sc)
+        kw = dict(spread=float(rng.uniform(0.2, 2.5)), scale_mul=float(rng.uniform(0.5, 8.0)), bg=tuple(rng.uniform(0, 1, 3)),
+                  seed=int(rng.integers(1 << 30)))
+        W, H = (int(v) for v in cam_rng.integers(8, 300, 2))
+        fx = 0.8 * math.sqrt(W * H) * cam_rng.uniform(0.7, 1.4)
+        aniso = dict(width=W, height=H, focal=(fx, fx * cam_rng.uniform(0.6, 1.6)),
+                     principal=(W * cam_rng.uniform(0.3, 0.7), H * cam_rng.uniform(0.3, 0.7)),
+                     scale_modifier=cam_rng.uniform(0.5, 2.0))
+        _assert_forward_parity(synth.random_cube_scene(P, res, **kw))
+        _assert_forward_parity(synth.random_cube_scene(P, res, **kw, **aniso))
 
 
 def test_pts2render_batch_of_two_and_host_pipeline():
     """bs = 2 through the reference-signature pts2render, and the packed host-buffer pipeline == direct render."""
     from gps_gaussian_b200.GaussianRender import pts2render
     from gps_gaussian_b200.pipeline import HostRenderPipeline, pack_host
-    res = 96
-    sc0, d0 = _stereo_data(res, seed=11)
-    sc1, d1 = _stereo_data(res, seed=12)
-    data = {"novel_view": {k: torch.cat([d0["novel_view"][k], d1["novel_view"][k]]) for k in d0["novel_view"]}}
-    for v in ("lmain", "rmain"):
-        data[v] = {k: torch.cat([d0[v][k], d1[v][k]]) for k in d0[v]}
-    out = pts2render(data, [0.0, 0.0, 0.0])["novel_view"]["img_pred"]
-    assert out.shape == (2, 3, res, res)
-    for i, sc in enumerate((sc0, sc1)):
-        _, ref = oracle_forward(sc, "f32")
-        d = np.abs(_np(out[i]) - ref["color"]).max(0)
-        assert (d > RGB_TOL).mean() < 1e-3 and d.max() < 1e-2
-    pipe = HostRenderPipeline("cuda", max(sc0["means3D"].shape[0], sc1["means3D"].shape[0]), res, res)
-    items = [(pack_host(sc), dd, 0) for sc, dd in ((sc0, d0), (sc1, d1), (sc0, d0))]
-    outs = [torch.empty(3, res, res).pin_memory() for _ in items]
-    pipe.run(items, outs)
-    assert torch.equal(outs[0], outs[2]) and torch.equal(outs[0].cuda(), out[0]) and torch.equal(outs[1].cuda(), out[1])
+    for cam in ({}, dict(width=112, height=80, focal=(95.0, 80.0), principal=(54.0, 41.0))):
+        res = 96
+        sc0, d0 = _stereo_data(res, seed=11, **cam)
+        sc1, d1 = _stereo_data(res, seed=12, **cam)
+        H, W = sc0["H"], sc0["W"]
+        data = {"novel_view": {k: torch.cat([d0["novel_view"][k], d1["novel_view"][k]]) for k in d0["novel_view"]}}
+        for v in ("lmain", "rmain"):
+            data[v] = {k: torch.cat([d0[v][k], d1[v][k]]) for k in d0[v]}
+        out = pts2render(data, [0.0, 0.0, 0.0])["novel_view"]["img_pred"]
+        assert out.shape == (2, 3, H, W)
+        for i, sc in enumerate((sc0, sc1)):
+            _, ref = oracle_forward(sc, "f32")
+            d = np.abs(_np(out[i]) - ref["color"]).max(0)
+            assert (d > RGB_TOL).mean() < 1e-3 and d.max() < 1e-2
+        pipe = HostRenderPipeline("cuda", max(sc0["means3D"].shape[0], sc1["means3D"].shape[0]), H, W)
+        items = [(pack_host(sc), dd, 0) for sc, dd in ((sc0, d0), (sc1, d1), (sc0, d0))]
+        outs = [torch.empty(3, H, W).pin_memory() for _ in items]
+        pipe.run(items, outs)
+        assert torch.equal(outs[0], outs[2]) and torch.equal(outs[0].cuda(), out[0]) and torch.equal(outs[1].cuda(), out[1])
 
 
 def test_batched_pts2render_one_sync_matches_per_sample_path():
