@@ -8,6 +8,8 @@ import ctypes as C
 import os
 import threading
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libgpsg_sm90.so")
 
@@ -81,9 +83,6 @@ lib.gpsg_raster_status_ptr.argtypes = [_vp, _i, _i]
 lib.gpsg_rasterize_forward_planned.restype = _i
 lib.gpsg_rasterize_forward_planned.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_vp] * 10 + [_i64, _vp, _vp]
 _pp = C.POINTER(C.c_void_p)
-lib.gpsg_rasterize_forward_maps.restype = _i
-lib.gpsg_rasterize_forward_maps.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _pp, _pp, _pp, _pp, _pp, _pp, _vp, _vp,
-                                            ALLOC_FN, _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, C.POINTER(C.c_int32)]
 lib.gpsg_rasterize_forward_maps_planned.restype = _i
 lib.gpsg_rasterize_forward_maps_planned.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _pp, _pp, _pp, _pp, _pp, _pp, _vp, _vp,
                                                     _vp, _vp, _i64, _vp, _vp]
@@ -130,7 +129,7 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_corr_sampler_forward", "gpsg_corr_sampler_backward", "gpsg_corr_build_pyramid", "gpsg_corr_build_backward",
             "gpsg_corr_lookup_pyramid_forward", "gpsg_corr_lookup_pyramid_backward", "gpsg_raster_geom_bytes",
             "gpsg_raster_binning_bytes", "gpsg_raster_image_bytes", "gpsg_raster_status_ptr",
-            "gpsg_rasterize_forward_planned", "gpsg_rasterize_forward_maps", "gpsg_rasterize_forward_maps_planned", "gpsg_rasterize_forward_maps_begin", "gpsg_rasterize_forward_maps_finish",
+            "gpsg_rasterize_forward_planned", "gpsg_rasterize_forward_maps_planned", "gpsg_rasterize_forward_maps_begin", "gpsg_rasterize_forward_maps_finish",
             "gpsg_rasterize_backward_maps_workspace_bytes",
             "gpsg_rasterize_backward_maps", "gpsg_unproject_forward", "gpsg_unproject_backward", "gpsg_l1_ssim_workspace_bytes", "gpsg_l1_ssim_forward",
             "gpsg_l1_ssim_backward", "gpsg_set_corr_build", "gpsg_profile_enable",
@@ -149,7 +148,6 @@ _tls = threading.local()
 
 
 def _alloc_trampoline(user, nbytes):
-    import torch
     try:
         t = torch.empty(int(nbytes), dtype=torch.uint8, device=_tls.device)
         _tls.bufs[int(user or 0)] = t
@@ -170,6 +168,68 @@ def end_alloc():
     bufs = _tls.bufs
     _tls.bufs = {}
     return bufs
+
+
+def device_stream(device):
+    """(device index, current stream handle) of a CUDA device: the first two arguments of every gpsg_* call."""
+    device = torch.device(device)
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    return idx, C.c_void_p(torch.cuda.current_stream(idx).cuda_stream)
+
+
+def _ptr(t):
+    return C.c_void_p(t.data_ptr()) if (t is not None and t.numel() > 0) else None
+
+
+def rasterize_forward(settings, out_color, radii, means3D, opacities, colors_precomp=None, shs=None, scales=None,
+                      rotations=None, cov3D_precomp=None):
+    """One forward through the exact entry point gpsg_rasterize_forward: one host synchronisation, and the global radix
+    fallback takes tile lists of any length.  Inputs are contiguous fp32 tensors on one CUDA device, absent ones None.
+    Writes out_color [3,H,W] and radii [P]; returns (num_rendered, (geom, binning, image)), the buffers the backward
+    reads."""
+    dev = means3D.device
+    idx, stream = device_stream(dev)
+    n = C.c_int32(0)
+    begin_alloc(dev)
+    try:
+        with torch.cuda.device(dev):
+            rc = lib.gpsg_rasterize_forward(
+                C.byref(settings), idx, stream, int(means3D.shape[0]), int(shs.shape[1]) if shs is not None else 0,
+                _ptr(means3D), _ptr(colors_precomp), _ptr(shs), _ptr(opacities), _ptr(scales), _ptr(rotations),
+                _ptr(cov3D_precomp), _ptr(out_color), _ptr(radii), ALLOC_CB, C.c_void_p(1), ALLOC_CB, C.c_void_p(2),
+                ALLOC_CB, C.c_void_p(3), C.byref(n))
+    finally:
+        bufs = end_alloc()
+    check(rc, "gpsg_rasterize_forward")
+    return int(n.value), (bufs.get(1), bufs.get(2), bufs.get(3))
+
+
+def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D, opacities, colors_precomp=None,
+                       shs=None, scales=None, rotations=None, cov3D_precomp=None, want_cov3D=False):
+    """Backward of `rasterize_forward` with the same inputs, its num_rendered, buffers and radii.  Returns the gradients
+    dL_dmeans2D [P,3], dL_dcolors [P,3], dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drots [P,4],
+    dL_dcov3D [P,6] and dL_dsh [P,M,3].  dL_dcolors is None on the SH path, dL_dsh is None without shs and dL_dcov3D
+    is None unless want_cov3D."""
+    dev = means3D.device
+    P = int(means3D.shape[0])
+    new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
+    out = dict(dL_dmeans2D=new(P, 3), dL_dcolors=new(P, 3) if colors_precomp is not None else None,
+               dL_dopacity=new(P, 1), dL_dmeans3D=new(P, 3), dL_dscales=new(P, 3), dL_drots=new(P, 4),
+               dL_dcov3D=new(P, 6) if want_cov3D else None,
+               dL_dsh=new(P, int(shs.shape[1]), 3) if shs is not None else None)
+    ws = torch.empty(int(lib.gpsg_rasterize_backward_workspace_bytes(P)), dtype=torch.uint8, device=dev)
+    g = grad_color.detach().to(torch.float32).contiguous()
+    idx, stream = device_stream(dev)
+    geom, binning, image = bufs
+    with torch.cuda.device(dev):
+        rc = lib.gpsg_rasterize_backward(
+            C.byref(settings), idx, stream, P, int(shs.shape[1]) if shs is not None else 0, num_rendered, _ptr(means3D),
+            _ptr(colors_precomp), _ptr(shs), _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(cov3D_precomp),
+            _ptr(radii), _ptr(geom), _ptr(binning), _ptr(image), _ptr(g), _ptr(out["dL_dmeans2D"]),
+            _ptr(out["dL_dcolors"]), _ptr(out["dL_dopacity"]), _ptr(out["dL_dmeans3D"]), _ptr(out["dL_dcov3D"]),
+            _ptr(out["dL_dsh"]), _ptr(out["dL_dscales"]), _ptr(out["dL_drots"]), _ptr(ws))
+    check(rc, "gpsg_rasterize_backward")
+    return out
 
 
 lib.gpsg_set_corr_build.restype = _i

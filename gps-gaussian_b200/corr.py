@@ -24,14 +24,6 @@ from . import _lib  # noqa: E402
 _DT = {torch.float32: 0, torch.float16: 1}
 
 
-def _dev(t):
-    return t.device.index if t.device.index is not None else torch.cuda.current_device()
-
-
-def _stream(t):
-    return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
-
-
 class CorrSampler(torch.autograd.Function):
     """Per-level sampler, exactly the reference class (core/corr.py:17-29)."""
 
@@ -68,7 +60,7 @@ class _BuildPyramid(torch.autograd.Function):
         vols = [buf[o:o + n].view(B, H, W1, W2 >> l) for l, (o, n) in enumerate(zip(offs, sizes))]
         ptrs = (C.c_void_p * 4)(*[v.data_ptr() if v.numel() else None for v in vols] + [None] * (4 - levels))
         with torch.cuda.device(f1.device):
-            rc = _lib.lib.gpsg_corr_build_pyramid(_dev(f1), _stream(f1), _DT[f1.dtype], B, D, H, W1, W2,
+            rc = _lib.lib.gpsg_corr_build_pyramid(*_lib.device_stream(f1.device), _DT[f1.dtype], B, D, H, W1, W2,
                                                   C.c_void_p(f1.data_ptr()), C.c_void_p(f2.data_ptr()), ptrs, levels)
         _lib.check(rc, "gpsg_corr_build_pyramid")
         ctx.save_for_backward(f1, f2)
@@ -96,7 +88,7 @@ class _BuildPyramid(torch.autograd.Function):
         g = g.to(f1.dtype).contiguous()
         d1, d2 = torch.empty_like(f1), torch.empty_like(f2)
         with torch.cuda.device(f1.device):
-            rc = _lib.lib.gpsg_corr_build_backward(_dev(f1), _stream(f1), _DT[f1.dtype], B, D, H, W1, W2,
+            rc = _lib.lib.gpsg_corr_build_backward(*_lib.device_stream(f1.device), _DT[f1.dtype], B, D, H, W1, W2,
                                                    C.c_void_p(f1.data_ptr()), C.c_void_p(f2.data_ptr()),
                                                    C.c_void_p(g.data_ptr()), C.c_void_p(d1.data_ptr()),
                                                    C.c_void_p(d2.data_ptr()))
@@ -120,9 +112,9 @@ class _LookupPyramid(torch.autograd.Function):
         ptrs = (C.c_void_p * 4)(*[v.data_ptr() if v.numel() else None for v in vs] + [None] * (4 - L))
         widths = (C.c_int32 * 4)(*[int(v.shape[3]) for v in vs] + [0] * (4 - L))
         with torch.cuda.device(v0.device):
-            rc = _lib.lib.gpsg_corr_lookup_pyramid_forward(_dev(v0), _stream(v0), _DT[v0.dtype], B, H, W1, ptrs, widths, L,
-                                                           C.c_void_p(c.data_ptr()), int(c.stride(0)), int(radius),
-                                                           C.c_void_p(out.data_ptr()))
+            rc = _lib.lib.gpsg_corr_lookup_pyramid_forward(*_lib.device_stream(v0.device), _DT[v0.dtype], B, H, W1, ptrs,
+                                                           widths, L, C.c_void_p(c.data_ptr()), int(c.stride(0)),
+                                                           int(radius), C.c_void_p(out.data_ptr()))
         _lib.check(rc, "gpsg_corr_lookup_pyramid_forward")
         ctx.save_for_backward(c)
         ctx.meta = (radius, [tuple(v.shape) for v in vs], v0.dtype)
@@ -139,9 +131,9 @@ class _LookupPyramid(torch.autograd.Function):
         ptrs = (C.c_void_p * 4)(*[v.data_ptr() if v.numel() else None for v in gv] + [None] * (4 - L))
         widths = (C.c_int32 * 4)(*[int(s[3]) for s in shapes] + [0] * (4 - L))
         with torch.cuda.device(g.device):
-            rc = _lib.lib.gpsg_corr_lookup_pyramid_backward(_dev(g), _stream(g), _DT[dtype], B, H, W1, ptrs, widths, L,
-                                                            C.c_void_p(c.data_ptr()), int(c.stride(0)), int(radius),
-                                                            C.c_void_p(g.data_ptr()))
+            rc = _lib.lib.gpsg_corr_lookup_pyramid_backward(*_lib.device_stream(g.device), _DT[dtype], B, H, W1, ptrs,
+                                                            widths, L, C.c_void_p(c.data_ptr()), int(c.stride(0)),
+                                                            int(radius), C.c_void_p(g.data_ptr()))
         _lib.check(rc, "gpsg_corr_lookup_pyramid_backward")
         return (None, None) + tuple(gv)
 

@@ -280,21 +280,6 @@ static int forward_exact_finish(const GpsgRasterSettings* s, int device, cudaStr
     return GPSG_OK;
 }
 
-static int forward_exact(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, int sh_M, GaussianSrc src,
-                         const float* shs, float* out_color, int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
-                         gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc, void* image_user,
-                         int32_t* num_rendered) {
-    uint32_t* slot = pinned_slot();      // thread-local pinned words for the one device->host read of this forward
-    GPSG_REQUIRE(slot != nullptr, "cudaHostAlloc failed");
-    void *geom_base = nullptr, *img_base = nullptr;
-    int rc = forward_exact_begin(s, device, stream, P, src, radii, geom_alloc, geom_user, image_alloc, image_user, slot,
-                                 &geom_base, &img_base);
-    if (rc) return rc;
-    if (P > 0) GPSG_CUDA(cudaStreamSynchronize(stream));
-    return forward_exact_finish(s, device, stream, P, sh_M, src, shs, out_color, radii, geom_base, img_base, binning_alloc,
-                                binning_user, slot, num_rendered);
-}
-
 int gpsg_rasterize_forward(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
                            const float* means3D, const float* colors_precomp, const float* shs,
                            const float* opacities, const float* scales, const float* rotations,
@@ -317,11 +302,18 @@ int gpsg_rasterize_forward(const GpsgRasterSettings* s, int device, void* stream
             GPSG_REQUIRE(sh_M >= (s->sh_degree + 1) * (s->sh_degree + 1), "shs has fewer coefficients than (sh_degree+1)^2");
         }
     }
-    return forward_exact(s, device, (cudaStream_t)stream_, P, sh_M,
-                         aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations, opacities,
-                                 colors_precomp, cov3D_precomp),
-                         shs, out_color, radii, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user,
-                         num_rendered);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const GaussianSrc src = aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations, opacities,
+                                    colors_precomp, cov3D_precomp);
+    uint32_t* slot = pinned_slot();      // thread-local pinned words for the one device->host read of this forward
+    GPSG_REQUIRE(slot != nullptr, "cudaHostAlloc failed");
+    void *geom_base = nullptr, *img_base = nullptr;
+    int rc = forward_exact_begin(s, device, stream, P, src, radii, geom_alloc, geom_user, image_alloc, image_user, slot,
+                                 &geom_base, &img_base);
+    if (rc) return rc;
+    if (P > 0) GPSG_CUDA(cudaStreamSynchronize(stream));
+    return forward_exact_finish(s, device, stream, P, sh_M, src, shs, out_color, radii, geom_base, img_base, binning_alloc,
+                                binning_user, slot, num_rendered);
 }
 
 static int check_maps(int S2, const uint8_t* const* valid, const float* const* xyz, const float* const* img,
@@ -342,23 +334,6 @@ static GaussianSrc maps_src(int S2, const uint8_t* const* valid, const float* co
         src.opac[v] = opacity[v];
     }
     return src;
-}
-
-int gpsg_rasterize_forward_maps(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                const float* const* rot, const float* const* scale, const float* const* opacity,
-                                float* out_color, int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
-                                gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
-                                void* image_user, int32_t* num_rendered) {
-    GPSG_REQUIRE(s != nullptr, "settings is NULL");
-    GPSG_REQUIRE(s->image_width > 0 && s->image_height > 0, "image size must be positive");
-    GPSG_REQUIRE(out_color && radii, "out_color / radii is NULL");
-    GPSG_REQUIRE(geom_alloc && binning_alloc && image_alloc, "allocator callback is NULL");
-    int rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
-    if (rc) return rc;
-    return forward_exact(s, device, (cudaStream_t)stream_, 2 * pixels_per_view, 0,
-                         maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), nullptr, out_color, radii,
-                         geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, num_rendered);
 }
 
 int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,

@@ -40,10 +40,6 @@ def _coords_x(coords):
     return c, int(c.stride(0))
 
 
-def _dev_index(t):
-    return t.device.index if t.device.index is not None else torch.cuda.current_device()
-
-
 def forward(volume, coords, radius):
     _check(volume, coords)
     vol = volume.detach()
@@ -54,7 +50,7 @@ def forward(volume, coords, radius):
     out = torch.empty((B, 2 * int(radius) + 1, H, W1), dtype=vol.dtype, device=vol.device)
     with torch.cuda.device(vol.device):
         rc = _lib.lib.gpsg_corr_sampler_forward(
-            _dev_index(vol), C.c_void_p(torch.cuda.current_stream(vol.device).cuda_stream), _DT[vol.dtype], B, H, W1, W2,
+            *_lib.device_stream(vol.device), _DT[vol.dtype], B, H, W1, W2,
             C.c_void_p(vol.data_ptr()), vol.stride(0), vol.stride(1), vol.stride(2), C.c_void_p(c.data_ptr()), csb,
             int(radius), C.c_void_p(out.data_ptr()))
     _lib.check(rc, "gpsg_corr_sampler_forward")
@@ -69,7 +65,7 @@ def backward(volume, coords, grad_output, radius):
     gvol = torch.empty((B, H, W1, W2), dtype=volume.dtype, device=volume.device)
     with torch.cuda.device(volume.device):
         rc = _lib.lib.gpsg_corr_sampler_backward(
-            _dev_index(volume), C.c_void_p(torch.cuda.current_stream(volume.device).cuda_stream), _DT[volume.dtype],
+            *_lib.device_stream(volume.device), _DT[volume.dtype],
             B, H, W1, W2, C.c_void_p(c.data_ptr()), csb, C.c_void_p(g.data_ptr()), int(radius),
             C.c_void_p(gvol.data_ptr()))
     _lib.check(rc, "gpsg_corr_sampler_backward")

@@ -98,10 +98,6 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if (t is not None and t.numel() > 0) else None
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings):
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
@@ -125,7 +121,6 @@ class _RasterizeGaussians(torch.autograd.Function):
         sc = _f32c(scales) if scales.numel() else None
         ro = _f32c(rotations) if rotations.numel() else None
         cp = _f32c(cov3Ds_precomp) if cov3Ds_precomp.numel() else None
-        sh_M = int(shs.shape[1]) if shs is not None else 0
         for name, t, k in (("opacities", op, 1), ("scales", sc, 3), ("rotations", ro, 4), ("colors_precomp", col, 3),
                            ("cov3D_precomp", cp, 6)):
             if t is not None and (t.numel() != k * P or t.device != dev):
@@ -135,54 +130,23 @@ class _RasterizeGaussians(torch.autograd.Function):
             raise RuntimeError(f"diff_gaussian_rasterization (gpsg): shs must be [{P}, M, 3] on {dev}")
         color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
         radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        num_rendered = C.c_int32(0)
-        _lib.begin_alloc(dev)
-        try:
-            with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_rasterize_forward(
-                    C.byref(settings), dev.index if dev.index is not None else torch.cuda.current_device(),
-                    _stream(dev), P, sh_M, _ptr(m3), _ptr(col), _ptr(shs), _ptr(op), _ptr(sc), _ptr(ro), _ptr(cp),
-                    _ptr(color), _ptr(radii), _lib.ALLOC_CB, C.c_void_p(1), _lib.ALLOC_CB, C.c_void_p(2),
-                    _lib.ALLOC_CB, C.c_void_p(3), C.byref(num_rendered))
-        finally:
-            bufs = _lib.end_alloc()
-        _lib.check(rc, "gpsg_rasterize_forward")
+        ctx.num_rendered, ctx.bufs = _lib.rasterize_forward(settings, color, radii, m3, op, colors_precomp=col, shs=shs,
+                                                            scales=sc, rotations=ro, cov3D_precomp=cp)
         ctx.settings = settings
-        ctx.num_rendered = int(num_rendered.value)
-        ctx.bufs = (bufs.get(1), bufs.get(2), bufs.get(3))
-        ctx.opt = (col is not None, shs is not None, sc is not None, ro is not None, cp is not None, sh_M)
-        ctx.save_for_backward(*[t if t is not None else torch.empty(0, device=dev) for t in
-                                (m3, col, shs, op, sc, ro, cp, radii)])
+        ctx.save_for_backward(m3, col, shs, op, sc, ro, cp, radii)
         ctx.mark_non_differentiable(radii)
         return color, radii
 
     @staticmethod
     def backward(ctx, grad_out_color, _grad_radii):
         m3, col, shs, op, sc, ro, cp, radii = ctx.saved_tensors
-        has_col, has_sh, has_sc, has_ro, has_cp, sh_M = ctx.opt
-        dev = m3.device
-        P = int(m3.shape[0])
-        g = _f32c(grad_out_color)
-        new = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
-        d_means2D, d_colors, d_opacity, d_means3D = new(P, 3), new(P, 3), new(P, 1), new(P, 3)
-        d_scales, d_rots = new(P, 3), new(P, 4)
-        d_cov3D = new(P, 6) if has_cp else None
-        d_sh = new(P, sh_M, 3) if has_sh else None
-        ws = torch.empty(int(_lib.lib.gpsg_rasterize_backward_workspace_bytes(P)), dtype=torch.uint8, device=dev)
-        geom, binning, image = ctx.bufs
-        if P > 0:
-            with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_rasterize_backward(
-                    C.byref(ctx.settings), dev.index if dev.index is not None else torch.cuda.current_device(),
-                    _stream(dev), P, sh_M, ctx.num_rendered, _ptr(m3), _ptr(col) if has_col else None,
-                    _ptr(shs) if has_sh else None, _ptr(op), _ptr(sc) if has_sc else None,
-                    _ptr(ro) if has_ro else None, _ptr(cp) if has_cp else None, _ptr(radii), _ptr(geom),
-                    _ptr(binning), _ptr(image), _ptr(g), _ptr(d_means2D), _ptr(d_colors) if has_col else None,
-                    _ptr(d_opacity), _ptr(d_means3D), _ptr(d_cov3D), _ptr(d_sh), _ptr(d_scales), _ptr(d_rots), _ptr(ws))
-            _lib.check(rc, "gpsg_rasterize_backward")
+        g = _lib.rasterize_backward(ctx.settings, ctx.num_rendered, ctx.bufs, radii, grad_out_color, m3, op,
+                                    colors_precomp=col, shs=shs, scales=sc, rotations=ro, cov3D_precomp=cp,
+                                    want_cov3D=cp is not None)
         # input order: means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings
-        return (d_means3D, d_means2D, d_sh, d_colors if has_col else None, d_opacity,
-                d_scales if has_sc else None, d_rots if has_ro else None, d_cov3D, None)
+        return (g["dL_dmeans3D"], g["dL_dmeans2D"], g["dL_dsh"], g["dL_dcolors"], g["dL_dopacity"],
+                g["dL_dscales"] if sc is not None else None, g["dL_drots"] if ro is not None else None, g["dL_dcov3D"],
+                None)
 
 
 class GaussianRasterizer(nn.Module):
@@ -197,8 +161,7 @@ class GaussianRasterizer(nn.Module):
             out = torch.empty((p.shape[0],), dtype=torch.uint8, device=dev)
             view = (C.c_float * 16)(*_host_floats(self.raster_settings.viewmatrix, 16))
             with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_mark_visible(dev.index if dev.index is not None else torch.cuda.current_device(),
-                                                _stream(dev), int(p.shape[0]), _ptr(p), view, _ptr(out))
+                rc = _lib.lib.gpsg_mark_visible(*_lib.device_stream(dev), int(p.shape[0]), _ptr(p), view, _ptr(out))
             _lib.check(rc, "gpsg_mark_visible")
         return out.bool()
 

@@ -51,49 +51,18 @@ class RasterCall:
         self.num_rendered = 0
         self.bufs = None
 
-    def _p(self, t):
-        return C.c_void_p(t.data_ptr()) if (t is not None and t.numel() > 0) else None
+    def _inputs(self):
+        i = self.inp
+        return dict(means3D=i["means3D"], opacities=i["opacity"], colors_precomp=i["colors"], scales=i["scales"],
+                    rotations=i["rots"], cov3D_precomp=i.get("cov3D_precomp"))
 
     def forward(self):
-        i = self.inp
-        n = C.c_int32(0)
-        dev = self.device
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        _lib.begin_alloc(dev)
-        try:
-            rc = _lib.lib.gpsg_rasterize_forward(
-                C.byref(self.settings), idx, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream), self.P, 0,
-                self._p(i["means3D"]), self._p(i["colors"]), None, self._p(i["opacity"]), self._p(i["scales"]),
-                self._p(i["rots"]), self._p(i.get("cov3D_precomp")), self._p(self.color), self._p(self.radii),
-                _lib.ALLOC_CB, C.c_void_p(1), _lib.ALLOC_CB, C.c_void_p(2), _lib.ALLOC_CB, C.c_void_p(3), C.byref(n))
-        finally:
-            bufs = _lib.end_alloc()
-        _lib.check(rc, "gpsg_rasterize_forward")
-        self.bufs = (bufs.get(1), bufs.get(2), bufs.get(3))
-        self.num_rendered = int(n.value)
+        self.num_rendered, self.bufs = _lib.rasterize_forward(self.settings, self.color, self.radii, **self._inputs())
         return self.color
 
     def backward(self, grad_color, want_cov3D=False):
-        i = self.inp
-        dev = self.device
-        P = self.P
-        new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
-        out = dict(dL_dmeans2D=new(P, 3), dL_dcolors=new(P, 3), dL_dopacity=new(P, 1), dL_dmeans3D=new(P, 3),
-                   dL_dscales=new(P, 3), dL_drots=new(P, 4), dL_dcov3D=new(P, 6) if want_cov3D else None)
-        ws = torch.empty(int(_lib.lib.gpsg_rasterize_backward_workspace_bytes(P)), dtype=torch.uint8, device=dev)
-        g = grad_color.to(torch.float32).contiguous()
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        rc = _lib.lib.gpsg_rasterize_backward(
-            C.byref(self.settings), idx, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream), P, 0,
-            self.num_rendered, self._p(i["means3D"]), self._p(i["colors"]), None, self._p(i["opacity"]),
-            self._p(i["scales"]), self._p(i["rots"]), self._p(i.get("cov3D_precomp")), self._p(self.radii),
-            self._p(self.bufs[0]), self._p(self.bufs[1]), self._p(self.bufs[2]), self._p(g),
-            self._p(out["dL_dmeans2D"]), self._p(out["dL_dcolors"]), self._p(out["dL_dopacity"]),
-            self._p(out["dL_dmeans3D"]), self._p(out["dL_dcov3D"]), None, self._p(out["dL_dscales"]),
-            self._p(out["dL_drots"]), self._p(ws))
-        _lib.check(rc, "gpsg_rasterize_backward")
-        self._ws = ws
-        return out
+        return _lib.rasterize_backward(self.settings, self.num_rendered, self.bufs, self.radii, grad_color,
+                                       want_cov3D=want_cov3D, **self._inputs())
 
     def state(self):
         """Saved buffers as torch tensors (views into the scratch buffers)."""

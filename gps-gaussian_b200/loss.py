@@ -17,10 +17,6 @@ def _p(t):
     return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
-def _dev(t):
-    return t.device.index if t.device.index is not None else torch.cuda.current_device()
-
-
 def _check_inputs(img, gt):
     if not (img.is_cuda and gt.is_cuda):
         raise RuntimeError("gpsg loss: CUDA tensors required (no CPU fallback)")
@@ -41,14 +37,14 @@ class _L1SSIM(torch.autograd.Function):
         out = torch.empty(3, dtype=torch.float32, device=x.device)
         ws = torch.empty(int(_lib.lib.gpsg_l1_ssim_workspace_bytes(planes, H, W)), dtype=torch.uint8, device=x.device)
         maps = [None, None]
-        stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+        dev_stream = _lib.device_stream(x.device)
         with torch.cuda.device(x.device):
             # SSIM and L1 are symmetric in their two arguments: d/d(gt) is the same kernel with the roles swapped.
             for k, (a, b) in enumerate(((x, y), (y, x))):
                 if k == 1 and not need[1]:
                     continue
                 maps[k] = torch.empty((3,) + tuple(x.shape), dtype=torch.float32, device=x.device) if need[k] else None
-                rc = _lib.lib.gpsg_l1_ssim_forward(_dev(x), stream, planes, H, W, _p(a), _p(b), float(w_l1), float(w_ssim),
+                rc = _lib.lib.gpsg_l1_ssim_forward(*dev_stream, planes, H, W, _p(a), _p(b), float(w_l1), float(w_ssim),
                                                    _p(out), _p(maps[k]), _p(ws))
                 _lib.check(rc, "gpsg_l1_ssim_forward")
         ctx.save_for_backward(x, y, *[m for m in maps if m is not None])
@@ -66,14 +62,14 @@ class _L1SSIM(torch.autograd.Function):
         x, y, rest = saved[0], saved[1], saved[2:]
         g = grad_out.detach().to(torch.float32).reshape(1).contiguous()  # d/d(loss), read on the device (no sync)
         res = [None, None]
-        stream = C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)
+        dev_stream = _lib.device_stream(x.device)
         with torch.cuda.device(x.device):
             for k, (a, b) in enumerate(((x, y), (y, x))):
                 if not need[k]:
                     continue
                 m = rest.pop(0)
                 d = torch.empty_like(a)
-                rc = _lib.lib.gpsg_l1_ssim_backward(_dev(x), stream, planes, H, W, _p(a), _p(b), _p(m), w_l1, w_ssim, _p(g), _p(d))
+                rc = _lib.lib.gpsg_l1_ssim_backward(*dev_stream, planes, H, W, _p(a), _p(b), _p(m), w_l1, w_ssim, _p(g), _p(d))
                 _lib.check(rc, "gpsg_l1_ssim_backward")
                 res[k] = d.to(dt_img if k == 0 else dt_gt)
         return res[0], res[1], None, None

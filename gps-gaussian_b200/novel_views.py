@@ -14,31 +14,16 @@ streams: no per-view gather, no host sync, no H2D camera copies inside the loop.
 
 Images equal `get_novel_calib(ratio)` + `pts2render` per ratio bit for bit in both modes.
 """
-import math
-
+import numpy as np
 import torch
 
 from . import _lib
+from .GaussianRender import _RasterizeMaps, novel_settings
 from .novel_calib import calib_from_data
-from .planned import PlannedRasterizer, exact_forward
+from .planned import PlannedRasterizer
 
 _VIEWS = ('lmain', 'rmain')
 _MAX_TILE_SORT = 4096          # kMaxTileSort (csrc/gpsg_internal.cuh): longest tile list the in-CTA sort takes
-
-
-def _settings(cal, b, r, height, width, bg_color):
-    s = _lib.RasterSettings()
-    s.image_height, s.image_width = int(height), int(width)
-    s.tanfovx = math.tan(float(cal['FovX'][b, r]) * 0.5)
-    s.tanfovy = math.tan(float(cal['FovY'][b, r]) * 0.5)
-    s.bg[:] = [float(v) for v in bg_color]
-    s.scale_modifier = 1.0
-    s.viewmatrix[:] = cal['world_view_transform'][b, r].reshape(-1).tolist()
-    s.projmatrix[:] = cal['full_proj_transform'][b, r].reshape(-1).tolist()
-    s.sh_degree = 3
-    s.campos[:] = cal['camera_center'][b, r].reshape(-1).tolist()
-    s.prefiltered, s.debug = 0, 0
-    return s
 
 
 class NovelViewRenderer:
@@ -100,19 +85,25 @@ class NovelViewRenderer:
             rast.forward_maps(settings, m['valid'], m['xyz'], m['img'], m['rot'], m['scale'], m['opacity'], out=out,
                               status_host=status_host)
 
+    def _settings(self, cal, b, r):
+        cam = np.concatenate([cal[k][b, r].reshape(-1) for k in ('world_view_transform', 'full_proj_transform',
+                                                                  'camera_center')]).tolist()
+        return novel_settings(self.H, self.W, cal['FovX'][b, r], cal['FovY'][b, r], self.bg, cam)
+
     def _render_exact(self, settings, b, out):
         """Exact entry point (one host sync, radix fallback for over-long tile lists) for one view of sample b."""
         if self.mode == 'compact':
             f = self.flat[b]
-            exact_forward(settings, f['xyz'], f['rgb'], f['opacity'], f['scale'], f['rot'], self.H, self.W, out=out)
+            radii = torch.empty((f['xyz'].shape[0],), dtype=torch.int32, device=self.dev)
+            _lib.rasterize_forward(settings, out, radii, f['xyz'], f['opacity'], colors_precomp=f['rgb'],
+                                   scales=f['scale'], rotations=f['rot'])
         else:
-            from .GaussianRender import _RasterizeMaps
             m = self.maps[b]
             args = []
             for v in range(2):
                 args += [m['valid'][v], m['xyz'][v], m['img'][v], m['rot'][v], m['scale'][v], m['opacity'][v]]
             with torch.no_grad():
-                out.copy_(_RasterizeMaps.apply(settings, *args))
+                out.copy_(_RasterizeMaps.apply([settings], *args)[0])
 
     def render(self, ratios, out=None, check=True):
         ratios = [float(r) for r in ratios]
@@ -127,7 +118,7 @@ class NovelViewRenderer:
         for k, (b, r) in enumerate(jobs):
             j = k % self.n_streams
             with torch.cuda.stream(self.streams[j]):
-                self._enqueue(self.rast[j], _settings(cal, b, r, self.H, self.W, self.bg), b, out[b, r], status[k])
+                self._enqueue(self.rast[j], self._settings(cal, b, r), b, out[b, r], status[k])
         for s in self.streams:
             cur.wait_stream(s)
         self.last_status = status
@@ -142,7 +133,7 @@ class NovelViewRenderer:
             n_pairs, max_tile, overflow = (int(v) for v in status[k, :3].tolist())
             if not overflow:
                 continue
-            settings = _settings(cal, b, r, self.H, self.W, self.bg)
+            settings = self._settings(cal, b, r)
             if max_tile > _MAX_TILE_SORT:
                 self._render_exact(settings, b, out[b, r])
                 continue

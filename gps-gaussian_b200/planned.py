@@ -17,34 +17,9 @@ from . import _lib
 from .introspect import make_settings
 
 
-def exact_forward(settings, means3D, colors, opacity, scales, rots, height, width, out=None):
-    """One forward through the exact (one host sync, allocator callbacks) entry point `gpsg_rasterize_forward` -- the path
-    that handles ANY scene, incl. tile lists longer than the in-CTA sort (global radix fallback).  Used by the sync-free
-    front ends when a view cannot be rendered from caller-owned buffers.  Returns the [3,H,W] image."""
-    dev = means3D.device
-    idx = dev.index if dev.index is not None else torch.cuda.current_device()
-    P = int(means3D.shape[0])
-    color = out if out is not None else torch.empty((3, int(height), int(width)), dtype=torch.float32, device=dev)
-    radii = torch.empty((max(P, 1),), dtype=torch.int32, device=dev)
-    n = C.c_int32(0)
-    p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-    _lib.begin_alloc(dev)
-    try:
-        with torch.cuda.device(dev):
-            rc = _lib.lib.gpsg_rasterize_forward(
-                C.byref(settings), idx, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream), P, 0, p(means3D), p(colors),
-                None, p(opacity), p(scales), p(rots), None, p(color), p(radii), _lib.ALLOC_CB, C.c_void_p(1), _lib.ALLOC_CB,
-                C.c_void_p(2), _lib.ALLOC_CB, C.c_void_p(3), C.byref(n))
-    finally:
-        _lib.end_alloc()
-    _lib.check(rc, "gpsg_rasterize_forward")
-    return color
-
-
 class PlannedRasterizer:
     def __init__(self, P, height, width, capacity_pairs, device="cuda"):
-        self.dev = torch.device(device)
-        self.idx = self.dev.index if self.dev.index is not None else torch.cuda.current_device()
+        self.dev = torch.device("cuda", _lib.device_stream(device)[0])
         self.P, self.H, self.W = int(P), int(height), int(width)
         new = lambda n: torch.empty(int(n), dtype=torch.uint8, device=self.dev)
         self.geom = new(_lib.lib.gpsg_raster_geom_bytes(self.P))
@@ -72,7 +47,7 @@ class PlannedRasterizer:
             raise ValueError(f"PlannedRasterizer scratch holds P<={self.P}, got {P}")
         color = self.color if out is None else out
         rc = _lib.lib.gpsg_rasterize_forward_planned(
-            C.byref(settings), self.idx, C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream), P, p(means3D),
+            C.byref(settings), *_lib.device_stream(self.dev), P, p(means3D),
             p(colors), p(opacity), p(scales), p(rots), p(cov3D_precomp), p(color), p(self.radii), p(self.geom),
             p(self.binning), self.capacity, p(self.image),
             C.c_void_p((self.status_host if status_host is None else status_host).data_ptr()))
@@ -91,7 +66,7 @@ class PlannedRasterizer:
         pp = lambda ts: (C.c_void_p * 2)(*[t.data_ptr() for t in ts])
         color = self.color if out is None else out
         rc = _lib.lib.gpsg_rasterize_forward_maps_planned(
-            C.byref(settings), self.idx, C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream), S2, pp(valid), pp(xyz),
+            C.byref(settings), *_lib.device_stream(self.dev), S2, pp(valid), pp(xyz),
             pp(img), pp(rot), pp(scale), pp(opacity), C.c_void_p(color.data_ptr()), C.c_void_p(self.radii.data_ptr()),
             C.c_void_p(self.geom.data_ptr()), C.c_void_p(self.binning.data_ptr()), self.capacity,
             C.c_void_p(self.image.data_ptr()),

@@ -22,29 +22,28 @@ class _Unproject(torch.autograd.Function):
         depth = torch.empty((B, 1, S, S), dtype=torch.float32, device=dev)
         xyz = torch.empty((B, S * S, 3), dtype=torch.float32, device=dev)
         valid = torch.empty((B, S * S), dtype=torch.bool, device=dev)
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
         p = lambda t: C.c_void_p(t.data_ptr())
         with torch.cuda.device(dev):
-            rc = _lib.lib.gpsg_unproject_forward(idx, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream), B, S, p(flow),
+            rc = _lib.lib.gpsg_unproject_forward(*_lib.device_stream(dev), B, S, p(flow),
                                                  p(m), int(m.stride(0)), p(K), p(E), int(E.shape[-2]), p(Kr), p(tf),
                                                  p(depth), p(xyz), p(valid))
         _lib.check(rc, "gpsg_unproject_forward")
         ctx.save_for_backward(depth, m, K, E, Kr, tf)
-        ctx.meta = (B, S, idx)
+        ctx.meta = (B, S)
         ctx.mark_non_differentiable(valid)
         return depth, xyz, valid
 
     @staticmethod
     def backward(ctx, g_depth, g_xyz, _g_valid):
         depth, m, K, E, Kr, tf = ctx.saved_tensors
-        B, S, idx = ctx.meta
+        B, S = ctx.meta
         dev = depth.device
         gx = g_xyz.detach().to(torch.float32).contiguous() if g_xyz is not None else None
         gd = g_depth.detach().to(torch.float32).contiguous() if g_depth is not None else None
         dflow = torch.empty((B, 1, S, S), dtype=torch.float32, device=dev)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
         with torch.cuda.device(dev):
-            rc = _lib.lib.gpsg_unproject_backward(idx, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream), B, S, p(depth),
+            rc = _lib.lib.gpsg_unproject_backward(*_lib.device_stream(dev), B, S, p(depth),
                                                   p(m), int(m.stride(0)), p(K), p(E), int(E.shape[-2]), p(Kr), p(tf),
                                                   p(gx), p(gd), p(dflow))
         _lib.check(rc, "gpsg_unproject_backward")

@@ -113,21 +113,15 @@ GPSG_API int gpsg_rasterize_backward(const GpsgRasterSettings* settings, int dev
  * pixel-aligned maps into [P,k] tensors, the maps are read in place: per view v in {0,1} (lmain, rmain), with S2 =
  * pixels_per_view:  valid[v][S2] (uint8/bool), xyz[v][S2,3], img[v][3,S2] in [-1,1] (colour = img*0.5+0.5),
  * rot[v][4,S2], scale[v][3,S2], opacity[v][1,S2].  Gaussian index = v*S2 + pixel; invalid pixels are culled.
- * radii has 2*S2 entries.  Results (image, and gradients in map layout) equal the gather+render path. */
-GPSG_API int gpsg_rasterize_forward_maps(const GpsgRasterSettings* settings, int device, void* stream, int pixels_per_view,
-                                         const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                         const float* const* rot, const float* const* scale, const float* const* opacity,
-                                         float* out_color, int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
-                                         gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
-                                         void* image_user, int32_t* num_rendered);
-/* gpsg_rasterize_forward_maps in two halves, for a BATCH of samples with ONE host synchronisation (reference
+ * radii has 2*S2 entries.  Results (image, and gradients in map layout) equal the gather+render path.
+ * The exact forward comes in two halves, so that a BATCH of samples needs ONE host synchronisation (reference
  * lib/GaussianRender.py:8 loops over the samples; upstream synchronises once per sample to read num_rendered):
  *   _begin : projection, pairs-per-tile counts, tile ranges; allocates the geometry and image buffers through the callbacks
  *            (the caller keeps the pointers they returned) and enqueues a copy of 6 status words into `totals_host`
  *            (pinned host memory).  Does NOT synchronise.
  *   ... the caller synchronises `stream` once after the _begin calls of all samples ...
  *   _finish: sizes and allocates the binning buffer from totals_host, bins, sorts, composites into out_color.
- * Results are identical to gpsg_rasterize_forward_maps; the saved buffers feed gpsg_rasterize_backward_maps unchanged. */
+ * A batch of one is begin, one synchronisation, finish.  The saved buffers feed gpsg_rasterize_backward_maps. */
 GPSG_API int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* settings, int device, void* stream, int pixels_per_view,
                                                const uint8_t* const* valid, const float* const* xyz, const float* const* img,
                                                const float* const* rot, const float* const* scale,
@@ -141,7 +135,7 @@ GPSG_API int gpsg_rasterize_forward_maps_finish(const GpsgRasterSettings* settin
                                                 void* geom_buffer, void* image_buffer, gpsg_alloc_fn binning_alloc,
                                                 void* binning_user, const uint32_t* totals_host, int32_t* num_rendered);
 
-/* sync-free form of gpsg_rasterize_forward_maps (same contract as gpsg_rasterize_forward_planned; geom buffer sized for
+/* sync-free form of the map-ingest forward (same contract as gpsg_rasterize_forward_planned; geom buffer sized for
  * P = 2*pixels_per_view): the serving loop of test_view_interp.py:39-47 renders many novel cameras from ONE pair's
  * cached maps without gathering them and without a host sync. */
 GPSG_API int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* settings, int device, void* stream,

@@ -520,14 +520,28 @@ def test_pts2render_batch_of_two_and_host_pipeline():
 
 
 def test_batched_pts2render_one_sync_matches_per_sample_path():
-    """pts2render on a batch of two = `_RasterizeMapsBatch` (begin x2 -> ONE stream synchronise -> finish x2): images and map
-    gradients equal the single-sample path (`_RasterizeMaps`, one synchronisation per sample) run on each sample alone."""
+    """pts2render on a batch of two (`_RasterizeMaps`: begin x2 -> ONE stream synchronise -> finish x2): images and map
+    gradients equal two batch-of-one calls of the same Function, one per sample, each with exactly one synchronisation."""
     from gps_gaussian_b200.GaussianRender import pts2render
     res = 96
     keys = ("xyz", "img", "rot_maps", "scale_maps", "opacity_maps")
     g = torch.randn(2, 3, res, res, device="cuda", generator=torch.Generator("cuda").manual_seed(5))
+    syncs = []
+    orig = torch.cuda.Stream.synchronize
+
+    def counting_syncs(d):
+        syncs.clear()
+        torch.cuda.Stream.synchronize = lambda self: (syncs.append(1), orig(self))[1]
+        try:
+            return pts2render(d, [0.1, 0.2, 0.3])["novel_view"]["img_pred"]
+        finally:
+            torch.cuda.Stream.synchronize = orig
+
     singles = [_stereo_data(res, requires_grad=True, seed=sd)[1] for sd in (11, 12)]
-    outs = [pts2render(d, [0.1, 0.2, 0.3])["novel_view"]["img_pred"] for d in singles]
+    outs = []
+    for d in singles:
+        outs.append(counting_syncs(d))
+        assert len(syncs) == 1                                               # one host synchronisation for a batch of one
     for i, o in enumerate(outs):
         (o * g[i:i + 1]).sum().backward()
     d0, d1 = (_stereo_data(res, seed=sd)[1] for sd in (11, 12))
@@ -536,13 +550,7 @@ def test_batched_pts2render_one_sync_matches_per_sample_path():
         batch[v] = {k: torch.cat([d0[v][k], d1[v][k]]) for k in d0[v]}
         for k in keys:
             batch[v][k].requires_grad_(True)
-    syncs = []
-    orig = torch.cuda.Stream.synchronize
-    torch.cuda.Stream.synchronize = lambda self: (syncs.append(1), orig(self))[1]
-    try:
-        out = pts2render(batch, [0.1, 0.2, 0.3])["novel_view"]["img_pred"]
-    finally:
-        torch.cuda.Stream.synchronize = orig
+    out = counting_syncs(batch)
     assert len(syncs) == 1                                                   # one host synchronisation for the batch
     assert torch.equal(out[0:1], outs[0]) and torch.equal(out[1:2], outs[1])
     (out * g).sum().backward()
