@@ -388,6 +388,8 @@ static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaS
     GeomState g = GeomState::carve(geom_buffer, P, 0);
     ImageState im = ImageState::carve(image_buffer, cam.W, cam.H);
     BinningState b = BinningState::carve(binning_buffer, (size_t)capacity_pairs, 0);
+    b.keys = nullptr;   // compositing and backward read only the slabs: the tile sort skips the sorted keys / point list
+    b.vals = nullptr;
     int rc = GPSG_OK;
     GPSG_CUDA(cudaMemsetAsync(im.tile_count, 0, (size_t)((char*)(im.totals + 64) - (char*)im.tile_count), stream));
     { StageTimer t(ST_PREPROCESS, stream, 1); rc = launch_preprocess(cam, P, src, radii, g, im, (uint32_t)capacity_pairs, stream); }

@@ -152,7 +152,7 @@ int run_sort(BinningState b, size_t N, int end_bit, cudaStream_t stream);
 int launch_gather_ranges(const Camera& cam, size_t N, const GaussianSrc& src, GeomState g, BinningState b, ImageState im,
                          cudaStream_t stream);
 // tile-bucket path (default): counts -> ranges, bucket scatter, per-tile in-CTA sort fused with the slab gather
-constexpr uint32_t kMaxTileSort = 4096;  // largest tile list the in-CTA sort handles (256 thr x 16 keys); beyond: radix path
+constexpr uint32_t kMaxTileSort = 4096;  // largest tile list the in-CTA sort handles (512 thr x 8 keys); beyond: radix path
 int launch_tile_scan(const Camera& cam, ImageState im, uint32_t capacity /*0 = unbounded*/, cudaStream_t stream);
 int launch_bucket_scatter(const Camera& cam, int P, const int32_t* radii, GeomState g, BinningState b, ImageState im,
                           cudaStream_t stream);

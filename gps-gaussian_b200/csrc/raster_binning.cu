@@ -183,64 +183,68 @@ __device__ __forceinline__ void slab_entry(uint32_t id, const GaussianSrc& src, 
     C = make_float4(r, gg, bb, __uint_as_float(id));
 }
 
-// one CTA per tile: radix sort of the tile's bucket inside the CTA (cub::BlockRadixSort, keys in registers) on
-// (depth bits << 32 | id), then the sorted point list, keys and parameter slabs are written coalesced -- the sort
+// one CTA per tile: radix sort of the tile's bucket inside the CTA (cub::BlockRadixSort, keys in registers), then the
+// parameter slabs (and, on the exact entry point, the sorted keys and point list) are written coalesced -- the sort
 // and the gather never round-trip to HBM.  The CTA picks the smallest items-per-thread variant that fits.
+// 512 threads: a 2048-entry tile needs only 4 keys + 4 ids per thread, so three CTAs (1536 threads, 40 registers)
+// fit per SM without spills.  Not memoising cub's outer scan and keeping the fix-up and gather loops rolled is what
+// keeps the kernel inside 40 registers.
+constexpr int kSortThreads = 512;
+constexpr int kSortCTAsPerSM = 3;
+constexpr int kBigItems = (int)kMaxTileSort / kSortThreads;   // big-tile kernel: 8 keys per thread
 template <int ITEMS>
 struct TileSort {
-    using BRS = cub::BlockRadixSort<unsigned long long, 256, ITEMS>;
+    // 32-bit keys (the tile's depth window) carrying the 32-bit Gaussian id
+    using BRS = cub::BlockRadixSort<uint32_t, kSortThreads, ITEMS, uint32_t, 4, /*MEMOIZE_OUTER_SCAN=*/false>;
     union Smem {
         typename BRS::TempStorage sort;
-        unsigned long long keys[256 * ITEMS];   // sorted keys, for the equal-depth fix-up
+        unsigned long long keys[kSortThreads * ITEMS];   // sorted (depth bits << 32 | id), for the equal-depth fix-up
     };
 
-    // Sorts the tile's (depth bits << 32 | id) keys and writes point list, keys and slabs.
-    //  * only the depth bits that differ inside the tile are radix-sorted (block-wide min/max of the keys);
-    //  * the Gaussian id (low word) is NOT radix-sorted: equal-depth runs -- the only place it matters -- are found
-    //    after the sort and ordered by id in shared memory.  A run longer than kMaxRun falls back to the full
-    //    (id + depth) radix sort, so degenerate inputs (thousands of identical depths) stay correct and bounded.
+    // Sorts the tile's entries in (depth bits << 32 | id) order and writes slabs (+ keys and point list if b.keys).
+    //  * only the depth window is radix-sorted: 32-bit keys `depth bits - tile minimum`, whose width is the bit length
+    //    of the tile's depth span (block-wide min/max; about 20 bits on real scenes, at most 31 as depth > 0);
+    //  * the Gaussian id rides along as the value and is NOT radix-sorted: equal-depth runs -- the only place it
+    //    matters -- are found after the sort and ordered by id in shared memory.  A run longer than kMaxRun falls back
+    //    to the full (id, then depth) LSD radix sort, so degenerate inputs (thousands of identical depths) stay correct
+    //    and bounded.
     static constexpr int kMaxRun = 16;
-    __device__ static void run(Smem& sm, int* flags, const unsigned long long* __restrict__ src, int n, int id_bits,
-                               uint32_t tile, size_t out0, const GaussianSrc& src_in, const GeomState& g,
-                               const BinningState& b) {
-        unsigned long long keys[ITEMS];
-        unsigned long long kmin = ~0ull, kmax = 0ull;
+    __device__ static void run(Smem& sm, uint32_t* flags, const uint2* __restrict__ src, int n, int id_bits, uint32_t tile,
+                               size_t out0, const GaussianSrc& src_in, const GeomState& g, const BinningState& b) {
+        uint32_t keys[ITEMS], ids[ITEMS];
+        uint32_t dmin = ~0u, dmax = 0u;
 #pragma unroll
-        for (int k = 0; k < ITEMS; ++k) {       // any input arrangement is fine: the keys are unique
-            const int i = k * 256 + (int)threadIdx.x;
-            keys[k] = i < n ? src[i] : ~0ull;
-            if (i < n) { kmin = min(kmin, keys[k]); kmax = max(kmax, keys[k]); }
+        for (int k = 0; k < ITEMS; ++k) {       // any input arrangement is fine: the bucket order is arbitrary
+            const int i = k * kSortThreads + (int)threadIdx.x;
+            const uint2 e = i < n ? src[i] : make_uint2(0u, 0u);   // (id, depth bits)
+            ids[k] = e.x;
+            keys[k] = e.y;
+            if (i < n) { dmin = min(dmin, e.y); dmax = max(dmax, e.y); }
         }
-        // block-wide min / max of the depth words -> highest differing depth bit
-        uint32_t dmin = (uint32_t)(kmin >> 32), dmax = (uint32_t)(kmax >> 32);
         dmin = __reduce_min_sync(0xffffffffu, dmin);
         dmax = __reduce_max_sync(0xffffffffu, dmax);
-        if (threadIdx.x == 0) { flags[0] = 0x7fffffff; flags[1] = 0; flags[2] = 0; }
+        if (threadIdx.x == 0) { flags[0] = ~0u; flags[1] = 0u; flags[2] = 0u; }
         __syncthreads();
-        if ((threadIdx.x & 31) == 0) { atomicMin(&flags[0], (int)(dmin >> 1)); atomicMax(&flags[1], (int)(dmax >> 1)); }
+        if ((threadIdx.x & 31) == 0) { atomicMin(&flags[0], dmin); atomicMax(&flags[1], dmax); }
         __syncthreads();
-        // Keys are re-based on the tile's smallest depth word so that only bit_length(max - min) depth bits need
-        // sorting; padding keys get the next higher bit, i.e. they are strictly greater than every real key inside
-        // the sorted window (with un-rebased keys a real key with an all-ones window would tie with the padding).
-        const uint32_t dlo = (uint32_t)flags[0] << 1;                              // <= true min (low bit dropped)
-        const uint32_t span = (((uint32_t)flags[1] << 1) | 1u) - dlo;              // >= true max - dlo
-        const int w = 32 - __clz(span);                                            // 1..32 (depth < 2^31 => w <= 31)
-        const unsigned long long base = (unsigned long long)dlo << 32;
-        const unsigned long long pad = 1ull << (32 + w);
+        // Keys are re-based on the tile's smallest depth word so that only w = bit_length(max - min) bits need sorting;
+        // padding keys get bit w, i.e. they are strictly greater than every real key and end up at ranks >= n.
+        const uint32_t dlo = flags[0];
+        const int w = 32 - __clz(flags[1] - dlo);                                  // 0..31 (depth bits < 2^31)
+        const uint32_t pad = 1u << w;
 #pragma unroll
-        for (int k = 0; k < ITEMS; ++k) keys[k] = (k * 256 + (int)threadIdx.x) < n ? keys[k] - base : pad;
-        BRS(sm.sort).SortBlockedToStriped(keys, 32, 32 + w + 1);
-#pragma unroll
-        for (int k = 0; k < ITEMS; ++k) keys[k] += base;                            // (padding ranks >= n are never read)
+        for (int k = 0; k < ITEMS; ++k) keys[k] = (k * kSortThreads + (int)threadIdx.x) < n ? keys[k] - dlo : pad;
+        BRS(sm.sort).SortBlockedToStriped(keys, ids, 0, w + 1);
         __syncthreads();
         // ---- equal-depth runs: order by id ----
 #pragma unroll
-        for (int k = 0; k < ITEMS; ++k) sm.keys[k * 256 + (int)threadIdx.x] = keys[k];   // rank r = k*256 + tid
+        for (int k = 0; k < ITEMS; ++k)                                             // rank r = k*kSortThreads + tid
+            sm.keys[k * kSortThreads + (int)threadIdx.x] = ((unsigned long long)(keys[k] + dlo) << 32) | ids[k];
         __syncthreads();
         bool redo = false;
-#pragma unroll
+#pragma unroll 1
         for (int k = 0; k < ITEMS; ++k) {
-            const int r = k * 256 + (int)threadIdx.x;
+            const int r = k * kSortThreads + (int)threadIdx.x;
             if (r + 1 < n) {
                 const uint32_t d = (uint32_t)(sm.keys[r] >> 32);
                 const bool start = (r == 0 || (uint32_t)(sm.keys[r - 1] >> 32) != d) && (uint32_t)(sm.keys[r + 1] >> 32) == d;
@@ -258,31 +262,52 @@ struct TileSort {
                 }
             }
         }
-        if (redo) flags[2] = 1;
+        if (redo) flags[2] = 1u;
         __syncthreads();
-        if (flags[2]) {   // degenerate tile: full LSD radix sort, id digits first, then all depth digits
+        if (flags[2]) {   // degenerate tile: full LSD radix sort, by id first, then (stably) by the depth window
 #pragma unroll
-            for (int k = 0; k < ITEMS; ++k) {
-                const int i = k * 256 + (int)threadIdx.x;
-                keys[k] = i < n ? src[i] : ~0ull;
+            for (int k = 0; k < ITEMS; ++k) {   // sm.keys still holds every entry (the fix-up only permutes runs)
+                const int r = k * kSortThreads + (int)threadIdx.x;
+                const unsigned long long v = sm.keys[r];
+                ids[k] = (uint32_t)v;
+                keys[k] = r < n ? (uint32_t)(v >> 32) - dlo : pad;
             }
             __syncthreads();
-            BRS(sm.sort).Sort(keys, 0, id_bits);
+            BRS(sm.sort).SortBlockedToStriped(ids, keys, 0, id_bits);
             __syncthreads();
-            BRS(sm.sort).SortBlockedToStriped(keys, 32, 64);
-        } else {
+            // striped -> blocked through shared memory, so that the depth pass sees the id order (LSD stability).
+            // The one sort instantiation serves both passes: a blocked-output Sort() would need more registers.
 #pragma unroll
-            for (int k = 0; k < ITEMS; ++k) keys[k] = sm.keys[k * 256 + (int)threadIdx.x];
+            for (int k = 0; k < ITEMS; ++k)
+                sm.keys[k * kSortThreads + (int)threadIdx.x] = ((unsigned long long)keys[k] << 32) | ids[k];
+            __syncthreads();
+#pragma unroll
+            for (int k = 0; k < ITEMS; ++k) {
+                const unsigned long long v = sm.keys[(int)threadIdx.x * ITEMS + k];
+                ids[k] = (uint32_t)v;
+                keys[k] = (uint32_t)(v >> 32);
+            }
+            __syncthreads();
+            BRS(sm.sort).SortBlockedToStriped(keys, ids, 0, w + 1);
+            __syncthreads();
+#pragma unroll
+            for (int k = 0; k < ITEMS; ++k)
+                sm.keys[k * kSortThreads + (int)threadIdx.x] = ((unsigned long long)(keys[k] + dlo) << 32) | ids[k];
+            __syncthreads();
         }
+        // ---- gather: each thread takes ranks tid, tid + kSortThreads, ... so every store below is coalesced ----
         const unsigned long long tile_hi = (unsigned long long)tile << 32;
-#pragma unroll
+#pragma unroll 1
         for (int k = 0; k < ITEMS; ++k) {
-            const int r = k * 256 + (int)threadIdx.x;
+            const int r = k * kSortThreads + (int)threadIdx.x;
             if (r < n) {
-                const uint32_t id = (uint32_t)keys[k];
+                const unsigned long long v = sm.keys[r];
+                const uint32_t id = (uint32_t)v;
                 const size_t o = out0 + r;
-                b.keys[o] = tile_hi | (keys[k] >> 32);
-                b.vals[o] = id;
+                if (b.keys) {   // the exact entry point keeps them for introspection; the planned one passes NULL
+                    b.keys[o] = tile_hi | (v >> 32);
+                    b.vals[o] = id;
+                }
                 float4 A, B, C;
                 slab_entry(id, src_in, g, A, B, C);
                 b.slabA[o] = A;
@@ -293,40 +318,42 @@ struct TileSort {
     }
 };
 
-// BIG = false: one CTA per tile, tiles with n <= 2048 (2/4/8 keys per thread).  BIG = true: a small persistent grid
-// that walks the list of big tiles (2048 < n <= 4096) built by the tile scan -- it costs ~nothing when the list is
-// empty, so the planned (sync-free) path can always launch it.  Two kernels so that the common case is not held at
-// the register / shared-memory footprint of the rare one.
+// BIG = false: one CTA per tile, tiles with n <= 2048 (1/2/3/4 keys per thread; real scenes put most busy tiles
+// between 1025 and 1536 entries).  BIG = true: a small persistent grid that walks the list of big tiles
+// (2048 < n <= 4096) built by the tile scan -- it costs ~nothing when the list is empty, so the planned (sync-free)
+// path can always launch it.  Two kernels so that the common case is not held at the register / shared-memory
+// footprint of the rare one.
 template <bool BIG>
-__global__ void __launch_bounds__(256, BIG ? 1 : 4) tile_sort_gather_kernel(const GaussianSrc colors, GeomState g,
+__global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_sort_gather_kernel(const GaussianSrc colors, GeomState g,
                                                                             BinningState b, ImageState im, int id_bits) {
-    __shared__ int flags[4];
+    __shared__ uint32_t flags[4];
     if (im.totals[2]) return;                   // planned mode overflow
     if constexpr (BIG) {
-        __shared__ typename TileSort<16>::Smem t16;
+        __shared__ typename TileSort<kBigItems>::Smem t16;
         const uint32_t nbig = im.totals[3];
         for (uint32_t k = blockIdx.x; k < nbig; k += gridDim.x) {
             const uint32_t tile = im.big_tiles[k];
             const uint2 range = im.ranges[tile];
             const int n = (int)(range.y - range.x);
-            const unsigned long long* __restrict__ src = reinterpret_cast<const unsigned long long*>(b.bucket) + range.x;
-            TileSort<16>::run(t16, flags, src, n, id_bits, tile, range.x, colors, g, b);
+            TileSort<kBigItems>::run(t16, flags, b.bucket + range.x, n, id_bits, tile, range.x, colors, g, b);
             __syncthreads();
         }
     } else {
         __shared__ union {
+            typename TileSort<1>::Smem t1;
             typename TileSort<2>::Smem t2;
+            typename TileSort<3>::Smem t3;
             typename TileSort<4>::Smem t4;
-            typename TileSort<8>::Smem t8;
         } temp;
-        const uint32_t tile = im.tile_order[blockIdx.x];       // longest lists first: the ~2.4 waves of very unequal CTAs pack better
+        const uint32_t tile = im.tile_order[blockIdx.x];       // longest lists first: the last wave holds the short ones
         const uint2 range = im.ranges[tile];
         const int n = (int)(range.y - range.x);
         if (n == 0 || n > (int)kBigTile) return;
-        const unsigned long long* __restrict__ src = reinterpret_cast<const unsigned long long*>(b.bucket) + range.x;
-        if (n <= 512) TileSort<2>::run(temp.t2, flags, src, n, id_bits, tile, range.x, colors, g, b);
-        else if (n <= 1024) TileSort<4>::run(temp.t4, flags, src, n, id_bits, tile, range.x, colors, g, b);
-        else TileSort<8>::run(temp.t8, flags, src, n, id_bits, tile, range.x, colors, g, b);
+        const uint2* __restrict__ src = b.bucket + range.x;
+        if (n <= 512) TileSort<1>::run(temp.t1, flags, src, n, id_bits, tile, range.x, colors, g, b);
+        else if (n <= 1024) TileSort<2>::run(temp.t2, flags, src, n, id_bits, tile, range.x, colors, g, b);
+        else if (n <= 1536) TileSort<3>::run(temp.t3, flags, src, n, id_bits, tile, range.x, colors, g, b);
+        else TileSort<4>::run(temp.t4, flags, src, n, id_bits, tile, range.x, colors, g, b);
     }
 }
 
@@ -337,10 +364,10 @@ int launch_tile_sort_gather(const Camera& cam, int P, uint32_t max_count, const 
     int id_bits = 1;
     while (id_bits < 32 && (1ll << id_bits) < (long long)P) ++id_bits;
     const int tiles = cam.grid_x * cam.grid_y;
-    tile_sort_gather_kernel<false><<<tiles, 256, 0, stream>>>(colors, g, b, im, id_bits);
+    tile_sort_gather_kernel<false><<<tiles, kSortThreads, 0, stream>>>(colors, g, b, im, id_bits);
     GPSG_LAUNCH_CHECK();
     if (max_count > kBigTile) {   // exact mode passes the real maximum; planned mode passes kMaxTileSort (always launch)
-        tile_sort_gather_kernel<true><<<min(tiles, kBigTileCTAs), 256, 0, stream>>>(colors, g, b, im, id_bits);
+        tile_sort_gather_kernel<true><<<min(tiles, kBigTileCTAs), kSortThreads, 0, stream>>>(colors, g, b, im, id_bits);
         GPSG_LAUNCH_CHECK();
     }
     return GPSG_OK;
