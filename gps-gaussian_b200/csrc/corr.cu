@@ -34,6 +34,13 @@ template <typename T> __device__ __forceinline__ void st_f(T* p, float v);
 template <> __device__ __forceinline__ void st_f<float>(float* p, float v) { *p = v; }
 template <> __device__ __forceinline__ void st_f<__half>(__half* p, float v) { *p = __float2half_rn(v); }
 
+// floor(x) as an int, clamped to [-r-2, W2+r].  Outside that range the taps xf-r .. xf+r+1 all lie outside [0, W2) (and
+// in the backward no x1 in [0, W2) falls in the window), so the clamp changes no output; it keeps the conversion and
+// xf +- r defined where floorf(x) is past 2^31 or NaN.  dx is still taken from the unclamped floor.
+__device__ __forceinline__ int window_floor(float fl, int r, int W2) {
+    return (int)fminf(fmaxf(fl, (float)(-r - 2)), (float)(W2 + r));
+}
+
 // thread = (n, y, x); reads 2r+2 consecutive taps of its volume row, writes 2r+1 outputs (coalesced over x).
 template <typename T, int R>
 __global__ void __launch_bounds__(256) corr_fwd_kernel(int B, int H, int W1, int W2, const T* __restrict__ vol,
@@ -51,7 +58,7 @@ __global__ void __launch_bounds__(256) corr_fwd_kernel(int B, int H, int W1, int
     const float x0 = coords[n * csb + (int64_t)y * W1 + x];
     const float fl = floorf(x0);
     const float dx = x0 - fl;
-    const int xf = (int)fl;
+    const int xf = window_floor(fl, r, W2);
     const T* row = vol + n * sb + y * sh + x * sw1;
     float prev = 0.f;  // tap i-1
     {
@@ -89,7 +96,7 @@ __global__ void __launch_bounds__(256) corr_bwd_kernel(int B, int H, int W1, int
     const float x0 = coords[n * csb + (int64_t)y * W1 + x];
     const float fl = floorf(x0);
     const float dx = x0 - fl;
-    const int xf = (int)fl;
+    const int xf = window_floor(fl, r, W2);
     const int64_t plane = (int64_t)H * W1;
     const T* go = gout + (int64_t)n * rd * plane + (int64_t)y * W1 + x;
     T* row = gvol + rowi * W2;
@@ -274,8 +281,8 @@ __global__ void __launch_bounds__(256) corr_lookup_fwd_kernel(int B, int H, int 
         const float x0 = c0 * scale;                                  // == coords / 2**l exactly (power of two)
         const float fl = floorf(x0);
         const float dx = x0 - fl;
-        const int xf = (int)fl;
         const int W2 = pyr.w[l];
+        const int xf = window_floor(fl, r, W2);
         const T* row = reinterpret_cast<const T*>(pyr.v[l]) + idx * W2;
         float prev = 0.f;
         { const int x1 = xf - r; if (x1 >= 0 && x1 < W2) prev = ld_f<T>(row + x1); }
@@ -309,8 +316,8 @@ __global__ void __launch_bounds__(256) corr_lookup_bwd_kernel(int B, int H, int 
     const float x0 = coords[n * csb + (int64_t)y * W1 + x] * (1.0f / (float)(1 << l));
     const float fl = floorf(x0);
     const float dx = x0 - fl;
-    const int xf = (int)fl;
     const int W2 = gp.w[l];
+    const int xf = window_floor(fl, r, W2);
     const int64_t plane = (int64_t)H * W1;
     const T* go = gout + ((int64_t)n * levels + l) * rd * plane + (int64_t)y * W1 + x;
     T* row = reinterpret_cast<T*>(gp.v[l]) + rowi * W2;

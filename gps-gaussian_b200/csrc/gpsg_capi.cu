@@ -577,7 +577,8 @@ int gpsg_corr_sampler_forward(int device, void* stream_, int dtype, int B, int H
     GPSG_REQUIRE(dtype == 0 || dtype == 1, "dtype must be 0 (fp32) or 1 (fp16)");
     GPSG_REQUIRE(B >= 0 && H >= 0 && W1 >= 0 && W2 >= 0 && radius >= 0 && radius <= 31, "bad shape / radius");
     if ((int64_t)B * H * W1 == 0) return GPSG_OK;
-    GPSG_REQUIRE(volume && coords && out, "NULL pointer");
+    // a volume of width 0 (a pooled level of rows narrower than 2^l) has no storage and no taps: every output is 0
+    GPSG_REQUIRE((volume || W2 == 0) && coords && out, "NULL pointer");
     GPSG_CUDA(cudaSetDevice(device));
     StageTimer t(ST_CORR_FWD, (cudaStream_t)stream_, 1);
     return launch_corr_fwd(dtype, B, H, W1, W2, volume, sb, sh, sw1, coords, coords_sb, radius, out,
