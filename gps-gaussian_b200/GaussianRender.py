@@ -104,21 +104,23 @@ class _RasterizeMaps(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         grads = [None]
+        flags = _lib.backward_flags()
         dev = grad_out.device
         idx, sptr = _lib.device_stream(dev)
         for b, p in enumerate(ctx.per):
             new = lambda ref: [torch.empty_like(ref[0]), torch.empty_like(ref[1])]
             dxyz, dimg, drot, dscale, dopac = (new(t) for t in p["tensors"][1:])
-            ws = torch.empty(int(_lib.lib.gpsg_rasterize_backward_maps_workspace_bytes(p["S2"])), dtype=torch.uint8, device=dev)
+            ws = torch.empty(int(_lib.lib.gpsg_rasterize_backward_maps_workspace_bytes_ex(p["S2"], p["n"], flags)),
+                             dtype=torch.uint8, device=dev)
             g = _f32(grad_out[b].detach())
             geom, binning, image = p["bufs"]
             with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_rasterize_backward_maps(
+                rc = _lib.lib.gpsg_rasterize_backward_maps_ex(
                     C.byref(ctx.settings_list[b]), idx, sptr, p["S2"], p["n"], *(_ptrs(t) for t in p["tensors"]),
                     C.c_void_p(p["radii"].data_ptr()), C.c_void_p(geom.data_ptr()), C.c_void_p(binning.data_ptr()),
                     C.c_void_p(image.data_ptr()), C.c_void_p(g.data_ptr()), _ptrs(dxyz), _ptrs(dimg), _ptrs(drot),
-                    _ptrs(dscale), _ptrs(dopac), C.c_void_p(ws.data_ptr()))
-            _lib.check(rc, "gpsg_rasterize_backward_maps")
+                    _ptrs(dscale), _ptrs(dopac), C.c_void_p(ws.data_ptr()), flags)
+            _lib.check(rc, "gpsg_rasterize_backward_maps_ex")
             sh = ctx.shapes[12 * b:12 * b + 12]
             grads += [None, dxyz[0].view(sh[1]), dimg[0].view(sh[2]), drot[0].view(sh[3]), dscale[0].view(sh[4]),
                       dopac[0].view(sh[5]), None, dxyz[1].view(sh[7]), dimg[1].view(sh[8]), drot[1].view(sh[9]),

@@ -59,6 +59,10 @@ lib.gpsg_rasterize_backward_workspace_bytes.restype = _sz
 lib.gpsg_rasterize_backward_workspace_bytes.argtypes = [_i]
 lib.gpsg_rasterize_backward.restype = _i
 lib.gpsg_rasterize_backward.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, C.c_int32] + [_vp] * 21
+lib.gpsg_rasterize_backward_workspace_bytes_ex.restype = _sz
+lib.gpsg_rasterize_backward_workspace_bytes_ex.argtypes = [_i, _i64, _i]
+lib.gpsg_rasterize_backward_ex.restype = _i
+lib.gpsg_rasterize_backward_ex.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, C.c_int32] + [_vp] * 21 + [_i]
 lib.gpsg_mark_visible.restype = _i
 lib.gpsg_mark_visible.argtypes = [_i, _vp, _i, _vp, C.POINTER(C.c_float), _vp]
 lib.gpsg_geom_view.restype = _i
@@ -97,6 +101,10 @@ lib.gpsg_rasterize_backward_maps_workspace_bytes.argtypes = [_i]
 lib.gpsg_rasterize_backward_maps.restype = _i
 lib.gpsg_rasterize_backward_maps.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, C.c_int32, _pp, _pp, _pp, _pp, _pp, _pp,
                                              _vp, _vp, _vp, _vp, _vp, _pp, _pp, _pp, _pp, _pp, _vp]
+lib.gpsg_rasterize_backward_maps_workspace_bytes_ex.restype = _sz
+lib.gpsg_rasterize_backward_maps_workspace_bytes_ex.argtypes = [_i, _i64, _i]
+lib.gpsg_rasterize_backward_maps_ex.restype = _i
+lib.gpsg_rasterize_backward_maps_ex.argtypes = lib.gpsg_rasterize_backward_maps.argtypes + [_i]
 lib.gpsg_corr_build_pyramid.restype = _i
 lib.gpsg_corr_build_pyramid.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, C.POINTER(C.c_void_p), _i]
 lib.gpsg_corr_build_backward.restype = _i
@@ -134,7 +142,10 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_rasterize_backward_maps", "gpsg_unproject_forward", "gpsg_unproject_backward", "gpsg_l1_ssim_workspace_bytes", "gpsg_l1_ssim_forward",
             "gpsg_l1_ssim_backward", "gpsg_set_corr_build", "gpsg_profile_enable",
             "gpsg_profile_read",
-            "gpsg_profile_stage_name"]
+            "gpsg_profile_stage_name", "gpsg_rasterize_backward_workspace_bytes_ex", "gpsg_rasterize_backward_ex",
+            "gpsg_rasterize_backward_maps_workspace_bytes_ex", "gpsg_rasterize_backward_maps_ex"]
+
+BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 
 
 def check(rc, what):
@@ -204,12 +215,22 @@ def rasterize_forward(settings, out_color, radii, means3D, opacities, colors_pre
     return int(n.value), (bufs.get(1), bufs.get(2), bufs.get(3))
 
 
+def backward_flags(deterministic=None):
+    """The `flags` word of the gpsg_*_backward_ex entry points.  deterministic=None follows PyTorch's switch,
+    torch.use_deterministic_algorithms(True), read when the backward runs (as PyTorch's own kernels read it); True / False
+    force the mode.  Deterministic mode gives bit-identical gradients on reruns (include/gpsg.h)."""
+    if deterministic is None:
+        deterministic = torch.are_deterministic_algorithms_enabled()
+    return BWD_DETERMINISTIC if deterministic else 0
+
+
 def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D, opacities, colors_precomp=None,
-                       shs=None, scales=None, rotations=None, cov3D_precomp=None, want_cov3D=False):
+                       shs=None, scales=None, rotations=None, cov3D_precomp=None, want_cov3D=False, deterministic=None):
     """Backward of `rasterize_forward` with the same inputs, its num_rendered, buffers and radii.  Returns the gradients
     dL_dmeans2D [P,3], dL_dcolors [P,3], dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drots [P,4],
     dL_dcov3D [P,6] and dL_dsh [P,M,3].  dL_dcolors is None on the SH path, dL_dsh is None without shs and dL_dcov3D
-    is None unless want_cov3D."""
+    is None unless want_cov3D.  `deterministic`: see `backward_flags`."""
+    flags = backward_flags(deterministic)
     dev = means3D.device
     P = int(means3D.shape[0])
     new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
@@ -217,18 +238,18 @@ def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D,
                dL_dopacity=new(P, 1), dL_dmeans3D=new(P, 3), dL_dscales=new(P, 3), dL_drots=new(P, 4),
                dL_dcov3D=new(P, 6) if want_cov3D else None,
                dL_dsh=new(P, int(shs.shape[1]), 3) if shs is not None else None)
-    ws = torch.empty(int(lib.gpsg_rasterize_backward_workspace_bytes(P)), dtype=torch.uint8, device=dev)
+    ws = torch.empty(int(lib.gpsg_rasterize_backward_workspace_bytes_ex(P, num_rendered, flags)), dtype=torch.uint8, device=dev)
     g = grad_color.detach().to(torch.float32).contiguous()
     idx, stream = device_stream(dev)
     geom, binning, image = bufs
     with torch.cuda.device(dev):
-        rc = lib.gpsg_rasterize_backward(
+        rc = lib.gpsg_rasterize_backward_ex(
             C.byref(settings), idx, stream, P, int(shs.shape[1]) if shs is not None else 0, num_rendered, _ptr(means3D),
             _ptr(colors_precomp), _ptr(shs), _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(cov3D_precomp),
             _ptr(radii), _ptr(geom), _ptr(binning), _ptr(image), _ptr(g), _ptr(out["dL_dmeans2D"]),
             _ptr(out["dL_dcolors"]), _ptr(out["dL_dopacity"]), _ptr(out["dL_dmeans3D"]), _ptr(out["dL_dcov3D"]),
-            _ptr(out["dL_dsh"]), _ptr(out["dL_dscales"]), _ptr(out["dL_drots"]), _ptr(ws))
-    check(rc, "gpsg_rasterize_backward")
+            _ptr(out["dL_dsh"]), _ptr(out["dL_dscales"]), _ptr(out["dL_drots"]), _ptr(ws), flags)
+    check(rc, "gpsg_rasterize_backward_ex")
     return out
 
 

@@ -165,7 +165,8 @@ static Profiler g_prof;
 static std::mutex g_prof_mu;
 static const char* kStageNames[ST_COUNT] = {"preprocess", "scan", "duplicate", "sort", "gather_ranges", "tile_scan",
                                             "bucket_scatter", "tile_sort_gather", "render_forward",
-                                            "render_backward", "preprocess_backward", "corr_forward", "corr_backward", "corr_build"};
+                                            "render_backward", "preprocess_backward", "corr_forward", "corr_backward", "corr_build",
+                                            "render_backward_det", "render_backward_det_reduce"};
 StageTimer::StageTimer(Stage s, cudaStream_t st, int launches) : stage(s), stream(st), slot(nullptr) {
     if (!g_prof.on) return;
     std::lock_guard<std::mutex> lk(g_prof_mu);
@@ -429,16 +430,35 @@ int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* s, int device,
                                   geom_buffer, binning_buffer, capacity_pairs, image_buffer, status_host);
 }
 
-size_t gpsg_rasterize_backward_workspace_bytes(int P) {
-    const size_t n = (size_t)(P > 0 ? P : 1);
-    return align_up(sizeof(float4) * 3 * n) + align_up(sizeof(float) * 3 * n) + 256;   // packed accumulator rows, dL_dcolors (SH path)
+// Backward workspace: [3 x float4 packed accumulator rows][3 floats: dL_dcolors (SH path) or dL_dmeans2D (maps)] per
+// Gaussian and, with GPSG_BWD_DETERMINISTIC, [mask: 1 byte per pair][partials: 8 slots x 9 floats per pair] after them
+// (raster_backward.cu): 289 B per pair plus alignment.
+static size_t bwd_base_bytes(size_t n) { return align_up(sizeof(float4) * 3 * n) + align_up(sizeof(float) * 3 * n); }
+static size_t bwd_det_mask_bytes(size_t N) { return (N + 3) / 4 * 4; }   // whole 32-bit words (atomicOr)
+static size_t bwd_det_bytes(size_t N) { return align_up(bwd_det_mask_bytes(N)) + align_up(sizeof(float) * 8 * 9 * N); }
+
+static int check_bwd_flags(int flags) {
+    GPSG_REQUIRE((flags & ~GPSG_BWD_DETERMINISTIC) == 0, "unknown backward flag bits (GPSG_BWD_DETERMINISTIC is the only flag)");
+    return GPSG_OK;
 }
+
+static size_t bwd_workspace_bytes(size_t n, size_t slack, int64_t num_rendered, int flags) {
+    if (check_bwd_flags(flags)) return 0;
+    if (!(flags & GPSG_BWD_DETERMINISTIC)) return bwd_base_bytes(n) + slack;
+    if (num_rendered < 0 || num_rendered >= (1ll << 31)) { set_error("num_rendered out of range"); return 0; }
+    return bwd_base_bytes(n) + slack + bwd_det_bytes((size_t)num_rendered);
+}
+
+size_t gpsg_rasterize_backward_workspace_bytes_ex(int P, int64_t num_rendered, int flags) {
+    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags);
+}
+size_t gpsg_rasterize_backward_workspace_bytes(int P) { return gpsg_rasterize_backward_workspace_bytes_ex(P, 0, 0); }
 
 static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, int sh_M,
                            int32_t num_rendered, const GaussianSrc& src, const float* shs, const int32_t* radii,
                            const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
                            const float* dL_dout_color, float* dL_dmeans2D, float* dL_dcolors, float* dL_dsh,
-                           const GaussianGrads& out, void* workspace) {
+                           const GaussianGrads& out, void* workspace, int flags) {
     GPSG_CUDA(cudaSetDevice(device));
     const Camera cam = make_camera(*s);
     BinningState b = BinningState::carve(const_cast<void*>(binning_buffer), (size_t)num_rendered, 0);
@@ -450,7 +470,18 @@ static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t
     if (!dL_dcolors && shs) dL_dcolors = (float*)((char*)grad_acc + align_up(sizeof(float4) * 3 * (size_t)P));   // SH path scratch
     GPSG_CUDA(cudaMemsetAsync(grad_acc, 0, sizeof(float4) * 3 * (size_t)P, stream));
     int rc = GPSG_OK;
-    if (num_rendered > 0) {
+    if (num_rendered > 0 && (flags & GPSG_BWD_DETERMINISTIC)) {
+        // stored per-(pair, half, warp) partials, then a fixed-order sum per Gaussian: bit-reproducible (raster_backward.cu)
+        char* det = (char*)grad_acc + bwd_base_bytes((size_t)P);
+        uint32_t* mask = (uint32_t*)det;
+        float* part = (float*)(det + align_up(bwd_det_mask_bytes((size_t)num_rendered)));
+        GPSG_CUDA(cudaMemsetAsync(mask, 0, bwd_det_mask_bytes((size_t)num_rendered), stream));
+        { StageTimer t(ST_RENDER_BWD_DET, stream, 1); rc = launch_render_backward_det(cam, b, im, dL_dout_color, part, mask, stream); }
+        if (rc) return rc;
+        { StageTimer t(ST_RENDER_BWD_DET_REDUCE, stream, 1);
+          rc = launch_det_reduce(cam, P, radii, gst, b, im, (const uint8_t*)mask, part, grad_acc, stream); }
+        if (rc) return rc;
+    } else if (num_rendered > 0) {
         { StageTimer t(ST_RENDER_BWD, stream, 1); rc = launch_render_backward(cam, b, im, dL_dout_color, grad_acc, stream); }
         if (rc) return rc;
     }
@@ -466,14 +497,16 @@ static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t
     return GPSG_OK;
 }
 
-int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
-                            int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
-                            const float* opacities, const float* scales, const float* rotations,
-                            const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
-                            const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                            float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                            float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                            void* workspace) {
+int gpsg_rasterize_backward_ex(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
+                               int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
+                               const float* opacities, const float* scales, const float* rotations,
+                               const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
+                               const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                               float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
+                               float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
+                               void* workspace, int flags) {
+    int rc = check_bwd_flags(flags);
+    if (rc) return rc;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(P >= 0 && num_rendered >= 0, "negative size");
     if (P == 0) return GPSG_OK;
@@ -489,11 +522,11 @@ int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* strea
     out.dmeans3D = dL_dmeans3D; out.dopacity = dL_dopacity; out.dcov3D = dL_dcov3D;
     out.dscales = cov3D_precomp ? nullptr : dL_dscales;
     out.drots = cov3D_precomp ? nullptr : dL_drotations;
-    int rc = backward_common(s, device, stream, P, sh_M, num_rendered,
-                             aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations,
-                                     opacities, colors_precomp, cov3D_precomp),
-                             shs, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, dL_dmeans2D, dL_dcolors,
-                             dL_dsh, out, workspace);
+    rc = backward_common(s, device, stream, P, sh_M, num_rendered,
+                         aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations,
+                                 opacities, colors_precomp, cov3D_precomp),
+                         shs, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, dL_dmeans2D, dL_dcolors,
+                         dL_dsh, out, workspace, flags);
     if (rc) return rc;
     if (cov3D_precomp) {
         if (dL_dscales) GPSG_CUDA(cudaMemsetAsync(dL_dscales, 0, sizeof(float) * 3 * (size_t)P, stream));
@@ -502,20 +535,38 @@ int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* strea
     return GPSG_OK;
 }
 
-size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view) {
-    const size_t n = (size_t)(pixels_per_view > 0 ? 2 * pixels_per_view : 1);
-    return align_up(sizeof(float4) * 3 * n) + align_up(sizeof(float) * 3 * n) + 512;     // accumulator rows + dL_dmeans2D
+int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
+                            int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
+                            const float* opacities, const float* scales, const float* rotations,
+                            const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
+                            const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                            float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
+                            float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
+                            void* workspace) {
+    return gpsg_rasterize_backward_ex(s, device, stream_, P, sh_M, num_rendered, means3D, colors_precomp, shs, opacities,
+                                      scales, rotations, cov3D_precomp, radii, geom_buffer, binning_buffer, image_buffer,
+                                      dL_dout_color, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh,
+                                      dL_dscales, dL_drotations, workspace, 0);
 }
 
-int gpsg_rasterize_backward_maps(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                 int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
-                                 const float* const* img, const float* const* rot, const float* const* scale,
-                                 const float* const* opacity, const int32_t* radii, const void* geom_buffer,
-                                 const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                                 float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
-                                 float* const* dL_dscale, float* const* dL_dopacity, void* workspace) {
+size_t gpsg_rasterize_backward_maps_workspace_bytes_ex(int pixels_per_view, int64_t num_rendered, int flags) {
+    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags);
+}
+size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view) {
+    return gpsg_rasterize_backward_maps_workspace_bytes_ex(pixels_per_view, 0, 0);
+}
+
+int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                    int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
+                                    const float* const* img, const float* const* rot, const float* const* scale,
+                                    const float* const* opacity, const int32_t* radii, const void* geom_buffer,
+                                    const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                                    float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
+                                    float* const* dL_dscale, float* const* dL_dopacity, void* workspace, int flags) {
+    int rc = check_bwd_flags(flags);
+    if (rc) return rc;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
-    int rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
+    rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
     if (rc) return rc;
     GPSG_REQUIRE(num_rendered >= 0 && radii && geom_buffer && binning_buffer && image_buffer && dL_dout_color && workspace,
                  "a required input pointer is NULL");
@@ -528,12 +579,24 @@ int gpsg_rasterize_backward_maps(const GpsgRasterSettings* s, int device, void* 
         out.dopac[v] = dL_dopacity[v];
     }
     const int P = 2 * pixels_per_view;
-    // workspace: [3 x float4 P accumulator rows][float 3P dL_dmeans2D]
+    // workspace: [3 x float4 P accumulator rows][float 3P dL_dmeans2D][deterministic mode: mask, partials]
     char* w = (char*)align_up((size_t)workspace);
     float* dmeans2D = (float*)(w + align_up(sizeof(float4) * 3 * (size_t)P));
     return backward_common(s, device, (cudaStream_t)stream_, P, 0, num_rendered,
                            maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), nullptr, radii, geom_buffer,
-                           binning_buffer, image_buffer, dL_dout_color, dmeans2D, nullptr, nullptr, out, workspace);
+                           binning_buffer, image_buffer, dL_dout_color, dmeans2D, nullptr, nullptr, out, workspace, flags);
+}
+
+int gpsg_rasterize_backward_maps(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                 int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
+                                 const float* const* img, const float* const* rot, const float* const* scale,
+                                 const float* const* opacity, const int32_t* radii, const void* geom_buffer,
+                                 const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                                 float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
+                                 float* const* dL_dscale, float* const* dL_dopacity, void* workspace) {
+    return gpsg_rasterize_backward_maps_ex(s, device, stream_, pixels_per_view, num_rendered, valid, xyz, img, rot, scale,
+                                           opacity, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, dL_dxyz,
+                                           dL_dimg, dL_drot, dL_dscale, dL_dopacity, workspace, 0);
 }
 
 int gpsg_mark_visible(int device, void* stream_, int P, const float* means3D, const float* viewmatrix_host16,

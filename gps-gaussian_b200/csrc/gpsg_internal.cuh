@@ -87,6 +87,18 @@ __device__ __forceinline__ bool src_geom(const GaussianSrc& s, int i, float& x, 
     op = s.opac[v][px];
     return true;
 }
+// Tile rectangle [rx0, rx1) x [ry0, ry1) of a Gaussian with saved screen position p and radius > 0: the tiles whose lists
+// it is binned into.  Both binning paths (duplicate_kernel, bucket_scatter_kernel) and the deterministic backward's reducer
+// call this one function on the same saved means2D / radii, so the reducer visits exactly the tiles the lists hold.
+// (Same expressions as preprocess: pure scaling by 1/16 and casts, exact.)
+__device__ __forceinline__ void tile_rect(int grid_x, int grid_y, float2 p, int radius, int& rx0, int& ry0, int& rx1,
+                                          int& ry1) {
+    const float rad = (float)radius;
+    rx0 = min(grid_x, max(0, (int)((p.x - rad) / (float)GPSG_TILE_X)));
+    ry0 = min(grid_y, max(0, (int)((p.y - rad) / (float)GPSG_TILE_Y)));
+    rx1 = min(grid_x, max(0, (int)((p.x + rad + (float)(GPSG_TILE_X - 1)) / (float)GPSG_TILE_X)));
+    ry1 = min(grid_y, max(0, (int)((p.y + rad + (float)(GPSG_TILE_Y - 1)) / (float)GPSG_TILE_Y)));
+}
 __device__ __forceinline__ void src_color(const GaussianSrc& s, uint32_t id, float& r, float& g, float& b) {
     if (s.S2 == 0) { r = s.colors[3 * id]; g = s.colors[3 * id + 1]; b = s.colors[3 * id + 2]; return; }
     const int v = (int)id >= s.S2 ? 1 : 0;
@@ -165,6 +177,13 @@ int launch_render_forward(const Camera& cam, BinningState b, ImageState im, floa
 // compositing backward: (S s dx, S s dy, S s dx^2, S s dx dy | S s dy^2, S s, S w g_r, S w g_g | S w g_b, -, -, -)
 int launch_render_backward(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float4* grad_acc,
                            cudaStream_t stream);
+// deterministic mode (GPSG_BWD_DETERMINISTIC): the compositing backward stores per-(pair, half, warp) partial sums
+// det_part [N*8*9] and flags them in det_mask [N bytes, zeroed by the caller]; det_reduce adds them per Gaussian in a
+// fixed order into grad_acc (every row written).  Needs the sorted keys / point list of an exact forward.
+int launch_render_backward_det(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float* det_part,
+                               uint32_t* det_mask, cudaStream_t stream);
+int launch_det_reduce(const Camera& cam, int P, const int32_t* radii, GeomState g, BinningState b, ImageState im,
+                      const uint8_t* det_mask, const float* det_part, float4* grad_acc, cudaStream_t stream);
 int launch_preprocess_backward(const Camera& cam, int P, const GaussianSrc& src, const int32_t* radii,
                                const float4* conic_opacity, const float4* grad_acc, float* dL_dmeans2D /* out [P,3] */,
                                float* dL_dcolors /* out [P,3] or NULL */, const GaussianGrads& out, cudaStream_t stream);
@@ -212,7 +231,7 @@ int launch_l1_ssim_bwd(int planes, int H, int W, const float* img, const float* 
 
 // ---- optional per-stage timing (bench.py); see gpsg_profile_* in gpsg.h ---------------------
 enum Stage { ST_PREPROCESS = 0, ST_SCAN, ST_DUPLICATE, ST_SORT, ST_GATHER, ST_TILE_SCAN, ST_SCATTER, ST_TILE_SORT, ST_RENDER_FWD, ST_RENDER_BWD,
-             ST_PREPROCESS_BWD, ST_CORR_FWD, ST_CORR_BWD, ST_CORR_BUILD, ST_COUNT };
+             ST_PREPROCESS_BWD, ST_CORR_FWD, ST_CORR_BWD, ST_CORR_BUILD, ST_RENDER_BWD_DET, ST_RENDER_BWD_DET_REDUCE, ST_COUNT };
 struct StageTimer {  // RAII: records begin/end events on `stream` when profiling is on
     StageTimer(Stage s, cudaStream_t stream, int launches);
     ~StageTimer();

@@ -39,7 +39,7 @@ constexpr int kBwdWarps = 4;    // consumer warps per CTA: 16 x 8 pixels (half a
 constexpr int kQ = 16;
 struct __align__(16) BwdWarpBuf {
     float4 gpix[32];        // (g_r, g_g, g_b, 0) of the warp's 32 pixels
-    float4 meta[kQ];        // (mean x, mean y, id bits, 0) of the parked Gaussians
+    float4 meta[kQ];        // (mean x, mean y, id bits, 0 | deterministic mode: position in the tile list) of the parked Gaussians
     float S[kQ][33];
     float Wt[kQ][33];
 };
@@ -65,7 +65,18 @@ struct __align__(128) BwdSmem {
     BwdQueue q[kBwdWarps];
 };
 
-template <int STAGES, int MIN_BLOCKS>
+// ---------------------------------------------------------------------------------------------------------------------
+// Deterministic variant (DET = true, GPSG_BWD_DETERMINISTIC).  The vector reductions above add a warp's sums into the
+// accumulator row in whatever order the CTAs happen to run, so the default gradients change in the last bits from run to
+// run.  Under DET the flush keeps the same sums and the same shuffle but STORES them: list position `pos` (the pair's
+// index in the sorted point list) owns 8 slots of 9 floats, one per (half, warp) of the two CTAs of its tile,
+//   det_part[(pos * 8 + half * 4 + warp) * 9 + k],   k in the order of the accumulator row,
+// and the slot's bit is set in the pair's mask byte det_mask[pos] (integer OR: order-independent).  A warp parks a pair
+// at most once, so no slot is written twice; unflagged slots are never read, so only the mask needs zeroing.  A slot
+// whose nine sums are all zero is not flagged (adding it would not change any sum).  det_reduce_kernel then adds the
+// flagged slots per Gaussian in a fixed order.  DET = false compiles to the kernel above unchanged.
+// ---------------------------------------------------------------------------------------------------------------------
+template <int STAGES, int MIN_BLOCKS, bool DET>
 __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backward_q_kernel(const __grid_constant__ Camera cam,
                                                                                const float4* __restrict__ slabA,
                                                                                const float4* __restrict__ slabB,
@@ -75,7 +86,9 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
                                                                                const float* __restrict__ final_T,
                                                                                const uint32_t* __restrict__ n_contrib,
                                                                                const float* __restrict__ dL_dpix,
-                                                                               float4* __restrict__ grad_acc) {
+                                                                               float4* __restrict__ grad_acc,
+                                                                               float* __restrict__ det_part,
+                                                                               uint32_t* __restrict__ det_mask) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BwdSmem<STAGES>& sm = *reinterpret_cast<BwdSmem<STAGES>*>(smem_raw);
     SlabRing<kBwdChunk, STAGES>& ring = sm.ring;
@@ -170,7 +183,21 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
         c0 += __shfl_xor_sync(0xffffffffu, c0, 16);
         c1 += __shfl_xor_sync(0xffffffffu, c1, 16);
         c2 += __shfl_xor_sync(0xffffffffu, c2, 16);
-        if (on) {
+        if constexpr (DET) {
+            // after the xor shuffle both halves hold the same nine sums, so both take the same decision
+            if (on && (m0 != 0.f || m1 != 0.f || k0 != 0.f || k1 != 0.f || k2 != 0.f || k3 != 0.f || c0 != 0.f ||
+                       c1 != 0.f || c2 != 0.f)) {
+                const uint32_t pos = range.x + (uint32_t)__float_as_int(me.w);
+                const int s = (half << 2) + warp;
+                float* dst = det_part + ((size_t)pos * 8 + s) * 9;
+                if (qh == 0) {
+                    dst[0] = m0; dst[1] = m1; dst[2] = k0; dst[3] = k1;
+                    atomicOr(det_mask + (pos >> 2), 1u << (((pos & 3u) << 3) + s));
+                } else {
+                    dst[4] = k2; dst[5] = k3; dst[6] = c0; dst[7] = c1; dst[8] = c2;
+                }
+            }
+        } else if (on) {
             const uint32_t id = __float_as_uint(me.z);
             float4* acc = grad_acc + 3 * (size_t)id;
             if (qh == 0) {
@@ -199,7 +226,7 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
         dL_dalpha = fmaf(dL_dalpha, T, nTf_bg * inv1ma);
         wb.S[slot][lane] = Ge * (q.w * dL_dalpha);
         wb.Wt[slot][lane] = alpha_e * T;
-        if (lane == 0) wb.meta[slot] = make_float4(xq.x, xq.y, xq.z, 0.f);
+        if (lane == 0) wb.meta[slot] = make_float4(xq.x, xq.y, xq.z, DET ? xq.w : 0.f);   // DET: position in the tile list
         lastc0 = c.x; lastc1 = c.y; lastc2 = c.z;
         last_alpha = alpha_e;
         if (++slot == kQ) { flush(kQ); slot = 0; }
@@ -262,7 +289,7 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
     if (slot > 0) flush(slot);
 }
 
-template <typename K>
+template <bool DET, typename K>   // one flag per instantiation: both kernels have the same function type
 static int set_dyn_smem(K kernel, size_t bytes) {
     static thread_local int done_dev = -1;
     int dev = 0;
@@ -274,16 +301,86 @@ static int set_dyn_smem(K kernel, size_t bytes) {
     return GPSG_OK;
 }
 
-int launch_render_backward(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float4* grad_acc,
-                           cudaStream_t stream) {
+template <bool DET>
+static int launch_render_backward_t(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix,
+                                    float4* grad_acc, float* det_part, uint32_t* det_mask, cudaStream_t stream) {
     constexpr int kStages = GPSG_BWD_STAGES, kBlocks = GPSG_BWD_BLOCKS;
     const unsigned grid = 2u * (unsigned)(cam.grid_x * cam.grid_y);
-    auto kern = render_backward_q_kernel<kStages, kBlocks>;
+    auto kern = render_backward_q_kernel<kStages, kBlocks, DET>;
     const size_t smem = sizeof(BwdSmem<kStages>);
-    int rc = set_dyn_smem(kern, smem);
+    int rc = set_dyn_smem<DET>(kern, smem);
     if (rc) return rc;
     kern<<<grid, (kBwdWarps + 1) * 32, smem, stream>>>(cam, b.slabA, b.slabB, b.slabC, im.ranges, im.tile_order, im.totals,
-                                                      im.final_T, im.n_contrib, dL_dpix, grad_acc);
+                                                      im.final_T, im.n_contrib, dL_dpix, grad_acc, det_part, det_mask);
+    GPSG_LAUNCH_CHECK();
+    return GPSG_OK;
+}
+
+int launch_render_backward(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float4* grad_acc,
+                           cudaStream_t stream) {
+    return launch_render_backward_t<false>(cam, b, im, dL_dpix, grad_acc, nullptr, nullptr, stream);
+}
+
+int launch_render_backward_det(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float* det_part,
+                               uint32_t* det_mask, cudaStream_t stream) {
+    return launch_render_backward_t<true>(cam, b, im, dL_dpix, nullptr, det_part, det_mask, stream);
+}
+
+// Reducer of the deterministic mode: one thread per Gaussian.  It finds its pairs without extra memory: the tiles of its
+// rectangle (tile_rect on the saved means2D / radii, the function the binning used, so the same tiles), in row-major
+// order, i.e. ascending list positions; in each tile a binary search for (depth bits, id), the order the tile list is
+// sorted in on both binning paths.  It adds the flagged slots of each position, 0..7 ascending, and writes the packed
+// accumulator row (every row, zero for Gaussians without pairs).  The order is fixed by the inputs alone.
+__global__ void __launch_bounds__(256) det_reduce_kernel(const __grid_constant__ Camera cam, int P,
+                                                         const int32_t* __restrict__ radii, const float2* __restrict__ means2D,
+                                                         const float* __restrict__ depths, const uint2* __restrict__ ranges,
+                                                         const uint32_t* __restrict__ keys_words,
+                                                         const uint32_t* __restrict__ point_list,
+                                                         const uint8_t* __restrict__ det_mask,
+                                                         const float* __restrict__ det_part, float4* __restrict__ grad_acc) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    float a[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) a[k] = 0.f;
+    const int radius = radii[i];
+    if (radius > 0) {
+        int rx0, ry0, rx1, ry1;
+        tile_rect(cam.grid_x, cam.grid_y, means2D[i], radius, rx0, ry0, rx1, ry1);
+        const uint32_t d = __float_as_uint(depths[i]), id = (uint32_t)i;
+        for (int y = ry0; y < ry1; ++y)
+            for (int x = rx0; x < rx1; ++x) {
+                const uint2 r = ranges[y * cam.grid_x + x];
+                uint32_t lo = r.x, hi = r.y;       // first entry not below (d, id); keys: (tile << 32 | depth bits)
+                while (lo < hi) {
+                    const uint32_t mid = (lo + hi) >> 1;
+                    const uint32_t kd = keys_words[2 * (size_t)mid];
+                    if (kd < d || (kd == d && point_list[mid] < id)) lo = mid + 1; else hi = mid;
+                }
+                if (lo >= r.y || point_list[lo] != id) continue;   // cannot happen: the pair is in this list
+                const uint32_t m = det_mask[lo];
+#pragma unroll
+                for (int s = 0; s < 8; ++s) {
+                    if (m & (1u << s)) {
+                        const float* src = det_part + ((size_t)lo * 8 + s) * 9;
+#pragma unroll
+                        for (int k = 0; k < 9; ++k) a[k] += src[k];
+                    }
+                }
+            }
+    }
+    float4* acc = grad_acc + 3 * (size_t)i;
+    acc[0] = make_float4(a[0], a[1], a[2], a[3]);
+    acc[1] = make_float4(a[4], a[5], a[6], a[7]);
+    acc[2] = make_float4(a[8], 0.f, 0.f, 0.f);
+}
+
+int launch_det_reduce(const Camera& cam, int P, const int32_t* radii, GeomState g, BinningState b, ImageState im,
+                      const uint8_t* det_mask, const float* det_part, float4* grad_acc, cudaStream_t stream) {
+    if (P <= 0) return GPSG_OK;
+    det_reduce_kernel<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, radii, g.means2D, g.depths, im.ranges,
+                                                          reinterpret_cast<const uint32_t*>(b.keys), b.vals, det_mask,
+                                                          det_part, grad_acc);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

@@ -40,13 +40,8 @@ __global__ void __launch_bounds__(256) duplicate_kernel(const __grid_constant__ 
     const int radius = radii[i];
     if (radius <= 0) return;
     uint32_t off = (i == 0) ? 0u : g.point_offsets[i - 1];
-    const float2 p = g.means2D[i];
-    const float rad = (float)radius;
-    // identical expressions to preprocess (pure scaling by 1/16 and casts: exact)
-    const int rx0 = min(cam.grid_x, max(0, (int)((p.x - rad) / (float)GPSG_TILE_X)));
-    const int ry0 = min(cam.grid_y, max(0, (int)((p.y - rad) / (float)GPSG_TILE_Y)));
-    const int rx1 = min(cam.grid_x, max(0, (int)((p.x + rad + (float)(GPSG_TILE_X - 1)) / (float)GPSG_TILE_X)));
-    const int ry1 = min(cam.grid_y, max(0, (int)((p.y + rad + (float)(GPSG_TILE_Y - 1)) / (float)GPSG_TILE_Y)));
+    int rx0, ry0, rx1, ry1;
+    tile_rect(cam.grid_x, cam.grid_y, g.means2D[i], radius, rx0, ry0, rx1, ry1);
     const uint64_t dbits = (uint64_t)__float_as_uint(g.depths[i]);
     for (int y = ry0; y < ry1; ++y)
         for (int x = rx0; x < rx1; ++x) {
@@ -112,12 +107,7 @@ __global__ void __launch_bounds__(256) bucket_scatter_kernel(const __grid_consta
     if (i < P) {
         const int radius = radii[i];
         if (radius > 0) {
-            const float2 p = g.means2D[i];
-            const float rad = (float)radius;
-            rx0 = min(cam.grid_x, max(0, (int)((p.x - rad) / (float)GPSG_TILE_X)));
-            ry0 = min(cam.grid_y, max(0, (int)((p.y - rad) / (float)GPSG_TILE_Y)));
-            rx1 = min(cam.grid_x, max(0, (int)((p.x + rad + (float)(GPSG_TILE_X - 1)) / (float)GPSG_TILE_X)));
-            ry1 = min(cam.grid_y, max(0, (int)((p.y + rad + (float)(GPSG_TILE_Y - 1)) / (float)GPSG_TILE_Y)));
+            tile_rect(cam.grid_x, cam.grid_y, g.means2D[i], radius, rx0, ry0, rx1, ry1);
             entry = make_uint2((uint32_t)i, __float_as_uint(g.depths[i]));   // little-endian u64 = depth<<32 | id
         }
     }

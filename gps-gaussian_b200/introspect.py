@@ -60,9 +60,10 @@ class RasterCall:
         self.num_rendered, self.bufs = _lib.rasterize_forward(self.settings, self.color, self.radii, **self._inputs())
         return self.color
 
-    def backward(self, grad_color, want_cov3D=False):
+    def backward(self, grad_color, want_cov3D=False, deterministic=None):
+        """deterministic: None follows torch.use_deterministic_algorithms, True / False force it (_lib.backward_flags)."""
         return _lib.rasterize_backward(self.settings, self.num_rendered, self.bufs, self.radii, grad_color,
-                                       want_cov3D=want_cov3D, **self._inputs())
+                                       want_cov3D=want_cov3D, deterministic=deterministic, **self._inputs())
 
     def state(self):
         """Saved buffers as torch tensors (views into the scratch buffers)."""

@@ -108,6 +108,28 @@ GPSG_API int gpsg_rasterize_backward(const GpsgRasterSettings* settings, int dev
                             float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
                             void* workspace);
 
+/* ---- deterministic backward: the same two backward entry points with a `flags` word -------------------------------
+ * flags = 0: exactly gpsg_rasterize_backward / _maps (same workspace size, same results; those two are these with 0).
+ * flags = GPSG_BWD_DETERMINISTIC: bit-identical gradients for identical inputs on the same device and build, whatever
+ *   the CTA schedule, concurrent work on other streams or the binning path (tile bucket or GPSG_BINNING=radix).  The
+ *   compositing backward stores its per-(pair, warp) partial sums instead of adding them with atomics, and one thread
+ *   per Gaussian adds them in a fixed order.  The gradients differ from flags = 0 only by fp32 re-association.  It reads
+ *   the sorted keys and point list, so it needs the buffers of an EXACT forward (gpsg_rasterize_forward or maps
+ *   _begin/_finish); the planned forwards do not write them and are not supported.  No host synchronisation, no
+ *   allocation: graph-capturable like flags = 0.  The workspace grows by 289 bytes per pair (1-byte slot mask + 8 x 9
+ *   floats), plus alignment, so the workspace-size functions also take num_rendered.
+ * Unknown flag bits: the backward returns GPSG_E_INVALID and the size functions return 0 (message in gpsg_last_error). */
+#define GPSG_BWD_DETERMINISTIC 1
+GPSG_API size_t gpsg_rasterize_backward_workspace_bytes_ex(int P, int64_t num_rendered, int flags);
+GPSG_API int gpsg_rasterize_backward_ex(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
+                                        int32_t num_rendered, const float* means3D, const float* colors_precomp,
+                                        const float* shs, const float* opacities, const float* scales,
+                                        const float* rotations, const float* cov3D_precomp, const int32_t* radii,
+                                        const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
+                                        const float* dL_dout_color, float* dL_dmeans2D, float* dL_dcolors,
+                                        float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
+                                        float* dL_dscales, float* dL_drotations, void* workspace, int flags);
+
 /* ---- fused map -> Gaussian ingest: the rasterizer behind lib/GaussianRender.py:5-39 (pts2render) -------------------
  * Instead of boolean-mask gathering (10 `nonzero` host syncs per sample) and concatenating the two source views'
  * pixel-aligned maps into [P,k] tensors, the maps are read in place: per view v in {0,1} (lmain, rmain), with S2 =
@@ -152,6 +174,17 @@ GPSG_API int gpsg_rasterize_backward_maps(const GpsgRasterSettings* settings, in
                                           const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
                                           float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
                                           float* const* dL_dscale, float* const* dL_dopacity, void* workspace);
+/* the map-ingest backward with a flags word (see gpsg_rasterize_backward_ex) */
+GPSG_API size_t gpsg_rasterize_backward_maps_workspace_bytes_ex(int pixels_per_view, int64_t num_rendered, int flags);
+GPSG_API int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* settings, int device, void* stream,
+                                             int pixels_per_view, int32_t num_rendered, const uint8_t* const* valid,
+                                             const float* const* xyz, const float* const* img, const float* const* rot,
+                                             const float* const* scale, const float* const* opacity,
+                                             const int32_t* radii, const void* geom_buffer, const void* binning_buffer,
+                                             const void* image_buffer, const float* dL_dout_color,
+                                             float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
+                                             float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
+                                             int flags);
 
 /* ---- replaces _C.mark_visible : present[P] (uint8) = view-space z > 0.2 ---------------------- */
 GPSG_API int gpsg_mark_visible(int device, void* stream, int P, const float* means3D, const float* viewmatrix_host16,
