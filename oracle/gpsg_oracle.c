@@ -347,17 +347,45 @@ void SUFFIX(oracle_render_margins)(int W, int H, const uint32_t* ranges, const u
 }
 
 /* ------------------------------------------------------------------ A.6 */
-/* dL_dmean2D: [P,2] (NDC-scaled, see A.6), dL_dconic: [P,3] = (x, y(half-convention), w), all zero-initialised here */
-void SUFFIX(oracle_render_backward)(int P, int W, int H, const uint32_t* ranges, const uint32_t* point_list,
-                                    const real* means2D, const real* colors, const real* conic_opacity, const real* bg,
-                                    const real* final_T, const uint32_t* n_contrib, const real* dL_dpix /*3HW*/,
-                                    /* out */ real* dL_dmean2D, real* dL_dconic, real* dL_dopacity, real* dL_dcolors) {
+/* Running fp32 error bound of A.6, in units of u = 2^-24 (see oracle_render_backward_mag).  Operation counts of one
+ * fp32 implementation of A.6 (this file's, or the device's with ex2.approx / rcp.approx):
+ *   MAG_POW  relative error of G per unit of |power| terms: conic (pre-scaled or not) 2, dx / dy rounding 2, the three
+ *            products and sums 3, the ex2 argument scaling 1                                                   -> 8
+ *   MAG_EXP  exp / ex2.approx (<= 2 ulp = 4u), opacity * G 1, log2(e) constant 1                                -> 6
+ *   MAG_STEP one recovery T /= (1 - alpha): 1 - alpha 1, rcp.approx 2, the product 1, the accum_rec update 2       -> 6
+ *   MAG_TERM the products after T and alpha: the three-channel dL_dalpha sum 3, * T 1, background dot 3 and its
+ *            product 2, G * o * dL_dalpha 2, the moment products 2, the preprocess step (1/o, conic * moment) 3  -> 16
+ * The error of alpha itself is MAG_POW * |power terms| + MAG_EXP; it enters every deeper transmittance through
+ * 1 / (1 - alpha) (alpha / (1 - alpha) for T, up to 1 for the accumulated colour).
+ * The device does not form dL_dmean2D / dL_dconic per pair: it accumulates the moments sum(s dx), sum(s dy), sum(s dx^2),
+ * sum(s dx dy), sum(s dy^2), sum(s) of s = G dL_dG and multiplies by the conic (and divides by the opacity) once, in the
+ * preprocess backward.  The mean2D columns bound that too because their per-pair magnitude is
+ * |s| (|dx| |conic_x| + |dy| |conic_y|), i.e. already carries |conic| per moment, and the rounding of those final products
+ * is counted in MAG_TERM. */
+#define MAG_POW 8.0
+#define MAG_EXP 6.0
+#define MAG_STEP 6.0
+#define MAG_TERM 16.0
+
+/* dL_dmean2D: [P,2] (NDC-scaled, see A.6), dL_dconic: [P,3] = (x, y(half-convention), w), all zero-initialised here.
+ * mag / absum (double [P,9]: mean2D 2, conic 3, opacity 1, colours 3) and nterm ([P]) may be NULL; col_err ([P,3], may
+ * be NULL) is a bound, in units of 2^-24, on how far the colours of the fp32 implementation may lie from `colors`. */
+static void render_backward_impl(int P, int W, int H, const uint32_t* ranges, const uint32_t* point_list,
+                                 const real* means2D, const real* colors, const real* conic_opacity, const real* bg,
+                                 const real* final_T, const uint32_t* n_contrib, const real* dL_dpix,
+                                 real* dL_dmean2D, real* dL_dconic, real* dL_dopacity, real* dL_dcolors,
+                                 const double* col_err, double* mag, double* absum, uint32_t* nterm) {
     const int gx = (W + BLOCK_X - 1) / BLOCK_X;
     const int64_t HW = (int64_t)W * H;
     memset(dL_dmean2D, 0, sizeof(real) * 2 * (size_t)P);
     memset(dL_dconic, 0, sizeof(real) * 3 * (size_t)P);
     memset(dL_dopacity, 0, sizeof(real) * (size_t)P);
     memset(dL_dcolors, 0, sizeof(real) * 3 * (size_t)P);
+    if (mag) {
+        memset(mag, 0, sizeof(double) * 9 * (size_t)P);
+        memset(absum, 0, sizeof(double) * 9 * (size_t)P);
+        memset(nterm, 0, sizeof(uint32_t) * (size_t)P);
+    }
     const real ddelx_dx = RC(0.5) * (real)W, ddely_dy = RC(0.5) * (real)H;
     for (int py = 0; py < H; ++py) {
         for (int px = 0; px < W; ++px) {
@@ -372,6 +400,9 @@ void SUFFIX(oracle_render_backward)(int P, int W, int H, const uint32_t* ranges,
             real accum_rec[3] = {0, 0, 0}, last_color[3] = {0, 0, 0};
             real last_alpha = 0;
             real dLp[3] = {dL_dpix[pid], dL_dpix[HW + pid], dL_dpix[2 * HW + pid]};
+            double w_run = 0.0;                             /* error weight of the recovered T / accum_rec so far */
+            double acc_err[3] = {0, 0, 0}, last_err[3] = {0, 0, 0};   /* colour error carried by accum_rec (col_err) */
+            double da_last = 0.0;
             for (uint32_t k = e; k-- > s;) {
                 --contributor;
                 if (contributor >= last_contributor) continue;
@@ -407,9 +438,77 @@ void SUFFIX(oracle_render_backward)(int P, int W, int H, const uint32_t* ranges,
                 dL_dconic[3 * id + 1] += RC(-0.5) * gdx * dy * dL_dG;
                 dL_dconic[3 * id + 2] += RC(-0.5) * gdy * dy * dL_dG;
                 dL_dopacity[id] += G * dL_dalpha;
+                if (mag) {
+                    /* the same terms with every factor in absolute value and every difference a - b as |a| + |b| */
+                    const double ddx = fabs((double)dx), ddy = fabs((double)dy), dG = (double)G, dT = (double)T;
+                    const double da = (double)alpha, op = fabs((double)co[3]);
+                    const double pabs = 0.5 * (fabs((double)co[0]) * ddx * ddx + fabs((double)co[2]) * ddy * ddy) +
+                                        fabs((double)co[1]) * ddx * ddy;
+                    const double e_alpha = MAG_POW * pabs + MAG_EXP;
+                    w_run += MAG_STEP + e_alpha / (1.0 - da);   /* this T was divided by this Gaussian's 1 - alpha */
+                    const double wt = w_run + e_alpha + MAG_TERM;
+                    double aa = 0.0, bgd = 0.0, ae = 0.0;
+                    for (int ch = 0; ch < 3; ++ch) {
+                        aa += (fabs((double)colors[3 * id + ch]) + fabs((double)accum_rec[ch])) * fabs((double)dLp[ch]);
+                        bgd += fabs((double)bg[ch]) * fabs((double)dLp[ch]);
+                        if (col_err) {               /* same update as accum_rec, on the error bounds */
+                            acc_err[ch] = da_last * last_err[ch] + (1.0 - da_last) * acc_err[ch];
+                            last_err[ch] = col_err[3 * (size_t)id + ch];
+                            ae += (last_err[ch] + acc_err[ch]) * fabs((double)dLp[ch]);
+                        }
+                    }
+                    da_last = da;
+                    const double A = dT * aa + (double)T_final / (1.0 - da) * bgd;   /* |dL_dalpha| */
+                    const double A_err = dT * ae;                                     /* colour error in dL_dalpha */
+                    /* the terms are k[q] * |dL_dalpha| (q < 6) */
+                    double k9[6];
+                    k9[0] = dG * op * (ddx * fabs((double)co[0]) + ddy * fabs((double)co[1])) * fabs((double)ddelx_dx);
+                    k9[1] = dG * op * (ddy * fabs((double)co[2]) + ddx * fabs((double)co[1])) * fabs((double)ddely_dy);
+                    k9[2] = 0.5 * dG * op * ddx * ddx;
+                    k9[3] = 0.5 * dG * op * ddx * ddy;
+                    k9[4] = 0.5 * dG * op * ddy * ddy;
+                    k9[5] = dG;
+                    for (int q = 0; q < 6; ++q) {
+                        mag[9 * (size_t)id + q] += wt * k9[q] * A + k9[q] * A_err;
+                        absum[9 * (size_t)id + q] += k9[q] * A;
+                    }
+                    for (int ch = 0; ch < 3; ++ch) {
+                        const double t = da * dT * fabs((double)dLp[ch]);
+                        mag[9 * (size_t)id + 6 + ch] += wt * t;
+                        absum[9 * (size_t)id + 6 + ch] += t;
+                    }
+                    ++nterm[id];
+                }
             }
         }
     }
+}
+
+void SUFFIX(oracle_render_backward)(int P, int W, int H, const uint32_t* ranges, const uint32_t* point_list,
+                                    const real* means2D, const real* colors, const real* conic_opacity, const real* bg,
+                                    const real* final_T, const uint32_t* n_contrib, const real* dL_dpix /*3HW*/,
+                                    /* out */ real* dL_dmean2D, real* dL_dconic, real* dL_dopacity, real* dL_dcolors) {
+    render_backward_impl(P, W, H, ranges, point_list, means2D, colors, conic_opacity, bg, final_T, n_contrib, dL_dpix,
+                         dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, NULL, NULL, NULL, NULL);
+}
+
+/* oracle_render_backward plus a running error bound of an fp32 A.6 on the same state, per Gaussian:
+ *   mag[P,9]   sum over its (pixel, Gaussian) terms of  weight * |term|,  |term| the term of the gradient with every
+ *              factor in absolute value and every difference a - b replaced by |a| + |b|; weight (units of 2^-24) the
+ *              rounding count of that term: MAG_TERM + its own alpha error + one MAG_STEP + e_alpha / (1 - alpha) per
+ *              transmittance recovery the pixel has done to reach it (see the MAG_* constants above);
+ *   absum[P,9] the same sum with weight 1 (times the depth of a summation tree it bounds that tree's rounding);
+ *   nterm[P]   the number of (pixel, Gaussian) terms.
+ * col_err[P,3] (may be NULL): when the fp32 implementation computes its colours itself (SH), a bound on their error in
+ * units of 2^-24; it enters mag through dL_dalpha (own colour and the accumulated colour behind it).
+ * Columns: dL_dmean2D (2), dL_dconic (3), dL_dopacity (1), dL_dcolors (3).  A culled or never-evaluated Gaussian gets 0. */
+void SUFFIX(oracle_render_backward_mag)(int P, int W, int H, const uint32_t* ranges, const uint32_t* point_list,
+                                        const real* means2D, const real* colors, const real* conic_opacity, const real* bg,
+                                        const real* final_T, const uint32_t* n_contrib, const real* dL_dpix,
+                                        real* dL_dmean2D, real* dL_dconic, real* dL_dopacity, real* dL_dcolors,
+                                        const double* col_err, double* mag, double* absum, uint32_t* nterm) {
+    render_backward_impl(P, W, H, ranges, point_list, means2D, colors, conic_opacity, bg, final_T, n_contrib, dL_dpix,
+                         dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolors, col_err, mag, absum, nterm);
 }
 
 /* ------------------------------------------------------------------ A.7 + A.8 */

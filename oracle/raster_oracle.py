@@ -174,6 +174,35 @@ class RasterOracle:
                                                _p(out["dL_dcov3D"]), _p(out["dL_dscales"]), _p(out["dL_drots"]))
         return out
 
+    def backward_mag(self, st, dL_dpix, col_err=None):
+        """`backward` plus the running error bound of A.6 (oracle_render_backward_mag): out["mag"], out["absum"] [P,9]
+        (columns dL_dmean2D 2, dL_dconic 3, dL_dopacity 1, dL_dcolors 3) and out["nterm"] [P].  col_err [P,3]: bound, in
+        units of 2^-24, on the colour error of the fp32 implementation compared (None: it uses these colours exactly)."""
+        P, W, H = st["P"], st["W"], st["H"]
+        r = self.np
+        i = st["inputs"]
+        g = self._a(dL_dpix, (3, H, W))
+        out = dict(dL_dmean2D=np.zeros((P, 2), r), dL_dconic=np.zeros((P, 3), r), dL_dopacity=np.zeros(P, r),
+                   dL_dcolors=np.zeros((P, 3), r), dL_dmeans3D=np.zeros((P, 3), r), dL_dcov3D=np.zeros((P, 6), r),
+                   dL_dscales=np.zeros((P, 3), r), dL_drots=np.zeros((P, 4), r), mag=np.zeros((P, 9)),
+                   absum=np.zeros((P, 9)), nterm=np.zeros(P, np.uint32))
+        self._fn("oracle_render_backward_mag")(C.c_int(P), C.c_int(W), C.c_int(H), _p(st["ranges"]), _p(st["_vals_full"]),
+                                               _p(self._a(st["means2D"])), _p(self._a(i["colors"])),
+                                               _p(self._a(st["conic_opacity"])), _p(self._a(i["bg"])),
+                                               _p(self._a(st["final_T"])), _p(st["n_contrib"]), _p(g),
+                                               _p(out["dL_dmean2D"]), _p(out["dL_dconic"]), _p(out["dL_dopacity"]),
+                                               _p(out["dL_dcolors"]),
+                                               _p(None if col_err is None else np.ascontiguousarray(col_err, np.float64)),
+                                               _p(out["mag"]), _p(out["absum"]), _p(out["nterm"]))
+        cr = self.creal
+        self._fn("oracle_preprocess_backward")(C.c_int(P), C.c_int(W), C.c_int(H), _p(self._a(i["means3D"])), _p(st["radii"]),
+                                               _p(self._a(i["scales"])), _p(self._a(i["rots"])),
+                                               _p(self._a(i["cov3D_precomp"])), cr(i["scale_mod"]), _p(self._a(i["view"])),
+                                               _p(self._a(i["proj"])), cr(i["tanfovx"]), cr(i["tanfovy"]),
+                                               _p(out["dL_dmean2D"]), _p(out["dL_dconic"]), _p(out["dL_dmeans3D"]),
+                                               _p(out["dL_dcov3D"]), _p(out["dL_dscales"]), _p(out["dL_drots"]))
+        return out
+
     def mark_visible(self, means3D, view):
         P = int(np.asarray(means3D).reshape(-1, 3).shape[0])
         m3 = self._a(means3D, (P, 3)); vm = self._a(view, (16,))

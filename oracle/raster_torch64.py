@@ -34,19 +34,22 @@ def cov3d(scales, rots, scale_mod=1.0):
     return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], -1)
 
 
-def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0, cov3D=None, denom_eps=0.0):
-    """st: state dict of RasterOracle('f64').forward (supplies view/proj/camera + the discrete binning).
-    Tensor args: fp64 torch tensors (requires_grad as desired).  `cov3D` [P,6] (see `cov3d`), when given, replaces the
-    scale/rotation covariance, as cov3D_precomp does; one symmetric off-diagonal entry stands for both Sigma_ab and Sigma_ba.
-    `denom_eps` > 0 scales the gradient through the conic by det^2 / (det^2 + denom_eps) without changing the image: the
-    regulariser of the hand-written backward's 1/(det^2 + 1e-7).  Returns image [3,H,W] fp64."""
+def camera(st):
+    """The camera of a RasterOracle state as fp64 tensors: dict(view, proj, W, H, tanfovx, tanfovy)."""
     i = st["inputs"]
-    W, H = st["W"], st["H"]
     dt = torch.float64
-    view = torch.tensor(np.asarray(i["view"], np.float64).reshape(4, 4), dtype=dt)   # tensor as passed: W2V^T
-    proj = torch.tensor(np.asarray(i["proj"], np.float64).reshape(4, 4), dtype=dt)
-    bg = torch.tensor(np.asarray(i["bg"], np.float64), dtype=dt)
-    tanx, tany = float(i["tanfovx"]), float(i["tanfovy"])
+    return dict(view=torch.tensor(np.asarray(i["view"], np.float64).reshape(4, 4), dtype=dt),    # tensor as passed: W2V^T
+                proj=torch.tensor(np.asarray(i["proj"], np.float64).reshape(4, 4), dtype=dt),
+                W=st["W"], H=st["H"], tanfovx=float(i["tanfovx"]), tanfovy=float(i["tanfovy"]))
+
+
+def project(cam, means3D, c6, denom_eps=0.0):
+    """A.2 per Gaussian (every Gaussian independent of the others): world means [P,3] and covariances [P,6] ->
+    (ndc [P,2], pixel means [P,2], conic (x, y, w) [P,3], cov2D + 0.3 as (a, b, c) [P,3]).  See render_autograd for the
+    frustum clamp and `denom_eps`."""
+    dt = torch.float64
+    view, proj, W, H = cam["view"], cam["proj"], cam["W"], cam["H"]
+    tanx, tany = cam["tanfovx"], cam["tanfovy"]
     fx, fy = W / (2.0 * tanx), H / (2.0 * tany)
     P = means3D.shape[0]
     hom = torch.cat([means3D, torch.ones(P, 1, dtype=dt)], 1)
@@ -55,7 +58,6 @@ def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0, c
     pw = 1.0 / (ph[:, 3] + float(np.float32(0.0000001)))
     ndc = ph[:, :2] * pw[:, None]
     pix = torch.stack([((ndc[:, 0] + 1.0) * W - 1.0) * 0.5, ((ndc[:, 1] + 1.0) * H - 1.0) * 0.5], 1)
-    c6 = cov3d(scales, rots, scale_mod) if cov3D is None else cov3D
     Sigma = torch.stack([c6[:, 0], c6[:, 1], c6[:, 2], c6[:, 1], c6[:, 3], c6[:, 4], c6[:, 2], c6[:, 4], c6[:, 5]], -1)
     Sigma = Sigma.reshape(-1, 3, 3)
     limx, limy = float(np.float32(1.3)) * tanx, float(np.float32(1.3)) * tany
@@ -72,12 +74,28 @@ def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0, c
     cov = A @ Sigma @ A.transpose(1, 2)
     k03 = float(np.float32(0.3))
     a, b, c = cov[:, 0, 0] + k03, cov[:, 0, 1], cov[:, 1, 1] + k03
+    abc = torch.stack([a, b, c], 1)
     det = a * c - b * b
     if denom_eps:
         k = (det * det / (det * det + denom_eps)).detach()
         a, b, c = ((k * v + ((1 - k) * v).detach()) for v in (a, b, c))
         det = a * c - b * b
-    conx, cony, conz = c / det, -b / det, a / det
+    return ndc, pix, torch.stack([c / det, -b / det, a / det], 1), abc
+
+
+def render_autograd(st, means3D, colors, opacity, scales, rots, scale_mod=1.0, cov3D=None, denom_eps=0.0):
+    """st: state dict of RasterOracle('f64').forward (supplies view/proj/camera + the discrete binning).
+    Tensor args: fp64 torch tensors (requires_grad as desired).  `cov3D` [P,6] (see `cov3d`), when given, replaces the
+    scale/rotation covariance, as cov3D_precomp does; one symmetric off-diagonal entry stands for both Sigma_ab and Sigma_ba.
+    `denom_eps` > 0 scales the gradient through the conic by det^2 / (det^2 + denom_eps) without changing the image: the
+    regulariser of the hand-written backward's 1/(det^2 + 1e-7).  Returns image [3,H,W] fp64."""
+    i = st["inputs"]
+    W, H = st["W"], st["H"]
+    dt = torch.float64
+    bg = torch.tensor(np.asarray(i["bg"], np.float64), dtype=dt)
+    c6 = cov3d(scales, rots, scale_mod) if cov3D is None else cov3D
+    _, pix, con, _ = project(camera(st), means3D, c6, denom_eps)
+    conx, cony, conz = con[:, 0], con[:, 1], con[:, 2]
     op = opacity.reshape(-1)
 
     ranges = st["ranges"]
