@@ -46,6 +46,91 @@ def _sample_maps(maps, dev):
     return S2, (valid, xyz, img, rot, scale, opac)
 
 
+def _maps_forward(ctx, settings_list, maps, aux):
+    """Forward of `_RasterizeMaps` (aux: `_RasterizeMapsAux`, which also writes depth and alpha [B,1,H,W])."""
+    B = len(settings_list)
+    assert len(maps) == 12 * B
+    dev = maps[1].device
+    idx, sptr = _lib.device_stream(dev)
+    H, W = int(settings_list[0].image_height), int(settings_list[0].image_width)
+    out = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev)
+    depth = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev) if aux else None
+    alpha = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev) if aux else None
+    totals = torch.empty((B, 8), dtype=torch.int32, pin_memory=True)
+    per = []
+    for b in range(B):
+        st = settings_list[b]
+        if int(st.image_height) != H or int(st.image_width) != W:
+            raise RuntimeError("pts2render (gpsg): all samples of a batch must render at one resolution")
+        S2, tensors = _sample_maps(maps[12 * b:12 * b + 12], dev)
+        radii = torch.empty((2 * S2,), dtype=torch.int32, device=dev)
+        ptrs = [_ptrs(t) for t in tensors]
+        _lib.begin_alloc(dev)
+        try:
+            with torch.cuda.device(dev):
+                rc = _lib.lib.gpsg_rasterize_forward_maps_begin(
+                    C.byref(st), idx, sptr, S2, *ptrs, C.c_void_p(radii.data_ptr()), _lib.ALLOC_CB, C.c_void_p(1),
+                    _lib.ALLOC_CB, C.c_void_p(3), C.c_void_p(totals[b].data_ptr()))
+        finally:
+            bufs = _lib.end_alloc()
+        _lib.check(rc, "gpsg_rasterize_forward_maps_begin")
+        per.append(dict(S2=S2, tensors=tensors, ptrs=ptrs, radii=radii, geom=bufs.get(1), image=bufs.get(3)))
+    torch.cuda.current_stream(dev).synchronize()           # the ONE host synchronisation of the batch
+    ctx.per = []
+    for b in range(B):
+        p = per[b]
+        n = C.c_int32(0)
+        fn = _lib.lib.gpsg_rasterize_forward_maps_finish_aux if aux else _lib.lib.gpsg_rasterize_forward_maps_finish
+        extra = [C.c_void_p(depth[b].data_ptr()), C.c_void_p(alpha[b].data_ptr())] if aux else []
+        _lib.begin_alloc(dev)
+        try:
+            with torch.cuda.device(dev):
+                rc = fn(C.byref(settings_list[b]), idx, sptr, p["S2"], *p["ptrs"], C.c_void_p(out[b].data_ptr()), *extra,
+                        C.c_void_p(p["radii"].data_ptr()), C.c_void_p(p["geom"].data_ptr()),
+                        C.c_void_p(p["image"].data_ptr()), _lib.ALLOC_CB, C.c_void_p(2),
+                        C.c_void_p(totals[b].data_ptr()), C.byref(n))
+        finally:
+            bufs = _lib.end_alloc()
+        _lib.check(rc, fn.__name__)
+        ctx.per.append(dict(S2=p["S2"], n=int(n.value), tensors=p["tensors"], radii=p["radii"],
+                            bufs=(p["geom"], bufs.get(2), p["image"])))
+    ctx.settings_list = settings_list
+    ctx.shapes = [tuple(m.shape) for m in maps]
+    ctx._totals = totals                                   # keep the pinned words alive until the copies have landed
+    return (out, depth, alpha) if aux else out
+
+
+def _maps_backward(ctx, grad_out, grad_depth=None, grad_alpha=None):
+    """Backward of both map Functions: gradients in map layout; with grad_depth / grad_alpha [B,1,H,W] the aux entry
+    point on the aux forward's own buffers."""
+    aux = grad_depth is not None
+    grads = [None]
+    flags = _lib.backward_flags()
+    dev = grad_out.device
+    idx, sptr = _lib.device_stream(dev)
+    for b, p in enumerate(ctx.per):
+        new = lambda ref: [torch.empty_like(ref[0]), torch.empty_like(ref[1])]
+        dxyz, dimg, drot, dscale, dopac = (new(t) for t in p["tensors"][1:])
+        L = _lib.lib
+        size_fn = L.gpsg_rasterize_backward_maps_aux_workspace_bytes if aux else L.gpsg_rasterize_backward_maps_workspace_bytes_ex
+        fn = L.gpsg_rasterize_backward_maps_aux if aux else L.gpsg_rasterize_backward_maps_ex
+        ws = torch.empty(int(size_fn(p["S2"], p["n"], flags)), dtype=torch.uint8, device=dev)
+        g = _f32(grad_out[b].detach())
+        gaux = [_f32(grad_depth[b].detach()), _f32(grad_alpha[b].detach())] if aux else []
+        geom, binning, image = p["bufs"]
+        with torch.cuda.device(dev):
+            rc = fn(C.byref(ctx.settings_list[b]), idx, sptr, p["S2"], p["n"], *(_ptrs(t) for t in p["tensors"]),
+                    C.c_void_p(p["radii"].data_ptr()), C.c_void_p(geom.data_ptr()), C.c_void_p(binning.data_ptr()),
+                    C.c_void_p(image.data_ptr()), C.c_void_p(g.data_ptr()), *(C.c_void_p(t.data_ptr()) for t in gaux),
+                    _ptrs(dxyz), _ptrs(dimg), _ptrs(drot), _ptrs(dscale), _ptrs(dopac), C.c_void_p(ws.data_ptr()), flags)
+        _lib.check(rc, fn.__name__)
+        sh = ctx.shapes[12 * b:12 * b + 12]
+        grads += [None, dxyz[0].view(sh[1]), dimg[0].view(sh[2]), drot[0].view(sh[3]), dscale[0].view(sh[4]),
+                  dopac[0].view(sh[5]), None, dxyz[1].view(sh[7]), dimg[1].view(sh[8]), drot[1].view(sh[9]),
+                  dscale[1].view(sh[10]), dopac[1].view(sh[11])]
+    return tuple(grads)
+
+
 class _RasterizeMaps(torch.autograd.Function):
     """(settings_list, *12 maps per sample) -> images [B,3,H,W] with ONE host synchronisation for the whole batch: every
     sample's projection / tile counting is enqueued first (`gpsg_rasterize_forward_maps_begin`), the stream is synchronised
@@ -54,78 +139,24 @@ class _RasterizeMaps(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, settings_list, *maps):
-        B = len(settings_list)
-        assert len(maps) == 12 * B
-        dev = maps[1].device
-        idx, sptr = _lib.device_stream(dev)
-        H, W = int(settings_list[0].image_height), int(settings_list[0].image_width)
-        out = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev)
-        totals = torch.empty((B, 8), dtype=torch.int32, pin_memory=True)
-        per = []
-        for b in range(B):
-            st = settings_list[b]
-            if int(st.image_height) != H or int(st.image_width) != W:
-                raise RuntimeError("pts2render (gpsg): all samples of a batch must render at one resolution")
-            S2, tensors = _sample_maps(maps[12 * b:12 * b + 12], dev)
-            radii = torch.empty((2 * S2,), dtype=torch.int32, device=dev)
-            ptrs = [_ptrs(t) for t in tensors]
-            _lib.begin_alloc(dev)
-            try:
-                with torch.cuda.device(dev):
-                    rc = _lib.lib.gpsg_rasterize_forward_maps_begin(
-                        C.byref(st), idx, sptr, S2, *ptrs, C.c_void_p(radii.data_ptr()), _lib.ALLOC_CB, C.c_void_p(1),
-                        _lib.ALLOC_CB, C.c_void_p(3), C.c_void_p(totals[b].data_ptr()))
-            finally:
-                bufs = _lib.end_alloc()
-            _lib.check(rc, "gpsg_rasterize_forward_maps_begin")
-            per.append(dict(S2=S2, tensors=tensors, ptrs=ptrs, radii=radii, geom=bufs.get(1), image=bufs.get(3)))
-        torch.cuda.current_stream(dev).synchronize()           # the ONE host synchronisation of the batch
-        ctx.per = []
-        for b in range(B):
-            p = per[b]
-            n = C.c_int32(0)
-            _lib.begin_alloc(dev)
-            try:
-                with torch.cuda.device(dev):
-                    rc = _lib.lib.gpsg_rasterize_forward_maps_finish(
-                        C.byref(settings_list[b]), idx, sptr, p["S2"], *p["ptrs"], C.c_void_p(out[b].data_ptr()),
-                        C.c_void_p(p["radii"].data_ptr()), C.c_void_p(p["geom"].data_ptr()), C.c_void_p(p["image"].data_ptr()),
-                        _lib.ALLOC_CB, C.c_void_p(2), C.c_void_p(totals[b].data_ptr()), C.byref(n))
-            finally:
-                bufs = _lib.end_alloc()
-            _lib.check(rc, "gpsg_rasterize_forward_maps_finish")
-            ctx.per.append(dict(S2=p["S2"], n=int(n.value), tensors=p["tensors"], radii=p["radii"],
-                                bufs=(p["geom"], bufs.get(2), p["image"])))
-        ctx.settings_list = settings_list
-        ctx.shapes = [tuple(m.shape) for m in maps]
-        ctx._totals = totals                                   # keep the pinned words alive until the copies have landed
-        return out
+        return _maps_forward(ctx, settings_list, maps, aux=False)
 
     @staticmethod
     def backward(ctx, grad_out):
-        grads = [None]
-        flags = _lib.backward_flags()
-        dev = grad_out.device
-        idx, sptr = _lib.device_stream(dev)
-        for b, p in enumerate(ctx.per):
-            new = lambda ref: [torch.empty_like(ref[0]), torch.empty_like(ref[1])]
-            dxyz, dimg, drot, dscale, dopac = (new(t) for t in p["tensors"][1:])
-            ws = torch.empty(int(_lib.lib.gpsg_rasterize_backward_maps_workspace_bytes_ex(p["S2"], p["n"], flags)),
-                             dtype=torch.uint8, device=dev)
-            g = _f32(grad_out[b].detach())
-            geom, binning, image = p["bufs"]
-            with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_rasterize_backward_maps_ex(
-                    C.byref(ctx.settings_list[b]), idx, sptr, p["S2"], p["n"], *(_ptrs(t) for t in p["tensors"]),
-                    C.c_void_p(p["radii"].data_ptr()), C.c_void_p(geom.data_ptr()), C.c_void_p(binning.data_ptr()),
-                    C.c_void_p(image.data_ptr()), C.c_void_p(g.data_ptr()), _ptrs(dxyz), _ptrs(dimg), _ptrs(drot),
-                    _ptrs(dscale), _ptrs(dopac), C.c_void_p(ws.data_ptr()), flags)
-            _lib.check(rc, "gpsg_rasterize_backward_maps_ex")
-            sh = ctx.shapes[12 * b:12 * b + 12]
-            grads += [None, dxyz[0].view(sh[1]), dimg[0].view(sh[2]), drot[0].view(sh[3]), dscale[0].view(sh[4]),
-                      dopac[0].view(sh[5]), None, dxyz[1].view(sh[7]), dimg[1].view(sh[8]), drot[1].view(sh[9]),
-                      dscale[1].view(sh[10]), dopac[1].view(sh[11])]
-        return tuple(grads)
+        return _maps_backward(ctx, grad_out)
+
+
+class _RasterizeMapsAux(torch.autograd.Function):
+    """`_RasterizeMaps` in aux mode: (images [B,3,H,W], depth [B,1,H,W], alpha [B,1,H,W]), same single synchronisation;
+    the images are bit-identical to `_RasterizeMaps`'."""
+
+    @staticmethod
+    def forward(ctx, settings_list, *maps):
+        return _maps_forward(ctx, settings_list, maps, aux=True)
+
+    @staticmethod
+    def backward(ctx, grad_out, grad_depth, grad_alpha):
+        return _maps_backward(ctx, grad_out, grad_depth, grad_alpha)
 
 
 def novel_settings(height, width, fovx, fovy, bg_color, cam):
@@ -148,6 +179,18 @@ def novel_settings(height, width, fovx, fovy, bg_color, cam):
 
 def pts2render(data, bg_color):
     """Whole batch with one host synchronisation (`_RasterizeMaps`)."""
+    return _pts2render(data, bg_color, aux=False)
+
+
+def pts2render_aux(data, bg_color):
+    """`pts2render` that also sets data['novel_view']['depth_pred'] (expected view-space depth, 0 where nothing is drawn)
+    and ['alpha_pred'] (accumulated opacity: the foreground matte of the novel view), both [B,1,H,W] and differentiable,
+    from the same forward and the same single host synchronisation (`_RasterizeMapsAux`).  img_pred is bit-identical to
+    `pts2render`'s.  (A separate name keeps `pts2render`'s signature the reference's.)"""
+    return _pts2render(data, bg_color, aux=True)
+
+
+def _pts2render(data, bg_color, aux):
     nv = data['novel_view']
     bs = data['lmain']['img'].shape[0]
     maps, settings = [], []
@@ -159,7 +202,10 @@ def pts2render(data, bg_color):
         cam = torch.cat([nv[k][i].detach().reshape(-1).float()
                          for k in ('world_view_transform', 'full_proj_transform', 'camera_center')]).cpu().tolist()
         settings.append(novel_settings(nv['height'][i], nv['width'][i], nv['FovX'][i], nv['FovY'][i], bg_color, cam))
-    data['novel_view']['img_pred'] = _RasterizeMaps.apply(settings, *maps)
+    if aux:
+        nv['img_pred'], nv['depth_pred'], nv['alpha_pred'] = _RasterizeMapsAux.apply(settings, *maps)
+    else:
+        nv['img_pred'] = _RasterizeMaps.apply(settings, *maps)
     return data
 
 

@@ -105,6 +105,26 @@ lib.gpsg_rasterize_backward_maps_workspace_bytes_ex.restype = _sz
 lib.gpsg_rasterize_backward_maps_workspace_bytes_ex.argtypes = [_i, _i64, _i]
 lib.gpsg_rasterize_backward_maps_ex.restype = _i
 lib.gpsg_rasterize_backward_maps_ex.argtypes = lib.gpsg_rasterize_backward_maps.argtypes + [_i]
+lib.gpsg_rasterize_forward_aux.restype = _i
+lib.gpsg_rasterize_forward_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i] + [_vp] * 11 + [
+    ALLOC_FN, _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, C.POINTER(C.c_int32)]
+lib.gpsg_rasterize_forward_maps_finish_aux.restype = _i
+lib.gpsg_rasterize_forward_maps_finish_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_pp] * 6 + [_vp] * 6 + [
+    ALLOC_FN, _vp, _vp, C.POINTER(C.c_int32)]
+lib.gpsg_rasterize_forward_planned_aux.restype = _i
+lib.gpsg_rasterize_forward_planned_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_vp] * 12 + [_i64, _vp, _vp]
+lib.gpsg_rasterize_forward_maps_planned_aux.restype = _i
+lib.gpsg_rasterize_forward_maps_planned_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_pp] * 6 + [_vp] * 6 + [
+    _i64, _vp, _vp]
+lib.gpsg_rasterize_backward_aux_workspace_bytes.restype = _sz
+lib.gpsg_rasterize_backward_aux_workspace_bytes.argtypes = [_i, _i64, _i]
+lib.gpsg_rasterize_backward_aux.restype = _i
+lib.gpsg_rasterize_backward_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, C.c_int32] + [_vp] * 23 + [_i]
+lib.gpsg_rasterize_backward_maps_aux_workspace_bytes.restype = _sz
+lib.gpsg_rasterize_backward_maps_aux_workspace_bytes.argtypes = [_i, _i64, _i]
+lib.gpsg_rasterize_backward_maps_aux.restype = _i
+lib.gpsg_rasterize_backward_maps_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, C.c_int32] + [_pp] * 6 + [
+    _vp] * 7 + [_pp] * 5 + [_vp, _i]
 lib.gpsg_corr_build_pyramid.restype = _i
 lib.gpsg_corr_build_pyramid.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, C.POINTER(C.c_void_p), _i]
 lib.gpsg_corr_build_backward.restype = _i
@@ -143,7 +163,11 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_l1_ssim_backward", "gpsg_set_corr_build", "gpsg_profile_enable",
             "gpsg_profile_read",
             "gpsg_profile_stage_name", "gpsg_rasterize_backward_workspace_bytes_ex", "gpsg_rasterize_backward_ex",
-            "gpsg_rasterize_backward_maps_workspace_bytes_ex", "gpsg_rasterize_backward_maps_ex"]
+            "gpsg_rasterize_backward_maps_workspace_bytes_ex", "gpsg_rasterize_backward_maps_ex",
+            "gpsg_rasterize_forward_aux", "gpsg_rasterize_forward_maps_finish_aux", "gpsg_rasterize_forward_planned_aux",
+            "gpsg_rasterize_forward_maps_planned_aux", "gpsg_rasterize_backward_aux_workspace_bytes",
+            "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
+            "gpsg_rasterize_backward_maps_aux"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 
@@ -193,25 +217,30 @@ def _ptr(t):
 
 
 def rasterize_forward(settings, out_color, radii, means3D, opacities, colors_precomp=None, shs=None, scales=None,
-                      rotations=None, cov3D_precomp=None):
+                      rotations=None, cov3D_precomp=None, out_depth=None, out_alpha=None):
     """One forward through the exact entry point gpsg_rasterize_forward: one host synchronisation, and the global radix
     fallback takes tile lists of any length.  Inputs are contiguous fp32 tensors on one CUDA device, absent ones None.
     Writes out_color [3,H,W] and radii [P]; returns (num_rendered, (geom, binning, image)), the buffers the backward
-    reads."""
+    reads.  out_depth / out_alpha ([H,W] fp32, both or neither): aux mode (gpsg_rasterize_forward_aux), which also writes
+    the expected depth and the accumulated opacity."""
+    if (out_depth is None) != (out_alpha is None):
+        raise ValueError("out_depth and out_alpha must be given together")
     dev = means3D.device
     idx, stream = device_stream(dev)
     n = C.c_int32(0)
+    aux = [] if out_depth is None else [_ptr(out_depth), _ptr(out_alpha)]
+    fn = lib.gpsg_rasterize_forward_aux if aux else lib.gpsg_rasterize_forward
     begin_alloc(dev)
     try:
         with torch.cuda.device(dev):
-            rc = lib.gpsg_rasterize_forward(
+            rc = fn(
                 C.byref(settings), idx, stream, int(means3D.shape[0]), int(shs.shape[1]) if shs is not None else 0,
                 _ptr(means3D), _ptr(colors_precomp), _ptr(shs), _ptr(opacities), _ptr(scales), _ptr(rotations),
-                _ptr(cov3D_precomp), _ptr(out_color), _ptr(radii), ALLOC_CB, C.c_void_p(1), ALLOC_CB, C.c_void_p(2),
+                _ptr(cov3D_precomp), _ptr(out_color), *aux, _ptr(radii), ALLOC_CB, C.c_void_p(1), ALLOC_CB, C.c_void_p(2),
                 ALLOC_CB, C.c_void_p(3), C.byref(n))
     finally:
         bufs = end_alloc()
-    check(rc, "gpsg_rasterize_forward")
+    check(rc, fn.__name__)
     return int(n.value), (bufs.get(1), bufs.get(2), bufs.get(3))
 
 
@@ -225,11 +254,16 @@ def backward_flags(deterministic=None):
 
 
 def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D, opacities, colors_precomp=None,
-                       shs=None, scales=None, rotations=None, cov3D_precomp=None, want_cov3D=False, deterministic=None):
+                       shs=None, scales=None, rotations=None, cov3D_precomp=None, want_cov3D=False, deterministic=None,
+                       grad_depth=None, grad_alpha=None):
     """Backward of `rasterize_forward` with the same inputs, its num_rendered, buffers and radii.  Returns the gradients
     dL_dmeans2D [P,3], dL_dcolors [P,3], dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drots [P,4],
     dL_dcov3D [P,6] and dL_dsh [P,M,3].  dL_dcolors is None on the SH path, dL_dsh is None without shs and dL_dcov3D
-    is None unless want_cov3D.  `deterministic`: see `backward_flags`."""
+    is None unless want_cov3D.  `deterministic`: see `backward_flags`.  grad_depth / grad_alpha ([H,W], both or
+    neither): the aux backward (gpsg_rasterize_backward_aux); the buffers must then come from an aux forward."""
+    if (grad_depth is None) != (grad_alpha is None):
+        raise ValueError("grad_depth and grad_alpha must be given together")
+    aux = grad_depth is not None
     flags = backward_flags(deterministic)
     dev = means3D.device
     P = int(means3D.shape[0])
@@ -238,18 +272,22 @@ def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D,
                dL_dopacity=new(P, 1), dL_dmeans3D=new(P, 3), dL_dscales=new(P, 3), dL_drots=new(P, 4),
                dL_dcov3D=new(P, 6) if want_cov3D else None,
                dL_dsh=new(P, int(shs.shape[1]), 3) if shs is not None else None)
-    ws = torch.empty(int(lib.gpsg_rasterize_backward_workspace_bytes_ex(P, num_rendered, flags)), dtype=torch.uint8, device=dev)
-    g = grad_color.detach().to(torch.float32).contiguous()
+    size_fn = lib.gpsg_rasterize_backward_aux_workspace_bytes if aux else lib.gpsg_rasterize_backward_workspace_bytes_ex
+    ws = torch.empty(int(size_fn(P, num_rendered, flags)), dtype=torch.uint8, device=dev)
+    f32 = lambda t: t.detach().to(torch.float32).contiguous()
+    g = f32(grad_color)
+    gaux = [f32(grad_depth), f32(grad_alpha)] if aux else []
+    fn = lib.gpsg_rasterize_backward_aux if aux else lib.gpsg_rasterize_backward_ex
     idx, stream = device_stream(dev)
     geom, binning, image = bufs
     with torch.cuda.device(dev):
-        rc = lib.gpsg_rasterize_backward_ex(
+        rc = fn(
             C.byref(settings), idx, stream, P, int(shs.shape[1]) if shs is not None else 0, num_rendered, _ptr(means3D),
             _ptr(colors_precomp), _ptr(shs), _ptr(opacities), _ptr(scales), _ptr(rotations), _ptr(cov3D_precomp),
-            _ptr(radii), _ptr(geom), _ptr(binning), _ptr(image), _ptr(g), _ptr(out["dL_dmeans2D"]),
+            _ptr(radii), _ptr(geom), _ptr(binning), _ptr(image), _ptr(g), *[_ptr(t) for t in gaux], _ptr(out["dL_dmeans2D"]),
             _ptr(out["dL_dcolors"]), _ptr(out["dL_dopacity"]), _ptr(out["dL_dmeans3D"]), _ptr(out["dL_dcov3D"]),
             _ptr(out["dL_dsh"]), _ptr(out["dL_dscales"]), _ptr(out["dL_drots"]), _ptr(ws), flags)
-    check(rc, "gpsg_rasterize_backward_ex")
+    check(rc, fn.__name__)
     return out
 
 

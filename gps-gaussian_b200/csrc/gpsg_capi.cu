@@ -232,7 +232,8 @@ static int forward_exact_begin(const GpsgRasterSettings* s, int device, cudaStre
 }
 
 static int forward_exact_finish(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, int sh_M, GaussianSrc src,
-                                const float* shs, float* out_color, int32_t* radii, void* geom_base, void* img_base,
+                                const float* shs, float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                void* geom_base, void* img_base,
                                 gpsg_alloc_fn binning_alloc, void* binning_user, const uint32_t* totals_host,
                                 int32_t* num_rendered) {
     GPSG_CUDA(cudaSetDevice(device));
@@ -275,9 +276,14 @@ static int forward_exact_finish(const GpsgRasterSettings* s, int device, cudaStr
         { StageTimer t(ST_GATHER, stream, 1); rc = launch_gather_ranges(cam, N, src, g, b, im, stream); }
         if (rc) return rc;
     }
-    { StageTimer t(ST_RENDER_FWD, stream, 1); rc = launch_render_forward(cam, b, im, out_color, stream); }
+    { StageTimer t(ST_RENDER_FWD, stream, 1); rc = launch_render_forward(cam, b, im, out_color, g.depths, out_depth, out_alpha, stream); }
     if (rc) return rc;
     if (s->debug) GPSG_CUDA(cudaStreamSynchronize(stream));
+    return GPSG_OK;
+}
+
+static int check_aux_outputs(const float* out_depth, const float* out_alpha) {
+    GPSG_REQUIRE((out_depth == nullptr) == (out_alpha == nullptr), "out_depth and out_alpha must both be NULL or both be set");
     return GPSG_OK;
 }
 
@@ -287,10 +293,22 @@ int gpsg_rasterize_forward(const GpsgRasterSettings* s, int device, void* stream
                            const float* cov3D_precomp, float* out_color, int32_t* radii, gpsg_alloc_fn geom_alloc,
                            void* geom_user, gpsg_alloc_fn binning_alloc, void* binning_user,
                            gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered) {
+    return gpsg_rasterize_forward_aux(s, device, stream_, P, sh_M, means3D, colors_precomp, shs, opacities, scales, rotations,
+                                      cov3D_precomp, out_color, nullptr, nullptr, radii, geom_alloc, geom_user, binning_alloc,
+                                      binning_user, image_alloc, image_user, num_rendered);
+}
+
+int gpsg_rasterize_forward_aux(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
+                               const float* means3D, const float* colors_precomp, const float* shs,
+                               const float* opacities, const float* scales, const float* rotations,
+                               const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
+                               int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
+                               void* binning_user, gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered) {
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(P >= 0, "P < 0");
     GPSG_REQUIRE(s->image_width > 0 && s->image_height > 0, "image size must be positive");
     GPSG_REQUIRE(out_color != nullptr, "out_color is NULL");
+    if (int rc_aux = check_aux_outputs(out_depth, out_alpha)) return rc_aux;
     GPSG_REQUIRE(geom_alloc && binning_alloc && image_alloc, "allocator callback is NULL");
     if (P > 0) {
         GPSG_REQUIRE(means3D && opacities && radii, "means3D / opacities / radii is NULL");
@@ -313,8 +331,8 @@ int gpsg_rasterize_forward(const GpsgRasterSettings* s, int device, void* stream
                                  &geom_base, &img_base);
     if (rc) return rc;
     if (P > 0) GPSG_CUDA(cudaStreamSynchronize(stream));
-    return forward_exact_finish(s, device, stream, P, sh_M, src, shs, out_color, radii, geom_base, img_base, binning_alloc,
-                                binning_user, slot, num_rendered);
+    return forward_exact_finish(s, device, stream, P, sh_M, src, shs, out_color, out_depth, out_alpha, radii, geom_base,
+                                img_base, binning_alloc, binning_user, slot, num_rendered);
 }
 
 static int check_maps(int S2, const uint8_t* const* valid, const float* const* xyz, const float* const* img,
@@ -358,13 +376,27 @@ int gpsg_rasterize_forward_maps_finish(const GpsgRasterSettings* s, int device, 
                                        float* out_color, int32_t* radii, void* geom_buffer, void* image_buffer,
                                        gpsg_alloc_fn binning_alloc, void* binning_user, const uint32_t* totals_host,
                                        int32_t* num_rendered) {
+    return gpsg_rasterize_forward_maps_finish_aux(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity,
+                                                  out_color, nullptr, nullptr, radii, geom_buffer, image_buffer, binning_alloc,
+                                                  binning_user, totals_host, num_rendered);
+}
+
+int gpsg_rasterize_forward_maps_finish_aux(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                           const uint8_t* const* valid, const float* const* xyz, const float* const* img,
+                                           const float* const* rot, const float* const* scale, const float* const* opacity,
+                                           float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                           void* geom_buffer, void* image_buffer, gpsg_alloc_fn binning_alloc,
+                                           void* binning_user, const uint32_t* totals_host, int32_t* num_rendered) {
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(out_color && radii && geom_buffer && image_buffer && binning_alloc && totals_host, "a required pointer is NULL");
-    int rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
+    int rc = check_aux_outputs(out_depth, out_alpha);
+    if (rc) return rc;
+    rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
     if (rc) return rc;
     return forward_exact_finish(s, device, (cudaStream_t)stream_, 2 * pixels_per_view, 0,
-                                maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), nullptr, out_color, radii,
-                                geom_buffer, image_buffer, binning_alloc, binning_user, totals_host, num_rendered);
+                                maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), nullptr, out_color, out_depth,
+                                out_alpha, radii, geom_buffer, image_buffer, binning_alloc, binning_user, totals_host,
+                                num_rendered);
 }
 
 size_t gpsg_raster_geom_bytes(int P) { return GeomState::required(P > 0 ? P : 0, scan_temp_bytes(P > 0 ? P : 0)); }
@@ -376,9 +408,10 @@ const uint32_t* gpsg_raster_status_ptr(const void* image_buffer, int W, int H) {
 }
 
 static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, const GaussianSrc& src,
-                                  float* out_color, int32_t* radii, void* geom_buffer, void* binning_buffer,
-                                  int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
+                                  float* out_color, float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
+                                  void* binning_buffer, int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
+    if (int rc_aux = check_aux_outputs(out_depth, out_alpha)) return rc_aux;
     GPSG_REQUIRE(P > 0, "planned forward needs P > 0");
     GPSG_REQUIRE(s->image_width > 0 && s->image_height > 0, "image size must be positive");
     GPSG_REQUIRE(out_color && radii, "out_color / radii is NULL");
@@ -400,7 +433,7 @@ static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaS
     if (rc) return rc;
     { StageTimer t(ST_TILE_SORT, stream, 2); rc = launch_tile_sort_gather(cam, P, kMaxTileSort, src, g, b, im, stream); }
     if (rc) return rc;
-    { StageTimer t(ST_RENDER_FWD, stream, 1); rc = launch_render_forward(cam, b, im, out_color, stream); }
+    { StageTimer t(ST_RENDER_FWD, stream, 1); rc = launch_render_forward(cam, b, im, out_color, g.depths, out_depth, out_alpha, stream); }
     return rc;
 }
 
@@ -409,13 +442,25 @@ int gpsg_rasterize_forward_planned(const GpsgRasterSettings* s, int device, void
                                    const float* rotations, const float* cov3D_precomp, float* out_color, int32_t* radii,
                                    void* geom_buffer, void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
                                    uint32_t* status_host) {
+    return gpsg_rasterize_forward_planned_aux(s, device, stream_, P, means3D, colors_precomp, opacities, scales, rotations,
+                                              cov3D_precomp, out_color, nullptr, nullptr, radii, geom_buffer, binning_buffer,
+                                              capacity_pairs, image_buffer, status_host);
+}
+
+int gpsg_rasterize_forward_planned_aux(const GpsgRasterSettings* s, int device, void* stream_, int P, const float* means3D,
+                                       const float* colors_precomp, const float* opacities, const float* scales,
+                                       const float* rotations, const float* cov3D_precomp, float* out_color,
+                                       float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
+                                       void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
+                                       uint32_t* status_host) {
     GPSG_REQUIRE(means3D && colors_precomp && opacities, "a required pointer is NULL");
     GPSG_REQUIRE(((scales != nullptr && rotations != nullptr) != (cov3D_precomp != nullptr)),
                  "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
     return forward_planned_common(s, device, (cudaStream_t)stream_, P,
                                   aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations,
                                           opacities, colors_precomp, cov3D_precomp),
-                                  out_color, radii, geom_buffer, binning_buffer, capacity_pairs, image_buffer, status_host);
+                                  out_color, out_depth, out_alpha, radii, geom_buffer, binning_buffer, capacity_pairs,
+                                  image_buffer, status_host);
 }
 
 int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
@@ -423,47 +468,66 @@ int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* s, int device,
                                         const float* const* rot, const float* const* scale, const float* const* opacity,
                                         float* out_color, int32_t* radii, void* geom_buffer, void* binning_buffer,
                                         int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
+    return gpsg_rasterize_forward_maps_planned_aux(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity,
+                                                   out_color, nullptr, nullptr, radii, geom_buffer, binning_buffer,
+                                                   capacity_pairs, image_buffer, status_host);
+}
+
+int gpsg_rasterize_forward_maps_planned_aux(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                            const uint8_t* const* valid, const float* const* xyz, const float* const* img,
+                                            const float* const* rot, const float* const* scale,
+                                            const float* const* opacity, float* out_color, float* out_depth,
+                                            float* out_alpha, int32_t* radii, void* geom_buffer, void* binning_buffer,
+                                            int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
     int rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
     if (rc) return rc;
     return forward_planned_common(s, device, (cudaStream_t)stream_, 2 * pixels_per_view,
-                                  maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), out_color, radii,
-                                  geom_buffer, binning_buffer, capacity_pairs, image_buffer, status_host);
+                                  maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), out_color, out_depth,
+                                  out_alpha, radii, geom_buffer, binning_buffer, capacity_pairs, image_buffer, status_host);
 }
 
 // Backward workspace: [3 x float4 packed accumulator rows][3 floats: dL_dcolors (SH path) or dL_dmeans2D (maps)] per
 // Gaussian and, with GPSG_BWD_DETERMINISTIC, [mask: 1 byte per pair][partials: 8 slots x 9 floats per pair] after them
-// (raster_backward.cu): 289 B per pair plus alignment.
+// (raster_backward.cu): 289 B per pair plus alignment; aux mode stores 10 floats per slot (321 B per pair).
 static size_t bwd_base_bytes(size_t n) { return align_up(sizeof(float4) * 3 * n) + align_up(sizeof(float) * 3 * n); }
 static size_t bwd_det_mask_bytes(size_t N) { return (N + 3) / 4 * 4; }   // whole 32-bit words (atomicOr)
-static size_t bwd_det_bytes(size_t N) { return align_up(bwd_det_mask_bytes(N)) + align_up(sizeof(float) * 8 * 9 * N); }
+static size_t bwd_det_nk(bool aux) { return aux ? 10 : 9; }               // floats per partial-sum slot
+static size_t bwd_det_bytes(size_t N, bool aux) {
+    return align_up(bwd_det_mask_bytes(N)) + align_up(sizeof(float) * 8 * bwd_det_nk(aux) * N);
+}
 
 static int check_bwd_flags(int flags) {
     GPSG_REQUIRE((flags & ~GPSG_BWD_DETERMINISTIC) == 0, "unknown backward flag bits (GPSG_BWD_DETERMINISTIC is the only flag)");
     return GPSG_OK;
 }
 
-static size_t bwd_workspace_bytes(size_t n, size_t slack, int64_t num_rendered, int flags) {
+static size_t bwd_workspace_bytes(size_t n, size_t slack, int64_t num_rendered, int flags, bool aux) {
     if (check_bwd_flags(flags)) return 0;
     if (!(flags & GPSG_BWD_DETERMINISTIC)) return bwd_base_bytes(n) + slack;
     if (num_rendered < 0 || num_rendered >= (1ll << 31)) { set_error("num_rendered out of range"); return 0; }
-    return bwd_base_bytes(n) + slack + bwd_det_bytes((size_t)num_rendered);
+    return bwd_base_bytes(n) + slack + bwd_det_bytes((size_t)num_rendered, aux);
 }
 
 size_t gpsg_rasterize_backward_workspace_bytes_ex(int P, int64_t num_rendered, int flags) {
-    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags);
+    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags, false);
+}
+size_t gpsg_rasterize_backward_aux_workspace_bytes(int P, int64_t num_rendered, int flags) {
+    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags, true);
 }
 size_t gpsg_rasterize_backward_workspace_bytes(int P) { return gpsg_rasterize_backward_workspace_bytes_ex(P, 0, 0); }
 
 static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, int sh_M,
                            int32_t num_rendered, const GaussianSrc& src, const float* shs, const int32_t* radii,
                            const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
-                           const float* dL_dout_color, float* dL_dmeans2D, float* dL_dcolors, float* dL_dsh,
-                           const GaussianGrads& out, void* workspace, int flags) {
+                           const float* dL_dout_color, const float* dL_dout_depth, const float* dL_dout_alpha,
+                           float* dL_dmeans2D, float* dL_dcolors, float* dL_dsh, const GaussianGrads& out, void* workspace,
+                           int flags) {
     GPSG_CUDA(cudaSetDevice(device));
     const Camera cam = make_camera(*s);
     BinningState b = BinningState::carve(const_cast<void*>(binning_buffer), (size_t)num_rendered, 0);
     ImageState im = ImageState::carve(const_cast<void*>(image_buffer), cam.W, cam.H);
     GeomState gst = GeomState::carve(const_cast<void*>(geom_buffer), P, 0);
+    const AuxGrads aux{dL_dout_depth ? gst.depths : nullptr, dL_dout_depth, dL_dout_alpha};
     // one packed accumulator row (3 x float4) per Gaussian: the only buffer that needs zeroing -- the projection backward
     // writes d/dmeans2D and d/dcolours for every Gaussian
     float4* grad_acc = (float4*)align_up((size_t)workspace);
@@ -476,17 +540,18 @@ static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t
         uint32_t* mask = (uint32_t*)det;
         float* part = (float*)(det + align_up(bwd_det_mask_bytes((size_t)num_rendered)));
         GPSG_CUDA(cudaMemsetAsync(mask, 0, bwd_det_mask_bytes((size_t)num_rendered), stream));
-        { StageTimer t(ST_RENDER_BWD_DET, stream, 1); rc = launch_render_backward_det(cam, b, im, dL_dout_color, part, mask, stream); }
+        { StageTimer t(ST_RENDER_BWD_DET, stream, 1); rc = launch_render_backward_det(cam, b, im, dL_dout_color, part, mask, aux, stream); }
         if (rc) return rc;
         { StageTimer t(ST_RENDER_BWD_DET_REDUCE, stream, 1);
-          rc = launch_det_reduce(cam, P, radii, gst, b, im, (const uint8_t*)mask, part, grad_acc, stream); }
+          rc = launch_det_reduce(cam, P, radii, gst, b, im, (const uint8_t*)mask, part, grad_acc, aux.on(), stream); }
         if (rc) return rc;
     } else if (num_rendered > 0) {
-        { StageTimer t(ST_RENDER_BWD, stream, 1); rc = launch_render_backward(cam, b, im, dL_dout_color, grad_acc, stream); }
+        { StageTimer t(ST_RENDER_BWD, stream, 1); rc = launch_render_backward(cam, b, im, dL_dout_color, grad_acc, aux, stream); }
         if (rc) return rc;
     }
     { StageTimer t(ST_PREPROCESS_BWD, stream, 1);
-      rc = launch_preprocess_backward(cam, P, src, radii, gst.conic_opacity, grad_acc, dL_dmeans2D, dL_dcolors, out, stream); }
+      rc = launch_preprocess_backward(cam, P, src, radii, gst.conic_opacity, grad_acc, dL_dmeans2D, dL_dcolors, out, aux.on(),
+                                      stream); }
     if (rc) return rc;
     if (shs) {
         rc = launch_sh_backward(P, s->sh_degree, sh_M, s->campos, src.means3D, shs, radii, gst.clamped, dL_dcolors, dL_dsh,
@@ -494,6 +559,12 @@ static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t
         if (rc) return rc;
     }
     if (s->debug) GPSG_CUDA(cudaStreamSynchronize(stream));
+    return GPSG_OK;
+}
+
+static int check_aux_grads(const float* dL_dout_depth, const float* dL_dout_alpha) {
+    GPSG_REQUIRE((dL_dout_depth == nullptr) == (dL_dout_alpha == nullptr),
+                 "dL_dout_depth and dL_dout_alpha must both be NULL or both be set");
     return GPSG_OK;
 }
 
@@ -505,7 +576,23 @@ int gpsg_rasterize_backward_ex(const GpsgRasterSettings* s, int device, void* st
                                float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
                                float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
                                void* workspace, int flags) {
+    return gpsg_rasterize_backward_aux(s, device, stream_, P, sh_M, num_rendered, means3D, colors_precomp, shs, opacities,
+                                       scales, rotations, cov3D_precomp, radii, geom_buffer, binning_buffer, image_buffer,
+                                       dL_dout_color, nullptr, nullptr, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D,
+                                       dL_dcov3D, dL_dsh, dL_dscales, dL_drotations, workspace, flags);
+}
+
+int gpsg_rasterize_backward_aux(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
+                                int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
+                                const float* opacities, const float* scales, const float* rotations,
+                                const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
+                                const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                                const float* dL_dout_depth, const float* dL_dout_alpha, float* dL_dmeans2D,
+                                float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
+                                float* dL_dscales, float* dL_drotations, void* workspace, int flags) {
     int rc = check_bwd_flags(flags);
+    if (rc) return rc;
+    rc = check_aux_grads(dL_dout_depth, dL_dout_alpha);
     if (rc) return rc;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(P >= 0 && num_rendered >= 0, "negative size");
@@ -525,8 +612,8 @@ int gpsg_rasterize_backward_ex(const GpsgRasterSettings* s, int device, void* st
     rc = backward_common(s, device, stream, P, sh_M, num_rendered,
                          aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations,
                                  opacities, colors_precomp, cov3D_precomp),
-                         shs, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, dL_dmeans2D, dL_dcolors,
-                         dL_dsh, out, workspace, flags);
+                         shs, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, dL_dout_depth, dL_dout_alpha,
+                         dL_dmeans2D, dL_dcolors, dL_dsh, out, workspace, flags);
     if (rc) return rc;
     if (cov3D_precomp) {
         if (dL_dscales) GPSG_CUDA(cudaMemsetAsync(dL_dscales, 0, sizeof(float) * 3 * (size_t)P, stream));
@@ -550,7 +637,10 @@ int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* strea
 }
 
 size_t gpsg_rasterize_backward_maps_workspace_bytes_ex(int pixels_per_view, int64_t num_rendered, int flags) {
-    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags);
+    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags, false);
+}
+size_t gpsg_rasterize_backward_maps_aux_workspace_bytes(int pixels_per_view, int64_t num_rendered, int flags) {
+    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags, true);
 }
 size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view) {
     return gpsg_rasterize_backward_maps_workspace_bytes_ex(pixels_per_view, 0, 0);
@@ -563,7 +653,22 @@ int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* s, int device, voi
                                     const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
                                     float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
                                     float* const* dL_dscale, float* const* dL_dopacity, void* workspace, int flags) {
+    return gpsg_rasterize_backward_maps_aux(s, device, stream_, pixels_per_view, num_rendered, valid, xyz, img, rot, scale,
+                                            opacity, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, nullptr,
+                                            nullptr, dL_dxyz, dL_dimg, dL_drot, dL_dscale, dL_dopacity, workspace, flags);
+}
+
+int gpsg_rasterize_backward_maps_aux(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                     int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
+                                     const float* const* img, const float* const* rot, const float* const* scale,
+                                     const float* const* opacity, const int32_t* radii, const void* geom_buffer,
+                                     const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                                     const float* dL_dout_depth, const float* dL_dout_alpha, float* const* dL_dxyz,
+                                     float* const* dL_dimg, float* const* dL_drot, float* const* dL_dscale,
+                                     float* const* dL_dopacity, void* workspace, int flags) {
     int rc = check_bwd_flags(flags);
+    if (rc) return rc;
+    rc = check_aux_grads(dL_dout_depth, dL_dout_alpha);
     if (rc) return rc;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
@@ -584,7 +689,8 @@ int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* s, int device, voi
     float* dmeans2D = (float*)(w + align_up(sizeof(float4) * 3 * (size_t)P));
     return backward_common(s, device, (cudaStream_t)stream_, P, 0, num_rendered,
                            maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), nullptr, radii, geom_buffer,
-                           binning_buffer, image_buffer, dL_dout_color, dmeans2D, nullptr, nullptr, out, workspace, flags);
+                           binning_buffer, image_buffer, dL_dout_color, dL_dout_depth, dL_dout_alpha, dmeans2D, nullptr,
+                           nullptr, out, workspace, flags);
 }
 
 int gpsg_rasterize_backward_maps(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,

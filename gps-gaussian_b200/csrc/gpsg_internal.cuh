@@ -171,22 +171,32 @@ int launch_bucket_scatter(const Camera& cam, int P, const int32_t* radii, GeomSt
 int launch_tile_sort_gather(const Camera& cam, int P, uint32_t max_count, const GaussianSrc& src, GeomState g,
                             BinningState b, ImageState im, cudaStream_t stream);
 // raster_render.cu
-int launch_render_forward(const Camera& cam, BinningState b, ImageState im, float* out_color, cudaStream_t stream);
+// out_depth / out_alpha [H,W] (both NULL, or both set: aux mode, z read from depths[P] of the geometry state)
+int launch_render_forward(const Camera& cam, BinningState b, ImageState im, float* out_color, const float* depths,
+                          float* out_depth, float* out_alpha, cudaStream_t stream);
 // raster_backward.cu
+// Aux-mode inputs of the compositing backward: the geometry state's depths[P] and dL/ddepth, dL/dalpha [H,W] of the
+// forward's depth and alpha outputs.  All NULL: the backward of the colour image alone.
+struct AuxGrads {
+    const float* depths; const float* dL_ddepth; const float* dL_dalpha;
+    bool on() const { return dL_ddepth != nullptr; }
+};
 // grad_acc: [P] rows of 3 x float4 (12 floats, zero-initialised by the caller) -- the packed accumulator of the
-// compositing backward: (S s dx, S s dy, S s dx^2, S s dx dy | S s dy^2, S s, S w g_r, S w g_g | S w g_b, -, -, -)
+// compositing backward: (S s dx, S s dy, S s dx^2, S s dx dy | S s dy^2, S s, S w g_r, S w g_g | S w g_b, S w g_D, -, -);
+// S w g_D (dL/dz of the view-space depth) only in aux mode
 int launch_render_backward(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float4* grad_acc,
-                           cudaStream_t stream);
+                           const AuxGrads& aux, cudaStream_t stream);
 // deterministic mode (GPSG_BWD_DETERMINISTIC): the compositing backward stores per-(pair, half, warp) partial sums
-// det_part [N*8*9] and flags them in det_mask [N bytes, zeroed by the caller]; det_reduce adds them per Gaussian in a
-// fixed order into grad_acc (every row written).  Needs the sorted keys / point list of an exact forward.
+// det_part [N*8*9, aux mode N*8*10] and flags them in det_mask [N bytes, zeroed by the caller]; det_reduce adds them per
+// Gaussian in a fixed order into grad_acc (every row written).  Needs the sorted keys / point list of an exact forward.
 int launch_render_backward_det(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float* det_part,
-                               uint32_t* det_mask, cudaStream_t stream);
+                               uint32_t* det_mask, const AuxGrads& aux, cudaStream_t stream);
 int launch_det_reduce(const Camera& cam, int P, const int32_t* radii, GeomState g, BinningState b, ImageState im,
-                      const uint8_t* det_mask, const float* det_part, float4* grad_acc, cudaStream_t stream);
+                      const uint8_t* det_mask, const float* det_part, float4* grad_acc, bool aux, cudaStream_t stream);
 int launch_preprocess_backward(const Camera& cam, int P, const GaussianSrc& src, const int32_t* radii,
                                const float4* conic_opacity, const float4* grad_acc, float* dL_dmeans2D /* out [P,3] */,
-                               float* dL_dcolors /* out [P,3] or NULL */, const GaussianGrads& out, cudaStream_t stream);
+                               float* dL_dcolors /* out [P,3] or NULL */, const GaussianGrads& out, bool aux,
+                               cudaStream_t stream);
 // sh.cu
 int launch_sh_forward(int P, int deg, int M, const float* campos3, const float* means3D, const float* shs,
                       const int32_t* radii, float* rgb, uint8_t* clamped, cudaStream_t stream);

@@ -38,7 +38,7 @@ constexpr int kBwdWarps = 4;    // consumer warps per CTA: 16 x 8 pixels (half a
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int kQ = 16;
 struct __align__(16) BwdWarpBuf {
-    float4 gpix[32];        // (g_r, g_g, g_b, 0) of the warp's 32 pixels
+    float4 gpix[32];        // (g_r, g_g, g_b, 0 | AUX: g_D) of the warp's 32 pixels
     float4 meta[kQ];        // (mean x, mean y, id bits, 0 | deterministic mode: position in the tile list) of the parked Gaussians
     float S[kQ][33];
     float Wt[kQ][33];
@@ -56,7 +56,7 @@ struct __align__(16) BwdWarpBuf {
 struct __align__(16) BwdQueue {
     float4 X[34];      // (mean x, mean y, Gaussian id bits, list position bits)
     float4 B[34];      // log2-domain conic + opacity
-    float4 C[34];      // (r, g, b, -)
+    float4 C[34];      // (r, g, b, - | AUX: view-space depth z)
 };
 template <int STAGES>
 struct __align__(128) BwdSmem {
@@ -75,8 +75,17 @@ struct __align__(128) BwdSmem {
 // at most once, so no slot is written twice; unflagged slots are never read, so only the mask needs zeroing.  A slot
 // whose nine sums are all zero is not flagged (adding it would not change any sum).  det_reduce_kernel then adds the
 // flagged slots per Gaussian in a fixed order.  DET = false compiles to the kernel above unchanged.
+//
+// Aux mode (AUX = true): the backward of the depth and alpha outputs of render_forward_kernel<true>.  Depth is a fourth
+// colour channel whose colour is z (gathered from depths[id], as the forward does) and whose background is 0: one more
+// running accum_rec channel adds (z - accum_z) * g_D to dL_dalpha, and the flush adds S w * g_D into slot 9 of the
+// accumulator row (the spare .y of its third float4; under DET the tenth float of a det_part slot, det_nk = 10).  Alpha
+// = 1 - T_final has d/dalpha_i = T_final / (1 - alpha_i), the shape of the background term, so it costs nothing: it is
+// folded into nTf_bg as -T_final * (bg . g_rgb - g_A).  AUX = false compiles to the kernel without these terms.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int STAGES, int MIN_BLOCKS, bool DET>
+template <bool AUX> constexpr int det_nk() { return AUX ? 10 : 9; }   // floats per det_part slot
+
+template <int STAGES, int MIN_BLOCKS, bool DET, bool AUX>
 __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backward_q_kernel(const __grid_constant__ Camera cam,
                                                                                const float4* __restrict__ slabA,
                                                                                const float4* __restrict__ slabB,
@@ -88,7 +97,10 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
                                                                                const float* __restrict__ dL_dpix,
                                                                                float4* __restrict__ grad_acc,
                                                                                float* __restrict__ det_part,
-                                                                               uint32_t* __restrict__ det_mask) {
+                                                                               uint32_t* __restrict__ det_mask,
+                                                                               const float* __restrict__ depths,
+                                                                               const float* __restrict__ dL_ddepth,
+                                                                               const float* __restrict__ dL_dalpha_out) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     BwdSmem<STAGES>& sm = *reinterpret_cast<BwdSmem<STAGES>*>(smem_raw);
     SlabRing<kBwdChunk, STAGES>& ring = sm.ring;
@@ -139,9 +151,14 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
     float accum0 = 0.f, accum1 = 0.f, accum2 = 0.f, lastc0 = 0.f, lastc1 = 0.f, lastc2 = 0.f, last_alpha = 0.f;
     float g0 = 0.f, g1 = 0.f, g2 = 0.f;
     if (inside) { g0 = dL_dpix[pid]; g1 = dL_dpix[HW + pid]; g2 = dL_dpix[2 * HW + pid]; }
-    wb.gpix[lane] = make_float4(g0, g1, g2, 0.f);
+    float accum3 = 0.f, lastc3 = 0.f, g3 = 0.f, gA = 0.f;     // AUX: depth channel, alpha gradient
+    if constexpr (AUX) {
+        if (inside) { g3 = dL_ddepth[pid]; gA = dL_dalpha_out[pid]; }
+    }
+    wb.gpix[lane] = make_float4(g0, g1, g2, g3);
     __syncwarp();
-    const float bg_dot = (cam.bg[0] * g0 + cam.bg[1] * g1) + cam.bg[2] * g2;
+    float bg_dot = (cam.bg[0] * g0 + cam.bg[1] * g1) + cam.bg[2] * g2;
+    if constexpr (AUX) bg_dot -= gA;
     const float nTf_bg = -T_final * bg_dot;
 
     const int qj = lane & (kQ - 1), qh = lane >> 4;
@@ -154,7 +171,7 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
         const float4 me = wb.meta[qj];
         const bool on = qj < cnt;
         const float dxb = me.x - fx0, dy0 = me.y - fy0, dy1 = dy0 - 1.0f;
-        float m0 = 0.f, m1 = 0.f, k0 = 0.f, k1 = 0.f, k2 = 0.f, k3 = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
+        float m0 = 0.f, m1 = 0.f, k0 = 0.f, k1 = 0.f, k2 = 0.f, k3 = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f;
 #pragma unroll
         for (int pp = 0; pp < 16; ++pp) {
             const int p = qh * 16 + pp;
@@ -173,6 +190,7 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
             c0 = fmaf(wv, gp.x, c0);
             c1 = fmaf(wv, gp.y, c1);
             c2 = fmaf(wv, gp.z, c2);
+            if constexpr (AUX) c3 = fmaf(wv, gp.w, c3);
         }
         m0 += __shfl_xor_sync(0xffffffffu, m0, 16);
         m1 += __shfl_xor_sync(0xffffffffu, m1, 16);
@@ -183,18 +201,20 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
         c0 += __shfl_xor_sync(0xffffffffu, c0, 16);
         c1 += __shfl_xor_sync(0xffffffffu, c1, 16);
         c2 += __shfl_xor_sync(0xffffffffu, c2, 16);
+        if constexpr (AUX) c3 += __shfl_xor_sync(0xffffffffu, c3, 16);
         if constexpr (DET) {
-            // after the xor shuffle both halves hold the same nine sums, so both take the same decision
+            // after the xor shuffle both halves hold the same nine (AUX: ten) sums, so both take the same decision
             if (on && (m0 != 0.f || m1 != 0.f || k0 != 0.f || k1 != 0.f || k2 != 0.f || k3 != 0.f || c0 != 0.f ||
-                       c1 != 0.f || c2 != 0.f)) {
+                       c1 != 0.f || c2 != 0.f || (AUX && c3 != 0.f))) {
                 const uint32_t pos = range.x + (uint32_t)__float_as_int(me.w);
                 const int s = (half << 2) + warp;
-                float* dst = det_part + ((size_t)pos * 8 + s) * 9;
+                float* dst = det_part + ((size_t)pos * 8 + s) * det_nk<AUX>();
                 if (qh == 0) {
                     dst[0] = m0; dst[1] = m1; dst[2] = k0; dst[3] = k1;
                     atomicOr(det_mask + (pos >> 2), 1u << (((pos & 3u) << 3) + s));
                 } else {
                     dst[4] = k2; dst[5] = k3; dst[6] = c0; dst[7] = c1; dst[8] = c2;
+                    if constexpr (AUX) dst[9] = c3;
                 }
             }
         } else if (on) {
@@ -204,7 +224,11 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
                 if (m0 != 0.f || m1 != 0.f || k0 != 0.f || k1 != 0.f) atomicAdd(acc, make_float4(m0, m1, k0, k1));
             } else {
                 if (k2 != 0.f || k3 != 0.f || c0 != 0.f || c1 != 0.f) atomicAdd(acc + 1, make_float4(k2, k3, c0, c1));
-                if (c2 != 0.f) atomicAdd(reinterpret_cast<float*>(acc + 2), c2);
+                if constexpr (AUX) {
+                    if (c2 != 0.f || c3 != 0.f) atomicAdd(reinterpret_cast<float2*>(acc + 2), make_float2(c2, c3));
+                } else {
+                    if (c2 != 0.f) atomicAdd(reinterpret_cast<float*>(acc + 2), c2);
+                }
             }
         }
         __syncwarp();
@@ -223,6 +247,11 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
         float dL_dalpha = (c.x - accum0) * g0;
         dL_dalpha = fmaf(c.y - accum1, g1, dL_dalpha);
         dL_dalpha = fmaf(c.z - accum2, g2, dL_dalpha);
+        if constexpr (AUX) {
+            accum3 = fmaf(last_alpha, lastc3 - accum3, accum3);
+            dL_dalpha = fmaf(c.w - accum3, g3, dL_dalpha);
+            lastc3 = c.w;
+        }
         dL_dalpha = fmaf(dL_dalpha, T, nTf_bg * inv1ma);
         wb.S[slot][lane] = Ge * (q.w * dL_dalpha);
         wb.Wt[slot][lane] = alpha_e * T;
@@ -259,7 +288,8 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
                     const float4 c = SC[my];
                     Q.X[r] = make_float4(a.x, a.y, c.w, __int_as_float(start + my));
                     Q.B[r] = SB[my];
-                    Q.C[r] = c;
+                    if constexpr (AUX) Q.C[r] = make_float4(c.x, c.y, c.z, depths[__float_as_uint(c.w)]);
+                    else Q.C[r] = c;
                 }
                 if (lane == 0) {                             // pad odd counts: position "infinity" -> never active
                     Q.X[cnt] = make_float4(0.f, 0.f, 0.f, __int_as_float(0x7fffffff));
@@ -289,7 +319,7 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
     if (slot > 0) flush(slot);
 }
 
-template <bool DET, typename K>   // one flag per instantiation: both kernels have the same function type
+template <bool DET, bool AUX, typename K>   // one flag per instantiation: all kernels have the same function type
 static int set_dyn_smem(K kernel, size_t bytes) {
     static thread_local int done_dev = -1;
     int dev = 0;
@@ -301,29 +331,33 @@ static int set_dyn_smem(K kernel, size_t bytes) {
     return GPSG_OK;
 }
 
-template <bool DET>
+template <bool DET, bool AUX>
 static int launch_render_backward_t(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix,
-                                    float4* grad_acc, float* det_part, uint32_t* det_mask, cudaStream_t stream) {
+                                    float4* grad_acc, float* det_part, uint32_t* det_mask, const AuxGrads& aux,
+                                    cudaStream_t stream) {
     constexpr int kStages = GPSG_BWD_STAGES, kBlocks = GPSG_BWD_BLOCKS;
     const unsigned grid = 2u * (unsigned)(cam.grid_x * cam.grid_y);
-    auto kern = render_backward_q_kernel<kStages, kBlocks, DET>;
+    auto kern = render_backward_q_kernel<kStages, kBlocks, DET, AUX>;
     const size_t smem = sizeof(BwdSmem<kStages>);
-    int rc = set_dyn_smem<DET>(kern, smem);
+    int rc = set_dyn_smem<DET, AUX>(kern, smem);
     if (rc) return rc;
     kern<<<grid, (kBwdWarps + 1) * 32, smem, stream>>>(cam, b.slabA, b.slabB, b.slabC, im.ranges, im.tile_order, im.totals,
-                                                      im.final_T, im.n_contrib, dL_dpix, grad_acc, det_part, det_mask);
+                                                      im.final_T, im.n_contrib, dL_dpix, grad_acc, det_part, det_mask,
+                                                      aux.depths, aux.dL_ddepth, aux.dL_dalpha);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }
 
 int launch_render_backward(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float4* grad_acc,
-                           cudaStream_t stream) {
-    return launch_render_backward_t<false>(cam, b, im, dL_dpix, grad_acc, nullptr, nullptr, stream);
+                           const AuxGrads& aux, cudaStream_t stream) {
+    if (aux.on()) return launch_render_backward_t<false, true>(cam, b, im, dL_dpix, grad_acc, nullptr, nullptr, aux, stream);
+    return launch_render_backward_t<false, false>(cam, b, im, dL_dpix, grad_acc, nullptr, nullptr, aux, stream);
 }
 
 int launch_render_backward_det(const Camera& cam, BinningState b, ImageState im, const float* dL_dpix, float* det_part,
-                               uint32_t* det_mask, cudaStream_t stream) {
-    return launch_render_backward_t<true>(cam, b, im, dL_dpix, nullptr, det_part, det_mask, stream);
+                               uint32_t* det_mask, const AuxGrads& aux, cudaStream_t stream) {
+    if (aux.on()) return launch_render_backward_t<true, true>(cam, b, im, dL_dpix, nullptr, det_part, det_mask, aux, stream);
+    return launch_render_backward_t<true, false>(cam, b, im, dL_dpix, nullptr, det_part, det_mask, aux, stream);
 }
 
 // Reducer of the deterministic mode: one thread per Gaussian.  It finds its pairs without extra memory: the tiles of its
@@ -331,6 +365,8 @@ int launch_render_backward_det(const Camera& cam, BinningState b, ImageState im,
 // order, i.e. ascending list positions; in each tile a binary search for (depth bits, id), the order the tile list is
 // sorted in on both binning paths.  It adds the flagged slots of each position, 0..7 ascending, and writes the packed
 // accumulator row (every row, zero for Gaussians without pairs).  The order is fixed by the inputs alone.
+// AUX: slots of 10 floats; the tenth (S w g_D) is added in the same order and lands in slot 9 of the row.
+template <bool AUX>
 __global__ void __launch_bounds__(256) det_reduce_kernel(const __grid_constant__ Camera cam, int P,
                                                          const int32_t* __restrict__ radii, const float2* __restrict__ means2D,
                                                          const float* __restrict__ depths, const uint2* __restrict__ ranges,
@@ -340,9 +376,10 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const __grid_constant__
                                                          const float* __restrict__ det_part, float4* __restrict__ grad_acc) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
-    float a[9];
+    constexpr int NK = det_nk<AUX>();
+    float a[NK];
 #pragma unroll
-    for (int k = 0; k < 9; ++k) a[k] = 0.f;
+    for (int k = 0; k < NK; ++k) a[k] = 0.f;
     const int radius = radii[i];
     if (radius > 0) {
         int rx0, ry0, rx1, ry1;
@@ -362,9 +399,9 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const __grid_constant__
 #pragma unroll
                 for (int s = 0; s < 8; ++s) {
                     if (m & (1u << s)) {
-                        const float* src = det_part + ((size_t)lo * 8 + s) * 9;
+                        const float* src = det_part + ((size_t)lo * 8 + s) * NK;
 #pragma unroll
-                        for (int k = 0; k < 9; ++k) a[k] += src[k];
+                        for (int k = 0; k < NK; ++k) a[k] += src[k];
                     }
                 }
             }
@@ -372,20 +409,24 @@ __global__ void __launch_bounds__(256) det_reduce_kernel(const __grid_constant__
     float4* acc = grad_acc + 3 * (size_t)i;
     acc[0] = make_float4(a[0], a[1], a[2], a[3]);
     acc[1] = make_float4(a[4], a[5], a[6], a[7]);
-    acc[2] = make_float4(a[8], 0.f, 0.f, 0.f);
+    acc[2] = make_float4(a[8], AUX ? a[NK - 1] : 0.f, 0.f, 0.f);
 }
 
 int launch_det_reduce(const Camera& cam, int P, const int32_t* radii, GeomState g, BinningState b, ImageState im,
-                      const uint8_t* det_mask, const float* det_part, float4* grad_acc, cudaStream_t stream) {
+                      const uint8_t* det_mask, const float* det_part, float4* grad_acc, bool aux, cudaStream_t stream) {
     if (P <= 0) return GPSG_OK;
-    det_reduce_kernel<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, radii, g.means2D, g.depths, im.ranges,
-                                                          reinterpret_cast<const uint32_t*>(b.keys), b.vals, det_mask,
-                                                          det_part, grad_acc);
+    auto kern = aux ? det_reduce_kernel<true> : det_reduce_kernel<false>;
+    kern<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, radii, g.means2D, g.depths, im.ranges,
+                                              reinterpret_cast<const uint32_t*>(b.keys), b.vals, det_mask, det_part,
+                                              grad_acc);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }
 
 // A.7 + A.8 fused: per Gaussian, (dL/dmean2D, dL/dconic) -> dL/d{mean3D, cov3D, scale, rotation}.
+// AUX: slot 9 of the accumulator row is dL/dz of the view-space depth z = view[2] x + view[6] y + view[10] z + view[14],
+// added to dL/dmeans3D (map mode: dL/dxyz) through the view matrix's third row.
+template <bool AUX>
 __global__ void __launch_bounds__(256) preprocess_backward_kernel(
     const __grid_constant__ Camera cam, int P, const GaussianSrc src, const int32_t* __restrict__ radii,
     const float4* __restrict__ conic_opacity, const float4* __restrict__ grad_acc, float* __restrict__ dL_dmeans2D_out,
@@ -516,6 +557,12 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(
         dm[0] += (proj[0] * m_w - proj[3] * mul1) * gm0 + (proj[1] * m_w - proj[3] * mul2) * gm1;
         dm[1] += (proj[4] * m_w - proj[7] * mul1) * gm0 + (proj[5] * m_w - proj[7] * mul2) * gm1;
         dm[2] += (proj[8] * m_w - proj[11] * mul1) * gm0 + (proj[9] * m_w - proj[11] * mul2) * gm1;
+        if constexpr (AUX) {
+            const float dz = reinterpret_cast<const float*>(grad_acc + 3 * (size_t)i + 2)[1];
+            dm[0] = fmaf(view[2], dz, dm[0]);
+            dm[1] = fmaf(view[6], dz, dm[1]);
+            dm[2] = fmaf(view[10], dz, dm[2]);
+        }
         // --- A.8: Sigma3D -> scale, rotation ---
         if (!cov3D_precomp) {
             const float dS[3][3] = {{dcov[0], 0.5f * dcov[1], 0.5f * dcov[2]},
@@ -582,10 +629,10 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(
 
 int launch_preprocess_backward(const Camera& cam, int P, const GaussianSrc& src, const int32_t* radii,
                                const float4* conic_opacity, const float4* grad_acc, float* dL_dmeans2D, float* dL_dcolors,
-                               const GaussianGrads& out, cudaStream_t stream) {
+                               const GaussianGrads& out, bool aux, cudaStream_t stream) {
     if (P <= 0) return GPSG_OK;
-    preprocess_backward_kernel<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, src, radii, conic_opacity, grad_acc, dL_dmeans2D,
-                                                                   dL_dcolors, out);
+    auto kern = aux ? preprocess_backward_kernel<true> : preprocess_backward_kernel<false>;
+    kern<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, src, radii, conic_opacity, grad_acc, dL_dmeans2D, dL_dcolors, out);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

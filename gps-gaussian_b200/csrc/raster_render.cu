@@ -43,6 +43,12 @@ constexpr int kFwdStages = 6;   // 6 x 3 KB ring + 5.4 KB of survivor queues = 2
 constexpr int kFwdWarps = 4;    // consumer warps per CTA: 16 x 8 pixels
 
 // 8 CTAs / SM (48 registers; 8 x 23.9 KB of shared memory also fits the 228 KB of an H100 SM)
+// AUX (aux mode): also composites the view-space depth z of every Gaussian as a fourth colour channel with background 0,
+// D = sum_i alpha_i T_i z_i, and writes alpha = 1 - T beside final_T.  z is gathered per survivor from the geometry
+// state's depths[id] (the value the tile lists are sorted by, so both binning paths see the same z) into a sixth queue
+// row.  The colour, final_T and n_contrib arithmetic is the same in both instantiations, so their results are identical;
+// AUX = false compiles to the kernel without the depth channel.
+template <bool AUX>
 __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel(const __grid_constant__ Camera cam,
                                                                             const float4* __restrict__ slabA,
                                                                             const float4* __restrict__ slabB,
@@ -51,13 +57,18 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
                                                                             const uint32_t* __restrict__ status,
                                                                             float* __restrict__ final_T,
                                                                             uint32_t* __restrict__ n_contrib,
-                                                                            float* __restrict__ out_color) {
+                                                                            float* __restrict__ out_color,
+                                                                            const float* __restrict__ depths,
+                                                                            float* __restrict__ out_depth,
+                                                                            float* __restrict__ out_alpha) {
     __shared__ SlabRing<kFwdChunk, kFwdStages> ring;
     // per consumer warp: queue of the (at most 32) entries of the current 32-entry group that survive the warp's cull,
     // + 1 pad slot.  Zero-initialised so that a pad / stale slot is always finite data with a defined (non-contributing) result.
     // Pair-interleaved queue -- pair p = survivors (2p, 2p+1): QP[k][p] = (xA,xB,yA,yB), (bxA,bxB,byA,byB),
     // (bzA,bzB,oA,oB), (rA,rB,gA,gB), (bA,bB,posA,posB): every LDS.128 lands the same two fields of both survivors.
-    __shared__ float4 qp[kFwdWarps][5][17];
+    // AUX adds a sixth row (zA,zB,-,-).
+    constexpr int kRows = AUX ? 6 : 5;
+    __shared__ float4 qp[kFwdWarps][kRows][17];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // two CTAs per 16x16 tile; tiles are taken longest list first (tile_order, see tile_scan.cuh)
@@ -68,7 +79,7 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
     const int nbatch = (total + kFwdChunk - 1) / kFwdChunk;
 
     if (tid == 0) ring_init(ring, kFwdWarps);
-    for (int e = tid; e < kFwdWarps * 5 * 17; e += (kFwdWarps + 1) * 32) (&qp[0][0][0])[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int e = tid; e < kFwdWarps * kRows * 17; e += (kFwdWarps + 1) * 32) (&qp[0][0][0])[e] = make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
 
     if (warp == kFwdWarps) {  // ---------------- producer warp ----------------
@@ -93,7 +104,7 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
     bool done = !inside;
     bool warp_done = __all_sync(0xffffffffu, done);
     if (warp_done && lane == 0) atomicAdd(&ring.done_warps, 1);
-    float T = 1.0f, C0 = 0.0f, C1 = 0.0f, C2 = 0.0f;
+    float T = 1.0f, C0 = 0.0f, C1 = 0.0f, C2 = 0.0f, D = 0.0f;
     int last_contributor = 0;
 
     for (int b = 0; b < nbatch; ++b) {
@@ -131,6 +142,7 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
                         base[2 * kS] = q.z;      base[2 * kS + 2] = q.w;
                         base[3 * kS] = c.x;      base[3 * kS + 2] = c.y;
                         base[4 * kS] = c.z;      base[4 * kS + 2] = __int_as_float(posbase + my);
+                        if constexpr (AUX) base[5 * kS] = depths[__float_as_uint(c.w)];
                     }
                     if (lane == 0 && (cnt & 1)) reinterpret_cast<float*>(&QP[2][cnt >> 1])[3] = 0.f;   // odd count: pad's opacity 0
                     __syncwarp();
@@ -138,6 +150,8 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
                     for (int i = 0; i < cnt; i += 2) {
                         const int pr = i >> 1;
                         const float4 v0 = QP[0][pr], v1 = QP[1][pr], v2 = QP[2][pr], v3 = QP[3][pr], v4 = QP[4][pr];
+                        float2 v5 = make_float2(0.f, 0.f);
+                        if constexpr (AUX) v5 = *reinterpret_cast<const float2*>(&QP[5][pr]);
                         const f2p dx2 = sub2(pk2(v0.x, v0.y), pixfx2), dy2 = sub2(pk2(v0.z, v0.w), pixfy2);
                         // p = log2e * power = bz*dy*dy + (bx*dx + by*dy)*dx, same operation order as the scalar kernel
                         const f2p t2 = fma2(pk2(v1.x, v1.y), dx2, mul2(pk2(v1.z, v1.w), dy2));
@@ -159,6 +173,7 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
                             C0 = fmaf(u ? v3.y : v3.x, w, C0);
                             C1 = fmaf(u ? v3.w : v3.z, w, C1);
                             C2 = fmaf(u ? v4.y : v4.x, w, C2);
+                            if constexpr (AUX) D = fmaf(u ? v5.y : v5.x, w, D);
                             T = upd ? test_T : T;
                             last_contributor = upd ? __float_as_int(u ? v4.w : v4.z) : last_contributor;
                         }
@@ -180,13 +195,24 @@ __global__ void __launch_bounds__((kFwdWarps + 1) * 32, 8) render_forward_kernel
         out_color[pid] = fmaf(T, cam.bg[0], C0);
         out_color[HW + pid] = fmaf(T, cam.bg[1], C1);
         out_color[2 * HW + pid] = fmaf(T, cam.bg[2], C2);
+        if constexpr (AUX) {
+            out_depth[pid] = D;
+            out_alpha[pid] = 1.0f - T;
+        }
     }
 }
 
-int launch_render_forward(const Camera& cam, BinningState b, ImageState im, float* out_color, cudaStream_t stream) {
+int launch_render_forward(const Camera& cam, BinningState b, ImageState im, float* out_color, const float* depths,
+                          float* out_depth, float* out_alpha, cudaStream_t stream) {
     const unsigned grid = 2u * (unsigned)(cam.grid_x * cam.grid_y);
-    render_forward_kernel<<<grid, (kFwdWarps + 1) * 32, 0, stream>>>(cam, b.slabA, b.slabB, b.slabC, im.ranges, im.tile_order,
-                                                                    im.totals, im.final_T, im.n_contrib, out_color);
+    if (out_depth)
+        render_forward_kernel<true><<<grid, (kFwdWarps + 1) * 32, 0, stream>>>(
+            cam, b.slabA, b.slabB, b.slabC, im.ranges, im.tile_order, im.totals, im.final_T, im.n_contrib, out_color, depths,
+            out_depth, out_alpha);
+    else
+        render_forward_kernel<false><<<grid, (kFwdWarps + 1) * 32, 0, stream>>>(
+            cam, b.slabA, b.slabB, b.slabC, im.ranges, im.tile_order, im.totals, im.final_T, im.n_contrib, out_color, nullptr,
+            nullptr, nullptr);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

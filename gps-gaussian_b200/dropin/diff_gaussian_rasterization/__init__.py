@@ -9,6 +9,9 @@ gaussian_renderer/__init__.py:36-49), `GaussianRasterizer(raster_settings)(means
 opacities, shs, colors_precomp, scales, rotations, cov3D_precomp) -> (color[3,H,W], radii[P])`,
 `GaussianRasterizer.markVisible`, `rasterize_gaussians`.  Same error behaviour for the
 "exactly one of" argument checks.
+
+Beyond the upstream surface, `rasterize_gaussians_aux` (same arguments) also returns the expected depth and the
+accumulated opacity (alpha) of every pixel, differentiable like the image (aux mode of include/gpsg.h).
 """
 import ctypes as C
 import os
@@ -104,49 +107,99 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales,
                                      cov3Ds_precomp, raster_settings)
 
 
+def rasterize_gaussians_aux(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                            raster_settings):
+    """`rasterize_gaussians` that also renders depth and alpha: returns (color [3,H,W], depth [H,W], alpha [H,W],
+    radii [P]).  depth = sum_i w_i z_i (view-space z, background 0), alpha = 1 - final transmittance; all three images
+    are differentiable.  The colour image and radii are bit-identical to `rasterize_gaussians`."""
+    return _RasterizeGaussiansAux.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                        cov3Ds_precomp, raster_settings)
+
+
+def _inputs(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
+    """Checked, contiguous fp32 inputs of one forward: (packed settings, dict of tensors or None), for both Functions."""
+    if not means3D.is_cuda:
+        raise RuntimeError("diff_gaussian_rasterization (gpsg): means3D must be a CUDA tensor")
+    dev = means3D.device
+    P = int(means3D.shape[0])
+    settings = _pack_settings(raster_settings)
+    t = dict(means3D=_f32c(means3D), colors_precomp=_f32c(colors_precomp) if colors_precomp.numel() else None,
+             shs=_f32c(sh) if sh.numel() else None, opacities=_f32c(opacities),
+             scales=_f32c(scales) if scales.numel() else None, rotations=_f32c(rotations) if rotations.numel() else None,
+             cov3D_precomp=_f32c(cov3Ds_precomp) if cov3Ds_precomp.numel() else None)
+    for name, k in (("opacities", 1), ("scales", 3), ("rotations", 4), ("colors_precomp", 3), ("cov3D_precomp", 6)):
+        v = t[name]
+        if v is not None and (v.numel() != k * P or v.device != dev):
+            raise RuntimeError(f"diff_gaussian_rasterization (gpsg): {name} must hold {P} x {k} values on {dev}, "
+                               f"got shape {tuple(v.shape)} on {v.device}")
+    shs = t["shs"]
+    if shs is not None and (shs.dim() != 3 or shs.shape[0] != P or shs.shape[2] != 3 or shs.device != dev):
+        raise RuntimeError(f"diff_gaussian_rasterization (gpsg): shs must be [{P}, M, 3] on {dev}")
+    return settings, t
+
+
+_SAVED = ("means3D", "colors_precomp", "shs", "opacities", "scales", "rotations", "cov3D_precomp")
+
+
+def _forward(ctx, t, aux):
+    """Exact forward (aux: also depth and alpha) with ctx.settings; saves what `_backward` needs on ctx.
+    Returns (color, radii, (depth, alpha) or (None, None))."""
+    dev = t["means3D"].device
+    H, W = int(ctx.settings.image_height), int(ctx.settings.image_width)
+    new = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
+    color = new(3, H, W)
+    maps = (new(H, W), new(H, W)) if aux else (None, None)
+    radii = torch.empty((int(t["means3D"].shape[0]),), dtype=torch.int32, device=dev)
+    ctx.num_rendered, ctx.bufs = _lib.rasterize_forward(ctx.settings, color, radii, t["means3D"], t["opacities"],
+                                                        colors_precomp=t["colors_precomp"], shs=t["shs"],
+                                                        scales=t["scales"], rotations=t["rotations"],
+                                                        cov3D_precomp=t["cov3D_precomp"], out_depth=maps[0],
+                                                        out_alpha=maps[1])
+    ctx.save_for_backward(*(t[k] for k in _SAVED), radii)
+    ctx.mark_non_differentiable(radii)
+    return color, radii, maps
+
+
+def _backward(ctx, grad_color, grad_depth=None, grad_alpha=None):
+    m3, col, shs, op, sc, ro, cp, radii = ctx.saved_tensors
+    g = _lib.rasterize_backward(ctx.settings, ctx.num_rendered, ctx.bufs, radii, grad_color, m3, op,
+                                colors_precomp=col, shs=shs, scales=sc, rotations=ro, cov3D_precomp=cp,
+                                want_cov3D=cp is not None, grad_depth=grad_depth, grad_alpha=grad_alpha)
+    # input order: means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings
+    return (g["dL_dmeans3D"], g["dL_dmeans2D"], g["dL_dsh"], g["dL_dcolors"], g["dL_dopacity"],
+            g["dL_dscales"] if sc is not None else None, g["dL_drots"] if ro is not None else None, g["dL_dcov3D"],
+            None)
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings):
-        if not means3D.is_cuda:
-            raise RuntimeError("diff_gaussian_rasterization (gpsg): means3D must be a CUDA tensor")
-        dev = means3D.device
-        P = int(means3D.shape[0])
-        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
-        settings = _pack_settings(raster_settings)
-        m3 = _f32c(means3D)
-        col = _f32c(colors_precomp) if colors_precomp.numel() else None
-        shs = _f32c(sh) if sh.numel() else None
-        op = _f32c(opacities)
-        sc = _f32c(scales) if scales.numel() else None
-        ro = _f32c(rotations) if rotations.numel() else None
-        cp = _f32c(cov3Ds_precomp) if cov3Ds_precomp.numel() else None
-        for name, t, k in (("opacities", op, 1), ("scales", sc, 3), ("rotations", ro, 4), ("colors_precomp", col, 3),
-                           ("cov3D_precomp", cp, 6)):
-            if t is not None and (t.numel() != k * P or t.device != dev):
-                raise RuntimeError(f"diff_gaussian_rasterization (gpsg): {name} must hold {P} x {k} values on {dev}, "
-                                   f"got shape {tuple(t.shape)} on {t.device}")
-        if shs is not None and (shs.dim() != 3 or shs.shape[0] != P or shs.shape[2] != 3 or shs.device != dev):
-            raise RuntimeError(f"diff_gaussian_rasterization (gpsg): shs must be [{P}, M, 3] on {dev}")
-        color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
-        ctx.num_rendered, ctx.bufs = _lib.rasterize_forward(settings, color, radii, m3, op, colors_precomp=col, shs=shs,
-                                                            scales=sc, rotations=ro, cov3D_precomp=cp)
-        ctx.settings = settings
-        ctx.save_for_backward(m3, col, shs, op, sc, ro, cp, radii)
-        ctx.mark_non_differentiable(radii)
+        ctx.settings, t = _inputs(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                                  raster_settings)
+        color, radii, _ = _forward(ctx, t, aux=False)
         return color, radii
 
     @staticmethod
     def backward(ctx, grad_out_color, _grad_radii):
-        m3, col, shs, op, sc, ro, cp, radii = ctx.saved_tensors
-        g = _lib.rasterize_backward(ctx.settings, ctx.num_rendered, ctx.bufs, radii, grad_out_color, m3, op,
-                                    colors_precomp=col, shs=shs, scales=sc, rotations=ro, cov3D_precomp=cp,
-                                    want_cov3D=cp is not None)
-        # input order: means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings
-        return (g["dL_dmeans3D"], g["dL_dmeans2D"], g["dL_dsh"], g["dL_dcolors"], g["dL_dopacity"],
-                g["dL_dscales"] if sc is not None else None, g["dL_drots"] if ro is not None else None, g["dL_dcov3D"],
-                None)
+        return _backward(ctx, grad_out_color)
+
+
+class _RasterizeGaussiansAux(torch.autograd.Function):
+    """Aux mode: (color, depth, alpha, radii).  The backward runs the aux entry point on this forward's own buffers (the
+    precondition of gpsg_rasterize_backward_aux); an output that received no gradient gets zeros from autograd."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                raster_settings):
+        ctx.settings, t = _inputs(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                                  raster_settings)
+        color, radii, (depth, alpha) = _forward(ctx, t, aux=True)
+        return color, depth, alpha, radii
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_depth, grad_alpha, _grad_radii):
+        return _backward(ctx, grad_color, grad_depth, grad_alpha)
 
 
 class GaussianRasterizer(nn.Module):

@@ -50,3 +50,14 @@ def render(data, idx, pts_xyz, pts_rgb, rotations, scales, opacity, bg_color):
     image, _radii = _dgr.rasterize_gaussians(pts_xyz, _grad_sink(pts_xyz), _NONE, pts_rgb, opacity, scales, rotations,
                                              _NONE, settings)
     return image
+
+
+def render_aux(data, idx, pts_xyz, pts_rgb, rotations, scales, opacity, bg_color):
+    """`render` that also returns the expected depth and the alpha matte of the novel view: (image [3,H,W],
+    depth [1,H,W], alpha [1,H,W]).  depth = sum_i w_i z_i over the compositing weights w_i (view-space z, 0 where nothing
+    is drawn; divide by alpha for the depth of the surface), alpha = 1 - final transmittance.  All three are
+    differentiable in every input; the image is bit-identical to `render`."""
+    settings = _camera(data['novel_view'], idx, bg_color)
+    image, depth, alpha, _radii = _dgr.rasterize_gaussians_aux(pts_xyz, _grad_sink(pts_xyz), _NONE, pts_rgb, opacity,
+                                                               scales, rotations, _NONE, settings)
+    return image, depth.unsqueeze(0), alpha.unsqueeze(0)

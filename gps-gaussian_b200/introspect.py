@@ -56,14 +56,18 @@ class RasterCall:
         return dict(means3D=i["means3D"], opacities=i["opacity"], colors_precomp=i["colors"], scales=i["scales"],
                     rotations=i["rots"], cov3D_precomp=i.get("cov3D_precomp"))
 
-    def forward(self):
-        self.num_rendered, self.bufs = _lib.rasterize_forward(self.settings, self.color, self.radii, **self._inputs())
+    def forward(self, out_depth=None, out_alpha=None):
+        """out_depth / out_alpha ([H,W], both or neither): aux mode, which also writes depth and alpha."""
+        self.num_rendered, self.bufs = _lib.rasterize_forward(self.settings, self.color, self.radii, out_depth=out_depth,
+                                                              out_alpha=out_alpha, **self._inputs())
         return self.color
 
-    def backward(self, grad_color, want_cov3D=False, deterministic=None):
-        """deterministic: None follows torch.use_deterministic_algorithms, True / False force it (_lib.backward_flags)."""
+    def backward(self, grad_color, want_cov3D=False, deterministic=None, grad_depth=None, grad_alpha=None):
+        """deterministic: None follows torch.use_deterministic_algorithms, True / False force it (_lib.backward_flags).
+        grad_depth / grad_alpha: the aux backward (after an aux forward)."""
         return _lib.rasterize_backward(self.settings, self.num_rendered, self.bufs, self.radii, grad_color,
-                                       want_cov3D=want_cov3D, deterministic=deterministic, **self._inputs())
+                                       want_cov3D=want_cov3D, deterministic=deterministic, grad_depth=grad_depth,
+                                       grad_alpha=grad_alpha, **self._inputs())
 
     def state(self):
         """Saved buffers as torch tensors (views into the scratch buffers)."""

@@ -12,13 +12,15 @@ streams: no per-view gather, no host sync, no H2D camera copies inside the loop.
   * mode="maps": zero-copy -- every view is a `gpsg_rasterize_forward_maps_planned` over the 2*S^2 candidates in place
     (120 MB read at C2, but no construction cost at all: right when only one or two views are rendered per pair).
 
-Images equal `get_novel_calib(ratio)` + `pts2render` per ratio bit for bit in both modes.
+Images equal `get_novel_calib(ratio)` + `pts2render` per ratio bit for bit in both modes.  With aux=True the sweep also
+carries the expected depth and the alpha matte of every view (aux mode of the planned forwards), equal to
+`pts2render_aux` per ratio bit for bit.
 """
 import numpy as np
 import torch
 
 from . import _lib
-from .GaussianRender import _RasterizeMaps, novel_settings
+from .GaussianRender import _RasterizeMaps, _RasterizeMapsAux, novel_settings
 from .novel_calib import calib_from_data
 from .planned import PlannedRasterizer
 
@@ -73,43 +75,63 @@ class NovelViewRenderer:
                      for _ in range(self.n_streams)]
         self.streams = [torch.cuda.Stream(self.dev) for _ in range(self.n_streams)]
 
-    def _enqueue(self, rast, settings, b, out, status_host=None):
+    def _enqueue(self, rast, settings, b, out, status_host=None, depth=None, alpha=None):
+        """depth / alpha ([H,W] each, or None): aux outputs of the view."""
         if self.mode == 'compact':
             f = self.flat[b]
             if f['xyz'].shape[0] == 0:                                  # empty mask: background only (reference P == 0)
                 out.copy_(torch.tensor(self.bg, device=self.dev).view(3, 1, 1).expand_as(out))
+                if depth is not None:
+                    depth.zero_()
+                    alpha.zero_()
                 return
-            rast.forward(settings, f['xyz'], f['rgb'], f['opacity'], f['scale'], f['rot'], out=out, status_host=status_host)
+            rast.forward(settings, f['xyz'], f['rgb'], f['opacity'], f['scale'], f['rot'], out=out, status_host=status_host,
+                         depth=depth, alpha=alpha)
         else:
             m = self.maps[b]
             rast.forward_maps(settings, m['valid'], m['xyz'], m['img'], m['rot'], m['scale'], m['opacity'], out=out,
-                              status_host=status_host)
+                              status_host=status_host, depth=depth, alpha=alpha)
 
     def _settings(self, cal, b, r):
         cam = np.concatenate([cal[k][b, r].reshape(-1) for k in ('world_view_transform', 'full_proj_transform',
                                                                   'camera_center')]).tolist()
         return novel_settings(self.H, self.W, cal['FovX'][b, r], cal['FovY'][b, r], self.bg, cam)
 
-    def _render_exact(self, settings, b, out):
-        """Exact entry point (one host sync, radix fallback for over-long tile lists) for one view of sample b."""
+    def _render_exact(self, settings, b, out, depth=None, alpha=None):
+        """Exact entry point (one host sync, radix fallback for over-long tile lists) for one view of sample b; depth /
+        alpha ([H,W] or None): aux outputs."""
         if self.mode == 'compact':
             f = self.flat[b]
             radii = torch.empty((f['xyz'].shape[0],), dtype=torch.int32, device=self.dev)
             _lib.rasterize_forward(settings, out, radii, f['xyz'], f['opacity'], colors_precomp=f['rgb'],
-                                   scales=f['scale'], rotations=f['rot'])
+                                   scales=f['scale'], rotations=f['rot'], out_depth=depth, out_alpha=alpha)
         else:
             m = self.maps[b]
             args = []
             for v in range(2):
                 args += [m['valid'][v], m['xyz'][v], m['img'][v], m['rot'][v], m['scale'][v], m['opacity'][v]]
             with torch.no_grad():
-                out.copy_(_RasterizeMaps.apply([settings], *args)[0])
+                if depth is None:
+                    out.copy_(_RasterizeMaps.apply([settings], *args)[0])
+                else:
+                    i, d, a = _RasterizeMapsAux.apply([settings], *args)
+                    out.copy_(i[0]); depth.copy_(d[0, 0]); alpha.copy_(a[0, 0])
 
-    def render(self, ratios, out=None, check=True):
+    def render(self, ratios, out=None, check=True, aux=False):
+        """Images [B, len(ratios), 3, H, W].  aux=True: returns (images, depth, alpha), depth and alpha
+        [B, len(ratios), 1, H, W] (expected view-space depth and alpha matte of every view); self.last_aux holds them
+        too, for check=False."""
         ratios = [float(r) for r in ratios]
         cal = calib_from_data(self.data, self.opt, ratios, *self.keys)
         if out is None:
             out = torch.empty((self.bs, len(ratios), 3, self.H, self.W), dtype=torch.float32, device=self.dev)
+        depth = alpha = None
+        if aux:
+            new = lambda: torch.empty((self.bs, len(ratios), 1, self.H, self.W), dtype=torch.float32, device=self.dev)
+            depth, alpha = new(), new()
+        self.last_aux = (depth, alpha)
+        maps = lambda b, r: (depth[b, r, 0], alpha[b, r, 0]) if aux else (None, None)
+        result = lambda: (out, depth, alpha) if aux else out
         cur = torch.cuda.current_stream(self.dev)
         for s in self.streams:
             s.wait_stream(cur)
@@ -118,12 +140,12 @@ class NovelViewRenderer:
         for k, (b, r) in enumerate(jobs):
             j = k % self.n_streams
             with torch.cuda.stream(self.streams[j]):
-                self._enqueue(self.rast[j], self._settings(cal, b, r), b, out[b, r], status[k])
+                self._enqueue(self.rast[j], self._settings(cal, b, r), b, out[b, r], status[k], *maps(b, r))
         for s in self.streams:
             cur.wait_stream(s)
         self.last_status = status
         if not check:
-            return out                                                  # fully asynchronous; caller checks last_status
+            return result()                                             # fully asynchronous; caller checks last_status
         torch.cuda.current_stream(self.dev).synchronize()
         # status[k] = (num_rendered, longest tile list, overflow flag) of job k.  Two different overflows (ADVICE r1):
         #  * more pairs than the binning buffer holds -> size the buffer from the reported count and render again;
@@ -135,25 +157,30 @@ class NovelViewRenderer:
                 continue
             settings = self._settings(cal, b, r)
             if max_tile > _MAX_TILE_SORT:
-                self._render_exact(settings, b, out[b, r])
+                self._render_exact(settings, b, out[b, r], *maps(b, r))
                 continue
             rast = self.rast[0]
             rast.grow(needed_pairs=n_pairs)
             rast.status_host.zero_()
-            self._enqueue(rast, settings, b, out[b, r])
+            self._enqueue(rast, settings, b, out[b, r], None, *maps(b, r))
             torch.cuda.synchronize(self.dev)
             if not rast.ok():
                 st = rast.status()
                 if st["max_tile"] > _MAX_TILE_SORT:
-                    self._render_exact(settings, b, out[b, r])
+                    self._render_exact(settings, b, out[b, r], *maps(b, r))
                 else:
                     raise _lib.GpsgError(f"novel view render: {st['num_rendered']} pairs do not fit capacity {rast.capacity}")
         torch.cuda.synchronize(self.dev)
-        return out
+        return result()
 
 
-def render_novel_views(data, opt, ratios, bg_color, intr_key='intr', extr_key='extr', streams=4, mode='compact'):
-    """data['novel_view']['img_pred_sweep'] = [B, len(ratios), 3, H, W]; returns data."""
-    data['novel_view']['img_pred_sweep'] = NovelViewRenderer(data, opt, bg_color, intr_key, extr_key, streams,
-                                                                mode=mode).render(ratios)
+def render_novel_views(data, opt, ratios, bg_color, intr_key='intr', extr_key='extr', streams=4, mode='compact', aux=False):
+    """data['novel_view']['img_pred_sweep'] = [B, len(ratios), 3, H, W]; returns data.  aux=True also sets
+    ['depth_pred_sweep'] and ['alpha_pred_sweep'], [B, len(ratios), 1, H, W]."""
+    nv = data['novel_view']
+    res = NovelViewRenderer(data, opt, bg_color, intr_key, extr_key, streams, mode=mode).render(ratios, aux=aux)
+    if aux:
+        nv['img_pred_sweep'], nv['depth_pred_sweep'], nv['alpha_pred_sweep'] = res
+    else:
+        nv['img_pred_sweep'] = res
     return data

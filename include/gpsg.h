@@ -186,6 +186,76 @@ GPSG_API int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* settings,
                                              float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
                                              int flags);
 
+/* ---- aux mode: expected depth and alpha beside the colour image ---------------------------------------------------
+ * Each forward above has an _aux form with two more outputs after out_color, out_depth[H,W] and out_alpha[H,W] (fp32,
+ * both NULL -- then it is exactly the forward without _aux, which is that form with NULL -- or both set):
+ *   alpha = 1 - T_final (accumulated opacity; exactly 1 - the transmittance the backward reads),
+ *   depth = sum_i w_i z_i,  w_i = alpha_i T_i the compositing weight and z_i the view-space depth of Gaussian i (the
+ *           key the tile lists are sorted by).  Not normalised by alpha and without background (depth = 0 where nothing
+ *           is drawn), i.e. depth is a fourth colour channel whose colour is z and whose background is 0.
+ * The colour image, radii and the saved buffers are bit-identical to the forward without _aux on the same inputs.  The
+ * buffers have the same sizes (z is read from the geometry buffer, so the planned forwards take the same
+ * gpsg_raster_binning_bytes capacity), and the sync-free / overflow contract of the planned forms is unchanged.
+ * maps: gpsg_rasterize_forward_maps_begin is shared; only _finish has an _aux form. */
+GPSG_API int gpsg_rasterize_forward_aux(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
+                                        const float* means3D, const float* colors_precomp, const float* shs,
+                                        const float* opacities, const float* scales, const float* rotations,
+                                        const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
+                                        int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
+                                        gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
+                                        void* image_user, int32_t* num_rendered);
+GPSG_API int gpsg_rasterize_forward_maps_finish_aux(const GpsgRasterSettings* settings, int device, void* stream,
+                                                    int pixels_per_view, const uint8_t* const* valid,
+                                                    const float* const* xyz, const float* const* img,
+                                                    const float* const* rot, const float* const* scale,
+                                                    const float* const* opacity, float* out_color, float* out_depth,
+                                                    float* out_alpha, int32_t* radii, void* geom_buffer,
+                                                    void* image_buffer, gpsg_alloc_fn binning_alloc, void* binning_user,
+                                                    const uint32_t* totals_host, int32_t* num_rendered);
+GPSG_API int gpsg_rasterize_forward_planned_aux(const GpsgRasterSettings* settings, int device, void* stream, int P,
+                                                const float* means3D, const float* colors_precomp, const float* opacities,
+                                                const float* scales, const float* rotations, const float* cov3D_precomp,
+                                                float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                                void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
+                                                void* image_buffer, uint32_t* status_host);
+GPSG_API int gpsg_rasterize_forward_maps_planned_aux(const GpsgRasterSettings* settings, int device, void* stream,
+                                                     int pixels_per_view, const uint8_t* const* valid,
+                                                     const float* const* xyz, const float* const* img,
+                                                     const float* const* rot, const float* const* scale,
+                                                     const float* const* opacity, float* out_color, float* out_depth,
+                                                     float* out_alpha, int32_t* radii, void* geom_buffer,
+                                                     void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
+                                                     uint32_t* status_host);
+/* Backward of the aux forwards: the _ex backwards with dL_dout_depth[H,W] and dL_dout_alpha[H,W] after dL_dout_color
+ * (both NULL -- then it is exactly the _ex backward, which is this with NULL -- or both set; either may hold zeros).
+ * Precondition: with the aux gradients set, the buffers (and num_rendered) must come from an _aux forward of the same
+ * inputs whose depth and alpha outputs those gradients belong to.  The depth gradient reaches dL_dmeans3D (maps:
+ * dL_dxyz) through the view matrix's third row; the alpha gradient reaches the opacities and the geometry through the
+ * compositing weights.  flags as for the _ex backwards (GPSG_BWD_DETERMINISTIC or 0).  The workspace must hold the
+ * _aux_workspace_bytes size: with GPSG_BWD_DETERMINISTIC the partial sums are 8 x 10 floats per pair (321 B per pair
+ * plus alignment); without it the size equals the _ex size. */
+GPSG_API size_t gpsg_rasterize_backward_aux_workspace_bytes(int P, int64_t num_rendered, int flags);
+GPSG_API int gpsg_rasterize_backward_aux(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
+                                         int32_t num_rendered, const float* means3D, const float* colors_precomp,
+                                         const float* shs, const float* opacities, const float* scales,
+                                         const float* rotations, const float* cov3D_precomp, const int32_t* radii,
+                                         const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
+                                         const float* dL_dout_color, const float* dL_dout_depth,
+                                         const float* dL_dout_alpha, float* dL_dmeans2D, float* dL_dcolors,
+                                         float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
+                                         float* dL_dscales, float* dL_drotations, void* workspace, int flags);
+GPSG_API size_t gpsg_rasterize_backward_maps_aux_workspace_bytes(int pixels_per_view, int64_t num_rendered, int flags);
+GPSG_API int gpsg_rasterize_backward_maps_aux(const GpsgRasterSettings* settings, int device, void* stream,
+                                              int pixels_per_view, int32_t num_rendered, const uint8_t* const* valid,
+                                              const float* const* xyz, const float* const* img, const float* const* rot,
+                                              const float* const* scale, const float* const* opacity,
+                                              const int32_t* radii, const void* geom_buffer, const void* binning_buffer,
+                                              const void* image_buffer, const float* dL_dout_color,
+                                              const float* dL_dout_depth, const float* dL_dout_alpha,
+                                              float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
+                                              float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
+                                              int flags);
+
 /* ---- replaces _C.mark_visible : present[P] (uint8) = view-space z > 0.2 ---------------------- */
 GPSG_API int gpsg_mark_visible(int device, void* stream, int P, const float* means3D, const float* viewmatrix_host16,
                       uint8_t* present);

@@ -2,7 +2,9 @@
 """Per-kernel times of the rasterizer forward + backward on the C2 scene (CUDA events around each launch, serialised on
 one stream) -- the quick loop used while tuning kernels:  python tools/stage_times.py [--reps 50] [--seeds 1314 1315]
 --deterministic times the deterministic backward (GPSG_BWD_DETERMINISTIC: render_backward_det, render_backward_det_reduce)
-instead of the default one and adds its workspace bytes per view."""
+instead of the default one and adds its workspace bytes per view.  --aux times aux mode (depth and alpha outputs, and the
+backward of all three images) under the same stage names.  --alternate R runs R rounds that alternate default and aux
+(same scenes, same process) and prints one line per round and mode."""
 import argparse
 import json
 import os
@@ -21,33 +23,51 @@ ap.add_argument("--res", type=int, default=1024)
 ap.add_argument("--seeds", type=int, nargs="*", default=[1314, 1315, 1316, 1317])
 ap.add_argument("--no-backward", action="store_true")
 ap.add_argument("--deterministic", action="store_true")
+ap.add_argument("--aux", action="store_true")
+ap.add_argument("--alternate", type=int, default=0)
 a = ap.parse_args()
 dev = torch.device("cuda", 0)
 calls = [RasterCall(sc, to_device(sc, dev), dev) for sc in (synth.stereo_pair_scene(a.res, seed=s) for s in a.seeds)]
 g = torch.randn(3, a.res, a.res, device=dev)
-for c in calls:
-    c.forward()
+gD, gA = torch.randn(a.res, a.res, device=dev), torch.randn(a.res, a.res, device=dev)
+depth, alpha = torch.empty(a.res, a.res, device=dev), torch.empty(a.res, a.res, device=dev)
+
+
+def step(c, aux):
+    c.forward(*((depth, alpha) if aux else (None, None)))
     if not a.no_backward:
-        c.backward(g, deterministic=a.deterministic)
-torch.cuda.synchronize()
-_lib.profile_enable(True)
-_lib.profile_read()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-for _ in range(a.reps):
+        c.backward(g, deterministic=a.deterministic, **(dict(grad_depth=gD, grad_alpha=gA) if aux else {}))
+
+
+def run(aux):
     for c in calls:
-        c.forward()
-        if not a.no_backward:
-            c.backward(g, deterministic=a.deterministic)
-e1.record()
-torch.cuda.synchronize()
-prof = _lib.profile_read()
-_lib.profile_enable(False)
-out = {k: round(v["ms"] / max(v["calls"], 1) * 1e3, 1) for k, v in prof.items() if v["calls"]}
-out["total_us_per_view"] = round(e0.elapsed_time(e1) * 1e3 / (a.reps * len(calls)), 1)
-out["N_dup_mean"] = sum(c.num_rendered for c in calls) / len(calls)
-flags = _lib.BWD_DETERMINISTIC if a.deterministic else 0
-out["bwd_workspace_bytes_mean"] = sum(_lib.lib.gpsg_rasterize_backward_workspace_bytes_ex(c.P, c.num_rendered, flags)
-                                      for c in calls) / len(calls)
-out["gpu"] = torch.cuda.get_device_name(0)
-print(json.dumps(out))
+        step(c, aux)
+    torch.cuda.synchronize()
+    _lib.profile_enable(True)
+    _lib.profile_read()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(a.reps):
+        for c in calls:
+            step(c, aux)
+    e1.record()
+    torch.cuda.synchronize()
+    prof = _lib.profile_read()
+    _lib.profile_enable(False)
+    out = {k: round(v["ms"] / max(v["calls"], 1) * 1e3, 1) for k, v in prof.items() if v["calls"]}
+    out["total_us_per_view"] = round(e0.elapsed_time(e1) * 1e3 / (a.reps * len(calls)), 1)
+    out["N_dup_mean"] = sum(c.num_rendered for c in calls) / len(calls)
+    flags = _lib.BWD_DETERMINISTIC if a.deterministic else 0
+    size = _lib.lib.gpsg_rasterize_backward_aux_workspace_bytes if aux else _lib.lib.gpsg_rasterize_backward_workspace_bytes_ex
+    out["bwd_workspace_bytes_mean"] = sum(size(c.P, c.num_rendered, flags) for c in calls) / len(calls)
+    out["aux"] = aux
+    out["gpu"] = torch.cuda.get_device_name(0)
+    return out
+
+
+if a.alternate:
+    for r in range(a.alternate):
+        for aux in (False, True):
+            print(json.dumps(dict(run(aux), round=r)))
+else:
+    print(json.dumps(run(a.aux)))
