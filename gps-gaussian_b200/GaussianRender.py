@@ -7,6 +7,8 @@ maps in place (`gpsg_rasterize_forward_maps_begin` / `_finish`): invalid pixels 
 kernel, colours are img*0.5+0.5 on the fly, and the backward writes gradients directly in map layout.  Same signature,
 same result (Gaussian order = lmain pixels then rmain pixels, exactly the order of the reference's gather + concat).
 `pts2render_gather` keeps the reference's op-by-op data flow (gather -> `render`) for comparison.
+`pts2render_ex(data, bg_color, aux=..., antialiasing=...)` is the one implementation behind `pts2render` and
+`pts2render_aux`; antialiasing=True renders with the opacity-compensated screen-space filter (GPSG_FWD_ANTIALIAS).
 """
 import ctypes as C
 import math
@@ -46,8 +48,9 @@ def _sample_maps(maps, dev):
     return S2, (valid, xyz, img, rot, scale, opac)
 
 
-def _maps_forward(ctx, settings_list, maps, aux):
-    """Forward of `_RasterizeMaps` (aux: `_RasterizeMapsAux`, which also writes depth and alpha [B,1,H,W])."""
+def _maps_forward(ctx, settings_list, flags, maps, aux):
+    """Forward of `_RasterizeMaps` (aux: `_RasterizeMapsAux`, which also writes depth and alpha [B,1,H,W]); `flags`: the
+    GPSG_FWD_* word of the projection (`_begin`), which the backward follows through the saved image buffers."""
     B = len(settings_list)
     assert len(maps) == 12 * B
     dev = maps[1].device
@@ -68,12 +71,12 @@ def _maps_forward(ctx, settings_list, maps, aux):
         _lib.begin_alloc(dev)
         try:
             with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_rasterize_forward_maps_begin(
+                rc = _lib.lib.gpsg_rasterize_forward_maps_begin_ex(
                     C.byref(st), idx, sptr, S2, *ptrs, C.c_void_p(radii.data_ptr()), _lib.ALLOC_CB, C.c_void_p(1),
-                    _lib.ALLOC_CB, C.c_void_p(3), C.c_void_p(totals[b].data_ptr()))
+                    _lib.ALLOC_CB, C.c_void_p(3), C.c_void_p(totals[b].data_ptr()), int(flags))
         finally:
             bufs = _lib.end_alloc()
-        _lib.check(rc, "gpsg_rasterize_forward_maps_begin")
+        _lib.check(rc, "gpsg_rasterize_forward_maps_begin_ex")
         per.append(dict(S2=S2, tensors=tensors, ptrs=ptrs, radii=radii, geom=bufs.get(1), image=bufs.get(3)))
     torch.cuda.current_stream(dev).synchronize()           # the ONE host synchronisation of the batch
     ctx.per = []
@@ -104,7 +107,7 @@ def _maps_backward(ctx, grad_out, grad_depth=None, grad_alpha=None):
     """Backward of both map Functions: gradients in map layout; with grad_depth / grad_alpha [B,1,H,W] the aux entry
     point on the aux forward's own buffers."""
     aux = grad_depth is not None
-    grads = [None]
+    grads = [None, None]                                   # settings_list, flags
     flags = _lib.backward_flags()
     dev = grad_out.device
     idx, sptr = _lib.device_stream(dev)
@@ -132,14 +135,14 @@ def _maps_backward(ctx, grad_out, grad_depth=None, grad_alpha=None):
 
 
 class _RasterizeMaps(torch.autograd.Function):
-    """(settings_list, *12 maps per sample) -> images [B,3,H,W] with ONE host synchronisation for the whole batch: every
+    """(settings_list, forward flags, *12 maps per sample) -> images [B,3,H,W] with ONE host synchronisation for the whole batch: every
     sample's projection / tile counting is enqueued first (`gpsg_rasterize_forward_maps_begin`), the stream is synchronised
     once, then every sample is binned, sorted and composited (`..._finish`).  The reference loops over the samples with one
     synchronisation each (lib/GaussianRender.py:8; upstream reads num_rendered per call)."""
 
     @staticmethod
-    def forward(ctx, settings_list, *maps):
-        return _maps_forward(ctx, settings_list, maps, aux=False)
+    def forward(ctx, settings_list, flags, *maps):
+        return _maps_forward(ctx, settings_list, flags, maps, aux=False)
 
     @staticmethod
     def backward(ctx, grad_out):
@@ -151,8 +154,8 @@ class _RasterizeMapsAux(torch.autograd.Function):
     the images are bit-identical to `_RasterizeMaps`'."""
 
     @staticmethod
-    def forward(ctx, settings_list, *maps):
-        return _maps_forward(ctx, settings_list, maps, aux=True)
+    def forward(ctx, settings_list, flags, *maps):
+        return _maps_forward(ctx, settings_list, flags, maps, aux=True)
 
     @staticmethod
     def backward(ctx, grad_out, grad_depth, grad_alpha):
@@ -179,7 +182,7 @@ def novel_settings(height, width, fovx, fovy, bg_color, cam):
 
 def pts2render(data, bg_color):
     """Whole batch with one host synchronisation (`_RasterizeMaps`)."""
-    return _pts2render(data, bg_color, aux=False)
+    return pts2render_ex(data, bg_color)
 
 
 def pts2render_aux(data, bg_color):
@@ -187,10 +190,14 @@ def pts2render_aux(data, bg_color):
     and ['alpha_pred'] (accumulated opacity: the foreground matte of the novel view), both [B,1,H,W] and differentiable,
     from the same forward and the same single host synchronisation (`_RasterizeMapsAux`).  img_pred is bit-identical to
     `pts2render`'s.  (A separate name keeps `pts2render`'s signature the reference's.)"""
-    return _pts2render(data, bg_color, aux=True)
+    return pts2render_ex(data, bg_color, aux=True)
 
 
-def _pts2render(data, bg_color, aux):
+def pts2render_ex(data, bg_color, *, aux=False, antialiasing=False):
+    """`pts2render` (aux=False) or `pts2render_aux` (aux=True); antialiasing=True renders every sample with the
+    opacity-compensated screen-space filter (upstream's `antialiasing` setting: each splat's opacity is scaled so its
+    integrated alpha does not grow with the fixed 0.3 px^2 dilation; conics, radii and tile lists are unchanged) and the
+    backward differentiates that filter.  Same single host synchronisation per batch."""
     nv = data['novel_view']
     bs = data['lmain']['img'].shape[0]
     maps, settings = [], []
@@ -202,10 +209,11 @@ def _pts2render(data, bg_color, aux):
         cam = torch.cat([nv[k][i].detach().reshape(-1).float()
                          for k in ('world_view_transform', 'full_proj_transform', 'camera_center')]).cpu().tolist()
         settings.append(novel_settings(nv['height'][i], nv['width'][i], nv['FovX'][i], nv['FovY'][i], bg_color, cam))
+    flags = _lib.forward_flags(antialiasing)
     if aux:
-        nv['img_pred'], nv['depth_pred'], nv['alpha_pred'] = _RasterizeMapsAux.apply(settings, *maps)
+        nv['img_pred'], nv['depth_pred'], nv['alpha_pred'] = _RasterizeMapsAux.apply(settings, flags, *maps)
     else:
-        nv['img_pred'] = _RasterizeMaps.apply(settings, *maps)
+        nv['img_pred'] = _RasterizeMaps.apply(settings, flags, *maps)
     return data
 
 

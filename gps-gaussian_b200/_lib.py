@@ -125,6 +125,14 @@ lib.gpsg_rasterize_backward_maps_aux_workspace_bytes.argtypes = [_i, _i64, _i]
 lib.gpsg_rasterize_backward_maps_aux.restype = _i
 lib.gpsg_rasterize_backward_maps_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, C.c_int32] + [_pp] * 6 + [
     _vp] * 7 + [_pp] * 5 + [_vp, _i]
+lib.gpsg_rasterize_forward_ex.restype = _i
+lib.gpsg_rasterize_forward_ex.argtypes = lib.gpsg_rasterize_forward_aux.argtypes + [_i]
+lib.gpsg_rasterize_forward_maps_begin_ex.restype = _i
+lib.gpsg_rasterize_forward_maps_begin_ex.argtypes = lib.gpsg_rasterize_forward_maps_begin.argtypes + [_i]
+lib.gpsg_rasterize_forward_planned_ex.restype = _i
+lib.gpsg_rasterize_forward_planned_ex.argtypes = lib.gpsg_rasterize_forward_planned_aux.argtypes + [_i]
+lib.gpsg_rasterize_forward_maps_planned_ex.restype = _i
+lib.gpsg_rasterize_forward_maps_planned_ex.argtypes = lib.gpsg_rasterize_forward_maps_planned_aux.argtypes + [_i]
 lib.gpsg_corr_build_pyramid.restype = _i
 lib.gpsg_corr_build_pyramid.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, C.POINTER(C.c_void_p), _i]
 lib.gpsg_corr_build_backward.restype = _i
@@ -167,9 +175,16 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_rasterize_forward_aux", "gpsg_rasterize_forward_maps_finish_aux", "gpsg_rasterize_forward_planned_aux",
             "gpsg_rasterize_forward_maps_planned_aux", "gpsg_rasterize_backward_aux_workspace_bytes",
             "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
-            "gpsg_rasterize_backward_maps_aux"]
+            "gpsg_rasterize_backward_maps_aux", "gpsg_rasterize_forward_ex", "gpsg_rasterize_forward_maps_begin_ex",
+            "gpsg_rasterize_forward_planned_ex", "gpsg_rasterize_forward_maps_planned_ex"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
+FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)
+
+
+def forward_flags(antialiasing=False):
+    """The `flags` word of the gpsg_*_forward*_ex entry points: GPSG_FWD_ANTIALIAS when `antialiasing`, else 0."""
+    return FWD_ANTIALIAS if antialiasing else 0
 
 
 def check(rc, what):
@@ -217,27 +232,27 @@ def _ptr(t):
 
 
 def rasterize_forward(settings, out_color, radii, means3D, opacities, colors_precomp=None, shs=None, scales=None,
-                      rotations=None, cov3D_precomp=None, out_depth=None, out_alpha=None):
+                      rotations=None, cov3D_precomp=None, out_depth=None, out_alpha=None, antialiasing=False):
     """One forward through the exact entry point gpsg_rasterize_forward: one host synchronisation, and the global radix
     fallback takes tile lists of any length.  Inputs are contiguous fp32 tensors on one CUDA device, absent ones None.
     Writes out_color [3,H,W] and radii [P]; returns (num_rendered, (geom, binning, image)), the buffers the backward
     reads.  out_depth / out_alpha ([H,W] fp32, both or neither): aux mode (gpsg_rasterize_forward_aux), which also writes
-    the expected depth and the accumulated opacity."""
+    the expected depth and the accumulated opacity.  antialiasing: the opacity-compensated screen-space filter
+    (GPSG_FWD_ANTIALIAS); the backward of these buffers follows it without being told.  Runs gpsg_rasterize_forward_ex."""
     if (out_depth is None) != (out_alpha is None):
         raise ValueError("out_depth and out_alpha must be given together")
     dev = means3D.device
     idx, stream = device_stream(dev)
     n = C.c_int32(0)
-    aux = [] if out_depth is None else [_ptr(out_depth), _ptr(out_alpha)]
-    fn = lib.gpsg_rasterize_forward_aux if aux else lib.gpsg_rasterize_forward
+    fn = lib.gpsg_rasterize_forward_ex
     begin_alloc(dev)
     try:
         with torch.cuda.device(dev):
             rc = fn(
                 C.byref(settings), idx, stream, int(means3D.shape[0]), int(shs.shape[1]) if shs is not None else 0,
                 _ptr(means3D), _ptr(colors_precomp), _ptr(shs), _ptr(opacities), _ptr(scales), _ptr(rotations),
-                _ptr(cov3D_precomp), _ptr(out_color), *aux, _ptr(radii), ALLOC_CB, C.c_void_p(1), ALLOC_CB, C.c_void_p(2),
-                ALLOC_CB, C.c_void_p(3), C.byref(n))
+                _ptr(cov3D_precomp), _ptr(out_color), _ptr(out_depth), _ptr(out_alpha), _ptr(radii), ALLOC_CB, C.c_void_p(1),
+                ALLOC_CB, C.c_void_p(2), ALLOC_CB, C.c_void_p(3), C.byref(n), forward_flags(antialiasing))
     finally:
         bufs = end_alloc()
     check(rc, fn.__name__)

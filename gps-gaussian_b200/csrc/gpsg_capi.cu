@@ -205,7 +205,7 @@ int gpsg_version(void) { return 90; }
 // `src` says where the Gaussians come from (AoS tensors or maps).
 static int forward_exact_begin(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, const GaussianSrc& src,
                                int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn image_alloc,
-                               void* image_user, uint32_t* totals_host, void** geom_out, void** image_out) {
+                               void* image_user, uint32_t* totals_host, void** geom_out, void** image_out, int flags) {
     GPSG_CUDA(cudaSetDevice(device));
     const Camera cam = make_camera(*s);
     const size_t scan_bytes = scan_temp_bytes(P);
@@ -220,7 +220,7 @@ static int forward_exact_begin(const GpsgRasterSettings* s, int device, cudaStre
     int rc = GPSG_OK;
     GPSG_CUDA(cudaMemsetAsync(im.tile_count, 0, (size_t)((char*)(im.totals + 64) - (char*)im.tile_count), stream));
     if (P > 0) {   // projection + pairs-per-tile histogram; its last CTA also scans the histogram into tile ranges
-        { StageTimer t(ST_PREPROCESS, stream, 1); rc = launch_preprocess(cam, P, src, radii, g, im, 0u, stream); }
+        { StageTimer t(ST_PREPROCESS, stream, 1); rc = launch_preprocess(cam, P, src, radii, g, im, 0u, flags, stream); }
         if (rc) return rc;
         GPSG_CUDA(cudaMemcpyAsync(totals_host, im.totals, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
     } else {
@@ -282,6 +282,11 @@ static int forward_exact_finish(const GpsgRasterSettings* s, int device, cudaStr
     return GPSG_OK;
 }
 
+static int check_fwd_flags(int flags) {
+    GPSG_REQUIRE((flags & ~GPSG_FWD_ANTIALIAS) == 0, "unknown forward flag bits (GPSG_FWD_ANTIALIAS is the only flag)");
+    return GPSG_OK;
+}
+
 static int check_aux_outputs(const float* out_depth, const float* out_alpha) {
     GPSG_REQUIRE((out_depth == nullptr) == (out_alpha == nullptr), "out_depth and out_alpha must both be NULL or both be set");
     return GPSG_OK;
@@ -304,6 +309,19 @@ int gpsg_rasterize_forward_aux(const GpsgRasterSettings* s, int device, void* st
                                const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
                                int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
                                void* binning_user, gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered) {
+    return gpsg_rasterize_forward_ex(s, device, stream_, P, sh_M, means3D, colors_precomp, shs, opacities, scales, rotations,
+                                     cov3D_precomp, out_color, out_depth, out_alpha, radii, geom_alloc, geom_user,
+                                     binning_alloc, binning_user, image_alloc, image_user, num_rendered, 0);
+}
+
+int gpsg_rasterize_forward_ex(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
+                              const float* means3D, const float* colors_precomp, const float* shs,
+                              const float* opacities, const float* scales, const float* rotations,
+                              const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
+                              int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
+                              void* binning_user, gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered,
+                              int flags) {
+    if (int rc_f = check_fwd_flags(flags)) return rc_f;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(P >= 0, "P < 0");
     GPSG_REQUIRE(s->image_width > 0 && s->image_height > 0, "image size must be positive");
@@ -328,7 +346,7 @@ int gpsg_rasterize_forward_aux(const GpsgRasterSettings* s, int device, void* st
     GPSG_REQUIRE(slot != nullptr, "cudaHostAlloc failed");
     void *geom_base = nullptr, *img_base = nullptr;
     int rc = forward_exact_begin(s, device, stream, P, src, radii, geom_alloc, geom_user, image_alloc, image_user, slot,
-                                 &geom_base, &img_base);
+                                 &geom_base, &img_base, flags);
     if (rc) return rc;
     if (P > 0) GPSG_CUDA(cudaStreamSynchronize(stream));
     return forward_exact_finish(s, device, stream, P, sh_M, src, shs, out_color, out_depth, out_alpha, radii, geom_base,
@@ -360,6 +378,16 @@ int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* s, int device, v
                                       const float* const* rot, const float* const* scale, const float* const* opacity,
                                       int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn image_alloc,
                                       void* image_user, uint32_t* totals_host) {
+    return gpsg_rasterize_forward_maps_begin_ex(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity, radii,
+                                                geom_alloc, geom_user, image_alloc, image_user, totals_host, 0);
+}
+
+int gpsg_rasterize_forward_maps_begin_ex(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                         const uint8_t* const* valid, const float* const* xyz, const float* const* img,
+                                         const float* const* rot, const float* const* scale, const float* const* opacity,
+                                         int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
+                                         gpsg_alloc_fn image_alloc, void* image_user, uint32_t* totals_host, int flags) {
+    if (int rc_f = check_fwd_flags(flags)) return rc_f;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(s->image_width > 0 && s->image_height > 0, "image size must be positive");
     GPSG_REQUIRE(radii && geom_alloc && image_alloc && totals_host, "radii / allocator / totals_host is NULL");
@@ -367,7 +395,7 @@ int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* s, int device, v
     if (rc) return rc;
     return forward_exact_begin(s, device, (cudaStream_t)stream_, 2 * pixels_per_view,
                                maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), radii, geom_alloc, geom_user,
-                               image_alloc, image_user, totals_host, nullptr, nullptr);
+                               image_alloc, image_user, totals_host, nullptr, nullptr, flags);
 }
 
 int gpsg_rasterize_forward_maps_finish(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
@@ -409,7 +437,8 @@ const uint32_t* gpsg_raster_status_ptr(const void* image_buffer, int W, int H) {
 
 static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, const GaussianSrc& src,
                                   float* out_color, float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
-                                  void* binning_buffer, int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
+                                  void* binning_buffer, int64_t capacity_pairs, void* image_buffer, uint32_t* status_host,
+                                  int flags) {
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     if (int rc_aux = check_aux_outputs(out_depth, out_alpha)) return rc_aux;
     GPSG_REQUIRE(P > 0, "planned forward needs P > 0");
@@ -426,7 +455,7 @@ static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaS
     b.vals = nullptr;
     int rc = GPSG_OK;
     GPSG_CUDA(cudaMemsetAsync(im.tile_count, 0, (size_t)((char*)(im.totals + 64) - (char*)im.tile_count), stream));
-    { StageTimer t(ST_PREPROCESS, stream, 1); rc = launch_preprocess(cam, P, src, radii, g, im, (uint32_t)capacity_pairs, stream); }
+    { StageTimer t(ST_PREPROCESS, stream, 1); rc = launch_preprocess(cam, P, src, radii, g, im, (uint32_t)capacity_pairs, flags, stream); }
     if (rc) return rc;
     if (status_host) GPSG_CUDA(cudaMemcpyAsync(status_host, im.totals, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
     { StageTimer t(ST_SCATTER, stream, 1); rc = launch_bucket_scatter(cam, P, radii, g, b, im, stream); }
@@ -453,6 +482,18 @@ int gpsg_rasterize_forward_planned_aux(const GpsgRasterSettings* s, int device, 
                                        float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
                                        void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
                                        uint32_t* status_host) {
+    return gpsg_rasterize_forward_planned_ex(s, device, stream_, P, means3D, colors_precomp, opacities, scales, rotations,
+                                             cov3D_precomp, out_color, out_depth, out_alpha, radii, geom_buffer,
+                                             binning_buffer, capacity_pairs, image_buffer, status_host, 0);
+}
+
+int gpsg_rasterize_forward_planned_ex(const GpsgRasterSettings* s, int device, void* stream_, int P, const float* means3D,
+                                      const float* colors_precomp, const float* opacities, const float* scales,
+                                      const float* rotations, const float* cov3D_precomp, float* out_color,
+                                      float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
+                                      void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
+                                      uint32_t* status_host, int flags) {
+    if (int rc_f = check_fwd_flags(flags)) return rc_f;
     GPSG_REQUIRE(means3D && colors_precomp && opacities, "a required pointer is NULL");
     GPSG_REQUIRE(((scales != nullptr && rotations != nullptr) != (cov3D_precomp != nullptr)),
                  "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
@@ -460,7 +501,7 @@ int gpsg_rasterize_forward_planned_aux(const GpsgRasterSettings* s, int device, 
                                   aos_src(means3D, cov3D_precomp ? nullptr : scales, cov3D_precomp ? nullptr : rotations,
                                           opacities, colors_precomp, cov3D_precomp),
                                   out_color, out_depth, out_alpha, radii, geom_buffer, binning_buffer, capacity_pairs,
-                                  image_buffer, status_host);
+                                  image_buffer, status_host, flags);
 }
 
 int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
@@ -479,11 +520,24 @@ int gpsg_rasterize_forward_maps_planned_aux(const GpsgRasterSettings* s, int dev
                                             const float* const* opacity, float* out_color, float* out_depth,
                                             float* out_alpha, int32_t* radii, void* geom_buffer, void* binning_buffer,
                                             int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
+    return gpsg_rasterize_forward_maps_planned_ex(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity,
+                                                  out_color, out_depth, out_alpha, radii, geom_buffer, binning_buffer,
+                                                  capacity_pairs, image_buffer, status_host, 0);
+}
+
+int gpsg_rasterize_forward_maps_planned_ex(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                           const uint8_t* const* valid, const float* const* xyz, const float* const* img,
+                                           const float* const* rot, const float* const* scale, const float* const* opacity,
+                                           float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                           void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
+                                           void* image_buffer, uint32_t* status_host, int flags) {
+    if (int rc_f = check_fwd_flags(flags)) return rc_f;
     int rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
     if (rc) return rc;
     return forward_planned_common(s, device, (cudaStream_t)stream_, 2 * pixels_per_view,
                                   maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), out_color, out_depth,
-                                  out_alpha, radii, geom_buffer, binning_buffer, capacity_pairs, image_buffer, status_host);
+                                  out_alpha, radii, geom_buffer, binning_buffer, capacity_pairs, image_buffer, status_host,
+                                  flags);
 }
 
 // Backward workspace: [3 x float4 packed accumulator rows][3 floats: dL_dcolors (SH path) or dL_dmeans2D (maps)] per
@@ -550,8 +604,8 @@ static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t
         if (rc) return rc;
     }
     { StageTimer t(ST_PREPROCESS_BWD, stream, 1);
-      rc = launch_preprocess_backward(cam, P, src, radii, gst.conic_opacity, grad_acc, dL_dmeans2D, dL_dcolors, out, aux.on(),
-                                      stream); }
+      rc = launch_preprocess_backward(cam, P, src, radii, gst.conic_opacity, im.totals + kFwdFlagsWord, grad_acc, dL_dmeans2D,
+                                      dL_dcolors, out, aux.on(), stream); }
     if (rc) return rc;
     if (shs) {
         rc = launch_sh_backward(P, s->sh_degree, sh_M, s->campos, src.means3D, shs, radii, gst.clamped, dL_dcolors, dL_dsh,

@@ -143,19 +143,24 @@ struct ImageState {
     uint2* ranges;        // [tiles]
     uint32_t* tile_count; // [tiles]  pairs per tile (counted by preprocess)
     uint32_t* tile_cursor;// [tiles]  scatter cursors
-    uint32_t* totals;     // [64]     N, max count, overflow flag, #big tiles, preprocess CTA ticket (see tile_scan.cuh)
+    uint32_t* totals;     // [64]     N, max count, overflow flag, #big tiles, preprocess CTA ticket (see tile_scan.cuh),
+                          //          [kFwdFlagsWord] the GPSG_FWD_* flags of the forward that wrote this state
     uint32_t* big_tiles;  // [tiles]  ids of tiles with more than kBigTile pairs
     uint32_t* tile_order; // [tiles]  all tile ids, longest list first (tile_scan.cuh): work order of the compositing kernels
     static size_t required(int W, int H);
     static ImageState carve(void* base, int W, int H);
 };
+// totals word holding the forward's GPSG_FWD_* flags: written on the device by the preprocess (zeroed with the rest of
+// totals at the start of every forward), read by the projection backward -- a backward always follows the mode of the
+// forward whose buffers it is given, without a host read or an extra ABI argument.
+constexpr int kFwdFlagsWord = 6;
 size_t scan_temp_bytes(int P);
 size_t sort_temp_bytes(size_t N, int end_bit);
 
 // ---- kernel launchers (each enqueues on `stream`) ------------------------------------------
 // raster_preprocess.cu  (compiled with -fmad=false: integer outputs follow the oracle's op order)
 int launch_preprocess(const Camera& cam, int P, const GaussianSrc& src, int32_t* radii, GeomState g, ImageState im,
-                      uint32_t capacity, cudaStream_t stream);   // also runs the tile scan (last CTA)
+                      uint32_t capacity, int fwd_flags, cudaStream_t stream);   // also runs the tile scan (last CTA)
 int launch_mark_visible(int P, const float* means3D, const float* view16_host, uint8_t* present, cudaStream_t stream);
 // raster_binning.cu
 int run_scan(GeomState g, int P, cudaStream_t stream);
@@ -194,7 +199,8 @@ int launch_render_backward_det(const Camera& cam, BinningState b, ImageState im,
 int launch_det_reduce(const Camera& cam, int P, const int32_t* radii, GeomState g, BinningState b, ImageState im,
                       const uint8_t* det_mask, const float* det_part, float4* grad_acc, bool aux, cudaStream_t stream);
 int launch_preprocess_backward(const Camera& cam, int P, const GaussianSrc& src, const int32_t* radii,
-                               const float4* conic_opacity, const float4* grad_acc, float* dL_dmeans2D /* out [P,3] */,
+                               const float4* conic_opacity, const uint32_t* fwd_flags /* &totals[kFwdFlagsWord] */,
+                               const float4* grad_acc, float* dL_dmeans2D /* out [P,3] */,
                                float* dL_dcolors /* out [P,3] or NULL */, const GaussianGrads& out, bool aux,
                                cudaStream_t stream);
 // sh.cu

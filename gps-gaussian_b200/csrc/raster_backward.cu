@@ -426,13 +426,17 @@ int launch_det_reduce(const Camera& cam, int P, const int32_t* radii, GeomState 
 // A.7 + A.8 fused: per Gaussian, (dL/dmean2D, dL/dconic) -> dL/d{mean3D, cov3D, scale, rotation}.
 // AUX: slot 9 of the accumulator row is dL/dz of the view-space depth z = view[2] x + view[6] y + view[10] z + view[14],
 // added to dL/dmeans3D (map mode: dL/dxyz) through the view matrix's third row.
-template <bool AUX>
-__global__ void __launch_bounds__(256) preprocess_backward_kernel(
-    const __grid_constant__ Camera cam, int P, const GaussianSrc src, const int32_t* __restrict__ radii,
+// fwd_flags: the forward's GPSG_FWD_* word (totals[kFwdFlagsWord] of its image state).  With GPSG_FWD_ANTIALIAS the stored
+// opacity is o' = o * rho, rho = sqrt(max(2.5e-5, r)), r = D0 / D, D0 = a0 c0 - b^2, D = a c - b^2 (a = a0 + 0.3,
+// c = c0 + 0.3): dL/do = rho dL/do', and off the floor rho adds g (c0 - r c, -2b (1 - r), a0 - r a) / D, g = dL/do' o / (2 rho),
+// to dL/d(a, b, c) ahead of the cov2D -> cov3D chain (DESIGN.md section 2).
+// The word is uniform over the launch, so the kernel branches once into one of two inlined bodies: the AA = false body is the
+// projection backward without anti-aliasing, with no AA code on its path.
+template <bool AUX, bool AA>
+__device__ __forceinline__ void preprocess_backward_one(
+    const Camera& cam, int i, const GaussianSrc& src, const int32_t* __restrict__ radii,
     const float4* __restrict__ conic_opacity, const float4* __restrict__ grad_acc, float* __restrict__ dL_dmeans2D_out,
-    float* __restrict__ dL_dcolors_out, const GaussianGrads out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P) return;
+    float* __restrict__ dL_dcolors_out, const GaussianGrads& out) {
     float dm[3] = {0.f, 0.f, 0.f}, dsc[3] = {0.f, 0.f, 0.f}, dq[4] = {0.f, 0.f, 0.f, 0.f};
     float dcov[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float dop = 0.f, dm2[2] = {0.f, 0.f};
@@ -510,16 +514,33 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(
             SA0[k] = S[k][0] * A0[0] + S[k][1] * A0[1] + S[k][2] * A0[2];
             SA1[k] = S[k][0] * A1[0] + S[k][1] * A1[1] + S[k][2] * A1[2];
         }
-        const float a = (A0[0] * SA0[0] + A0[1] * SA0[1] + A0[2] * SA0[2]) + 0.3f;
+        const float a0 = A0[0] * SA0[0] + A0[1] * SA0[1] + A0[2] * SA0[2];
         const float b = A0[0] * SA1[0] + A0[1] * SA1[1] + A0[2] * SA1[2];
-        const float c = (A1[0] * SA1[0] + A1[1] * SA1[1] + A1[2] * SA1[2]) + 0.3f;
+        const float c0 = A1[0] * SA1[0] + A1[1] * SA1[1] + A1[2] * SA1[2];
+        const float a = a0 + 0.3f, c = c0 + 0.3f;
         const float denom = a * c - b * b;
         const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
         float dT0[3] = {0.f, 0.f, 0.f}, dT1[3] = {0.f, 0.f, 0.f};
-        if (denom2inv != 0.f) {
-            const float dL_da = denom2inv * (-c * c * gco.x + 2.f * b * c * gco.y + (denom - a * c) * gco.z);
-            const float dL_dc = denom2inv * (-a * a * gco.z + 2.f * a * b * gco.y + (denom - a * c) * gco.x);
-            const float dL_db = denom2inv * 2.f * (b * c * gco.x - (denom + 2.f * b * b) * gco.y + a * b * gco.z);
+        float dL_da = 0.f, dL_db = 0.f, dL_dc = 0.f;
+        bool chain = denom2inv != 0.f;
+        if (chain) {
+            dL_da = denom2inv * (-c * c * gco.x + 2.f * b * c * gco.y + (denom - a * c) * gco.z);
+            dL_dc = denom2inv * (-a * a * gco.z + 2.f * a * b * gco.y + (denom - a * c) * gco.x);
+            dL_db = denom2inv * 2.f * (b * c * gco.x - (denom + 2.f * b * b) * gco.y + a * b * gco.z);
+        }
+        if constexpr (AA) {
+            const float r = (a0 * c0 - b * b) / denom;
+            const float rho = sqrtf(fmaxf(0.000025f, r));
+            if (r > 0.000025f) {   // on the floor rho is constant: no term
+                const float gr = dop * opac_in / (2.f * rho) / denom;
+                dL_da += gr * (c0 - r * c);
+                dL_db += gr * (-2.f * b * (1.f - r));
+                dL_dc += gr * (a0 - r * a);
+                chain = true;
+            }
+            dop *= rho;
+        }
+        if (chain) {
             dcov[0] = A0[0] * A0[0] * dL_da + A0[0] * A1[0] * dL_db + A1[0] * A1[0] * dL_dc;
             dcov[3] = A0[1] * A0[1] * dL_da + A0[1] * A1[1] * dL_db + A1[1] * A1[1] * dL_dc;
             dcov[5] = A0[2] * A0[2] * dL_da + A0[2] * A1[2] * dL_db + A1[2] * A1[2] * dL_dc;
@@ -627,12 +648,27 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(
     }
 }
 
+template <bool AUX>
+__global__ void __launch_bounds__(256) preprocess_backward_kernel(
+    const __grid_constant__ Camera cam, int P, const GaussianSrc src, const int32_t* __restrict__ radii,
+    const float4* __restrict__ conic_opacity, const uint32_t* __restrict__ fwd_flags, const float4* __restrict__ grad_acc,
+    float* __restrict__ dL_dmeans2D_out, float* __restrict__ dL_dcolors_out, const GaussianGrads out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P) return;
+    if (__ldg(fwd_flags) & GPSG_FWD_ANTIALIAS)
+        preprocess_backward_one<AUX, true>(cam, i, src, radii, conic_opacity, grad_acc, dL_dmeans2D_out, dL_dcolors_out, out);
+    else
+        preprocess_backward_one<AUX, false>(cam, i, src, radii, conic_opacity, grad_acc, dL_dmeans2D_out, dL_dcolors_out, out);
+}
+
 int launch_preprocess_backward(const Camera& cam, int P, const GaussianSrc& src, const int32_t* radii,
-                               const float4* conic_opacity, const float4* grad_acc, float* dL_dmeans2D, float* dL_dcolors,
-                               const GaussianGrads& out, bool aux, cudaStream_t stream) {
+                               const float4* conic_opacity, const uint32_t* fwd_flags, const float4* grad_acc,
+                               float* dL_dmeans2D, float* dL_dcolors, const GaussianGrads& out, bool aux,
+                               cudaStream_t stream) {
     if (P <= 0) return GPSG_OK;
     auto kern = aux ? preprocess_backward_kernel<true> : preprocess_backward_kernel<false>;
-    kern<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, src, radii, conic_opacity, grad_acc, dL_dmeans2D, dL_dcolors, out);
+    kern<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, src, radii, conic_opacity, fwd_flags, grad_acc, dL_dmeans2D, dL_dcolors,
+                                              out);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

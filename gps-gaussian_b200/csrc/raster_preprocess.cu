@@ -32,6 +32,11 @@ __device__ __forceinline__ void cov3d_from_scale_rot(const float s0_, const floa
     c6[5] = (M02 * M02 + M12 * M12) + M22 * M22;
 }
 
+// AA (GPSG_FWD_ANTIALIAS): the opacity stored in conic_opacity.w is o * rho, rho = sqrt(max(2.5e-5, det(Sigma2D) /
+// det(Sigma2D + 0.3 I))) (DESIGN.md section 2), so a splat's integrated alpha no longer depends on the 0.3 px^2 dilation;
+// the conic and the radius still come from the dilated covariance.  Block 0 records the mode in totals[kFwdFlagsWord]
+// (zeroed by the forward's memset), where the projection backward reads it.
+template <bool AA>
 __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__ Camera cam, int P,
                                                          const GaussianSrc src, int32_t* __restrict__ radii,
                                                          GeomState g, ImageState im, uint32_t capacity) {
@@ -43,6 +48,9 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
     //  its fp32 chain without FMA and the histogram, not by load instructions.  The quaternion,
     //  a natural 16-byte row, is loaded as one float4 in src_geom.)
     if (threadIdx.x == 0) { s_bb[0] = 0x7fffffff; s_bb[1] = 0x7fffffff; s_bb[2] = 0; s_bb[3] = 0; }
+    if constexpr (AA) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) im.totals[kFwdFlagsWord] = GPSG_FWD_ANTIALIAS;
+    }
     for (int t = threadIdx.x; t < kBoxBins; t += blockDim.x) sh_cnt[t] = 0u;
     __syncthreads();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -92,9 +100,10 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         const float B10 = (A[3] * S00 + A[4] * S01) + A[5] * S02;
         const float B11 = (A[3] * S01 + A[4] * S11) + A[5] * S12;
         const float B12 = (A[3] * S02 + A[4] * S12) + A[5] * S22;
-        const float a = ((B00 * A[0] + B01 * A[1]) + B02 * A[2]) + 0.3f;
+        const float a0 = (B00 * A[0] + B01 * A[1]) + B02 * A[2];
         const float b = (B00 * A[3] + B01 * A[4]) + B02 * A[5];
-        const float c = ((B10 * A[3] + B11 * A[4]) + B12 * A[5]) + 0.3f;
+        const float c0 = (B10 * A[3] + B11 * A[4]) + B12 * A[5];
+        const float a = a0 + 0.3f, c = c0 + 0.3f;
         const float det = a * c - b * b;
         if (det == 0.0f) break;
         const float det_inv = 1.0f / det;
@@ -120,7 +129,12 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         if (area == 0) break;
         g.depths[i] = tvz;
         g.means2D[i] = make_float2(px, py);
-        g.conic_opacity[i] = make_float4(conx, cony, conz, opac);
+        float op = opac;
+        if constexpr (AA) {
+            const float det0 = a0 * c0 - b * b;
+            op = opac * sqrtf(rmax(0.000025f, det0 / det));
+        }
+        g.conic_opacity[i] = make_float4(conx, cony, conz, op);
         out_radius = my_radius;
         out_tiles = (uint32_t)area;
         bx0 = rx0; by0 = ry0; bx1 = rx1; by1 = ry1;
@@ -158,9 +172,10 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
 }
 
 int launch_preprocess(const Camera& cam, int P, const GaussianSrc& src, int32_t* radii, GeomState g, ImageState im,
-                      uint32_t capacity, cudaStream_t stream) {
+                      uint32_t capacity, int fwd_flags, cudaStream_t stream) {
     if (P <= 0) return GPSG_OK;
-    preprocess_kernel<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, src, radii, g, im, capacity);
+    auto kern = (fwd_flags & GPSG_FWD_ANTIALIAS) ? preprocess_kernel<true> : preprocess_kernel<false>;
+    kern<<<(P + 255) / 256, 256, 0, stream>>>(cam, P, src, radii, g, im, capacity);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

@@ -12,6 +12,10 @@ opacities, shs, colors_precomp, scales, rotations, cov3D_precomp) -> (color[3,H,
 
 Beyond the upstream surface, `rasterize_gaussians_aux` (same arguments) also returns the expected depth and the
 accumulated opacity (alpha) of every pixel, differentiable like the image (aux mode of include/gpsg.h).
+
+`GaussianRasterizationSettings(..., antialiasing=True)` (keyword only, upstream's newer setting of that name; default
+False) turns on the opacity-compensated screen-space filter (GPSG_FWD_ANTIALIAS) in `rasterize_gaussians`,
+`rasterize_gaussians_aux` and `GaussianRasterizer`, forward and backward.  `_fields` stays the reference's 12 names.
 """
 import ctypes as C
 import os
@@ -27,7 +31,7 @@ if _REPO not in sys.path:
 from gps_gaussian_b200 import _lib  # noqa: E402  (raises if the CUDA library is not built)
 
 
-class GaussianRasterizationSettings(NamedTuple):
+class _SettingsFields(NamedTuple):
     image_height: int
     image_width: int
     tanfovx: float
@@ -40,6 +44,51 @@ class GaussianRasterizationSettings(NamedTuple):
     campos: torch.Tensor
     prefiltered: bool
     debug: bool
+
+
+class GaussianRasterizationSettings(_SettingsFields):
+    """The reference's 12 settings (positional or keyword, `_fields` unchanged) plus the keyword-only `antialiasing`,
+    an attribute beside the tuple: its length, unpacking and the reference's 12-keyword construction are as before."""
+
+    def __new__(cls, *args, antialiasing=False, **kwargs):
+        self = super().__new__(cls, *args, **kwargs)
+        self.antialiasing = bool(antialiasing)
+        return self
+
+    @classmethod
+    def _make(cls, iterable, antialiasing=False):
+        return cls(*iterable, antialiasing=antialiasing)
+
+    def _replace(self, **kwargs):
+        antialiasing = kwargs.pop("antialiasing", self.antialiasing)
+        return type(self)(**{**self._asdict(), **kwargs}, antialiasing=antialiasing)
+
+    def __repr__(self):
+        return super().__repr__()[:-1] + f", antialiasing={self.antialiasing})"
+
+    def __reduce__(self):
+        return (_settings_from, (tuple(self), self.antialiasing))
+
+    # equality and hash include the switch: settings that differ only in antialiasing render different images
+    def __eq__(self, other):
+        eq = tuple.__eq__(self, other)
+        return eq if (eq is NotImplemented or not eq) else self.antialiasing == _antialiasing(other)
+
+    def __ne__(self, other):
+        eq = self.__eq__(other)
+        return eq if eq is NotImplemented else not eq
+
+    def __hash__(self):
+        return hash((tuple(self), self.antialiasing))
+
+
+def _settings_from(fields, antialiasing):
+    return GaussianRasterizationSettings(*fields, antialiasing=antialiasing)
+
+
+def _antialiasing(rs):
+    """The antialiasing switch of a settings object (False for any other 12-field settings tuple)."""
+    return bool(getattr(rs, "antialiasing", False))
 
 
 def _host_floats(t, n):
@@ -154,7 +203,7 @@ def _forward(ctx, t, aux):
                                                         colors_precomp=t["colors_precomp"], shs=t["shs"],
                                                         scales=t["scales"], rotations=t["rotations"],
                                                         cov3D_precomp=t["cov3D_precomp"], out_depth=maps[0],
-                                                        out_alpha=maps[1])
+                                                        out_alpha=maps[1], antialiasing=ctx.antialiasing)
     ctx.save_for_backward(*(t[k] for k in _SAVED), radii)
     ctx.mark_non_differentiable(radii)
     return color, radii, maps
@@ -177,6 +226,7 @@ class _RasterizeGaussians(torch.autograd.Function):
                 raster_settings):
         ctx.settings, t = _inputs(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                   raster_settings)
+        ctx.antialiasing = _antialiasing(raster_settings)
         color, radii, _ = _forward(ctx, t, aux=False)
         return color, radii
 
@@ -194,6 +244,7 @@ class _RasterizeGaussiansAux(torch.autograd.Function):
                 raster_settings):
         ctx.settings, t = _inputs(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                   raster_settings)
+        ctx.antialiasing = _antialiasing(raster_settings)
         color, radii, (depth, alpha) = _forward(ctx, t, aux=True)
         return color, depth, alpha, radii
 

@@ -39,8 +39,9 @@ def to_device(sc, device="cuda"):
 class RasterCall:
     """One forward (and optionally backward) through gpsg_rasterize_* with raw tensors."""
 
-    def __init__(self, sc, dev_inputs=None, device="cuda"):
+    def __init__(self, sc, dev_inputs=None, device="cuda", antialiasing=False):
         self.sc = sc
+        self.antialiasing = bool(antialiasing)      # forward mode; the backward follows the saved state
         self.device = torch.device(device)
         self.inp = dev_inputs if dev_inputs is not None else to_device(sc, device)
         self.settings = make_settings(sc)
@@ -59,7 +60,8 @@ class RasterCall:
     def forward(self, out_depth=None, out_alpha=None):
         """out_depth / out_alpha ([H,W], both or neither): aux mode, which also writes depth and alpha."""
         self.num_rendered, self.bufs = _lib.rasterize_forward(self.settings, self.color, self.radii, out_depth=out_depth,
-                                                              out_alpha=out_alpha, **self._inputs())
+                                                              out_alpha=out_alpha, antialiasing=self.antialiasing,
+                                                              **self._inputs())
         return self.color
 
     def backward(self, grad_color, want_cov3D=False, deterministic=None, grad_depth=None, grad_alpha=None):

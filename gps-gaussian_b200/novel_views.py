@@ -14,7 +14,8 @@ streams: no per-view gather, no host sync, no H2D camera copies inside the loop.
 
 Images equal `get_novel_calib(ratio)` + `pts2render` per ratio bit for bit in both modes.  With aux=True the sweep also
 carries the expected depth and the alpha matte of every view (aux mode of the planned forwards), equal to
-`pts2render_aux` per ratio bit for bit.
+`pts2render_aux` per ratio bit for bit.  With antialiasing=True every view is rendered with the opacity-compensated
+screen-space filter (GPSG_FWD_ANTIALIAS), equal to `pts2render_ex(..., antialiasing=True)` per ratio bit for bit.
 """
 import numpy as np
 import torch
@@ -34,10 +35,11 @@ class NovelViewRenderer:
     `data` is the dict the network returns (reference lib/network.py:41-88) -- the same one `pts2render` takes."""
 
     def __init__(self, data, opt, bg_color, intr_key='intr', extr_key='extr', streams=4, capacity_pairs=None,
-                 mode='compact'):
+                 mode='compact', antialiasing=False):
         if mode not in ('compact', 'maps'):
             raise ValueError("mode must be 'compact' or 'maps'")
         self.mode = mode
+        self.antialiasing = bool(antialiasing)
         self.data, self.opt, self.bg = data, opt, [float(v) for v in bg_color]
         self.keys = (intr_key, extr_key)
         x = data['lmain']['xyz']
@@ -86,11 +88,11 @@ class NovelViewRenderer:
                     alpha.zero_()
                 return
             rast.forward(settings, f['xyz'], f['rgb'], f['opacity'], f['scale'], f['rot'], out=out, status_host=status_host,
-                         depth=depth, alpha=alpha)
+                         depth=depth, alpha=alpha, antialiasing=self.antialiasing)
         else:
             m = self.maps[b]
             rast.forward_maps(settings, m['valid'], m['xyz'], m['img'], m['rot'], m['scale'], m['opacity'], out=out,
-                              status_host=status_host, depth=depth, alpha=alpha)
+                              status_host=status_host, depth=depth, alpha=alpha, antialiasing=self.antialiasing)
 
     def _settings(self, cal, b, r):
         cam = np.concatenate([cal[k][b, r].reshape(-1) for k in ('world_view_transform', 'full_proj_transform',
@@ -104,17 +106,19 @@ class NovelViewRenderer:
             f = self.flat[b]
             radii = torch.empty((f['xyz'].shape[0],), dtype=torch.int32, device=self.dev)
             _lib.rasterize_forward(settings, out, radii, f['xyz'], f['opacity'], colors_precomp=f['rgb'],
-                                   scales=f['scale'], rotations=f['rot'], out_depth=depth, out_alpha=alpha)
+                                   scales=f['scale'], rotations=f['rot'], out_depth=depth, out_alpha=alpha,
+                                   antialiasing=self.antialiasing)
         else:
             m = self.maps[b]
             args = []
             for v in range(2):
                 args += [m['valid'][v], m['xyz'][v], m['img'][v], m['rot'][v], m['scale'][v], m['opacity'][v]]
+            flags = _lib.forward_flags(self.antialiasing)
             with torch.no_grad():
                 if depth is None:
-                    out.copy_(_RasterizeMaps.apply([settings], *args)[0])
+                    out.copy_(_RasterizeMaps.apply([settings], flags, *args)[0])
                 else:
-                    i, d, a = _RasterizeMapsAux.apply([settings], *args)
+                    i, d, a = _RasterizeMapsAux.apply([settings], flags, *args)
                     out.copy_(i[0]); depth.copy_(d[0, 0]); alpha.copy_(a[0, 0])
 
     def render(self, ratios, out=None, check=True, aux=False):
@@ -174,11 +178,13 @@ class NovelViewRenderer:
         return result()
 
 
-def render_novel_views(data, opt, ratios, bg_color, intr_key='intr', extr_key='extr', streams=4, mode='compact', aux=False):
+def render_novel_views(data, opt, ratios, bg_color, intr_key='intr', extr_key='extr', streams=4, mode='compact', aux=False,
+                       antialiasing=False):
     """data['novel_view']['img_pred_sweep'] = [B, len(ratios), 3, H, W]; returns data.  aux=True also sets
-    ['depth_pred_sweep'] and ['alpha_pred_sweep'], [B, len(ratios), 1, H, W]."""
+    ['depth_pred_sweep'] and ['alpha_pred_sweep'], [B, len(ratios), 1, H, W].  antialiasing: see NovelViewRenderer."""
     nv = data['novel_view']
-    res = NovelViewRenderer(data, opt, bg_color, intr_key, extr_key, streams, mode=mode).render(ratios, aux=aux)
+    res = NovelViewRenderer(data, opt, bg_color, intr_key, extr_key, streams, mode=mode,
+                            antialiasing=antialiasing).render(ratios, aux=aux)
     if aux:
         nv['img_pred_sweep'], nv['depth_pred_sweep'], nv['alpha_pred_sweep'] = res
     else:

@@ -12,12 +12,18 @@ installs a post-import hook that, right after the reference executes those two m
 so `from core.corr import CorrBlockFast1D` (core/raft_stereo_human.py:6) and `from lib.GaussianRender import pts2render`
 (train_stage2.py:15, test_view_interp.py:15) pick ours up.  Same names, signatures and results (tests/test_c3_gpu.py runs
 the stage-2 step both ways).  `install()` / `uninstall()` do the same for modules that are already imported.
+
+`GPSG_ANTIALIAS=1`, read once by `install()`, makes the rebound `pts2render` render with the opacity-compensated
+screen-space filter (`pts2render_ex(..., antialiasing=True)`, forward and backward), so the unmodified training and
+novel-view scripts train and render anti-aliased; unset or any other value keeps the reference's image.
 """
 import importlib.abc
 import importlib.machinery
+import os
 import sys
 
 _ORIG = {}            # (module name, attribute) -> original object
+_ANTIALIAS = False    # GPSG_ANTIALIAS=1 at install()
 
 
 def _set(mod, attr, new):
@@ -36,9 +42,15 @@ def _patch_corr(mod):
         _set(user, "CorrBlockFast1D", ours.CorrBlockFast1D)
 
 
+def _pts2render_antialiased(data, bg_color):
+    """`pts2render` with the opacity-compensated screen-space filter (GPSG_ANTIALIAS=1)."""
+    from gps_gaussian_b200 import GaussianRender as ours
+    return ours.pts2render_ex(data, bg_color, antialiasing=True)
+
+
 def _patch_render(mod):
     from gps_gaussian_b200 import GaussianRender as ours
-    _set(mod, "pts2render", ours.pts2render)
+    _set(mod, "pts2render", _pts2render_antialiased if _ANTIALIAS else ours.pts2render)
 
 
 _TARGETS = {"core.corr": _patch_corr, "lib.GaussianRender": _patch_render}
@@ -75,7 +87,9 @@ _FINDER = _Finder()
 
 
 def install():
-    """Hook future imports and patch what is already imported. Idempotent."""
+    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS here, once."""
+    global _ANTIALIAS
+    _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _TARGETS.items():
@@ -95,3 +109,8 @@ def uninstall():
 
 def active():
     return _FINDER in sys.meta_path
+
+
+def antialiasing():
+    """Whether the installed patch renders with the screen-space filter (GPSG_ANTIALIAS=1 at install())."""
+    return _ANTIALIAS

@@ -42,12 +42,14 @@ class PlannedRasterizer:
         self.binning = torch.empty(int(_lib.lib.gpsg_raster_binning_bytes(self.capacity)), dtype=torch.uint8, device=self.dev)
 
     def forward(self, settings, means3D, colors, opacity, scales, rots, cov3D_precomp=None, out=None, status_host=None,
-                depth=None, alpha=None):
+                depth=None, alpha=None, antialiasing=False):
         """Enqueue one forward on the current stream (P = means3D.shape[0] may be smaller than the P the scratch was
         sized for; `out` / `status_host` redirect the image / deferred status words, as in forward_maps).  Inputs: contiguous fp32 CUDA tensors; `settings`: a
         `_lib.RasterSettings` (see introspect.make_settings) or a synth scene dict.  Returns self.color (valid once the
         stream has run AND ok() holds).  depth / alpha ([H,W] fp32, both or neither): aux mode
-        (gpsg_rasterize_forward_planned_aux), which also writes the expected depth and the alpha matte."""
+        (gpsg_rasterize_forward_planned_aux), which also writes the expected depth and the alpha matte.  antialiasing: the
+        opacity-compensated screen-space filter (GPSG_FWD_ANTIALIAS); the image buffer then carries that mode to the
+        backward.  Runs gpsg_rasterize_forward_planned_ex."""
         if isinstance(settings, dict):
             settings = make_settings(settings)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
@@ -55,35 +57,38 @@ class PlannedRasterizer:
         if P > self.P:
             raise ValueError(f"PlannedRasterizer scratch holds P<={self.P}, got {P}")
         color = self.color if out is None else out
-        aux = _aux_args(depth, alpha)
-        fn = _lib.lib.gpsg_rasterize_forward_planned_aux if aux else _lib.lib.gpsg_rasterize_forward_planned
+        aux = _aux_args(depth, alpha) or [None, None]       # the _ex forwards take both pointers, NULL without aux
+        fn = _lib.lib.gpsg_rasterize_forward_planned_ex
         rc = fn(C.byref(settings), *_lib.device_stream(self.dev), P, p(means3D),
                 p(colors), p(opacity), p(scales), p(rots), p(cov3D_precomp), p(color), *aux, p(self.radii), p(self.geom),
                 p(self.binning), self.capacity, p(self.image),
-                C.c_void_p((self.status_host if status_host is None else status_host).data_ptr()))
+                C.c_void_p((self.status_host if status_host is None else status_host).data_ptr()),
+                _lib.forward_flags(antialiasing))
         _lib.check(rc, fn.__name__)
         return color
 
     def forward_maps(self, settings, valid, xyz, img, rot, scale, opacity, out=None, status_host=None, depth=None,
-                     alpha=None):
+                     alpha=None, antialiasing=False):
         """Same, reading the two source views' pixel-aligned maps in place (`gpsg_rasterize_forward_maps_planned`):
         each argument is a pair (lmain, rmain) of contiguous CUDA tensors -- valid uint8/bool [S2], xyz [S2,3], img
         [3,S2] in [-1,1], rot [4,S2], scale [3,S2], opacity [1,S2]; self.P must be 2*S2.  `out` optionally redirects
         the image to another [3,H,W] tensor (e.g. a slice of a batch); `status_host` optionally redirects the deferred
         status words to another pinned int32[>=3] tensor (one per in-flight job).  depth / alpha: aux mode, as in
-        forward (gpsg_rasterize_forward_maps_planned_aux)."""
+        forward (gpsg_rasterize_forward_maps_planned_aux).  antialiasing: as in forward
+        (gpsg_rasterize_forward_maps_planned_ex)."""
         S2 = int(valid[0].numel())
         if 2 * S2 != self.P:
             raise ValueError(f"PlannedRasterizer built for P={self.P}, maps hold 2*{S2} candidates")
         pp = lambda ts: (C.c_void_p * 2)(*[t.data_ptr() for t in ts])
         color = self.color if out is None else out
-        aux = _aux_args(depth, alpha)
-        fn = _lib.lib.gpsg_rasterize_forward_maps_planned_aux if aux else _lib.lib.gpsg_rasterize_forward_maps_planned
+        aux = _aux_args(depth, alpha) or [None, None]       # the _ex forwards take both pointers, NULL without aux
+        fn = _lib.lib.gpsg_rasterize_forward_maps_planned_ex
         rc = fn(C.byref(settings), *_lib.device_stream(self.dev), S2, pp(valid), pp(xyz),
                 pp(img), pp(rot), pp(scale), pp(opacity), C.c_void_p(color.data_ptr()), *aux,
                 C.c_void_p(self.radii.data_ptr()), C.c_void_p(self.geom.data_ptr()), C.c_void_p(self.binning.data_ptr()),
                 self.capacity, C.c_void_p(self.image.data_ptr()),
-                C.c_void_p((self.status_host if status_host is None else status_host).data_ptr()))
+                C.c_void_p((self.status_host if status_host is None else status_host).data_ptr()),
+                _lib.forward_flags(antialiasing))
         _lib.check(rc, fn.__name__)
         return color
 
@@ -104,20 +109,20 @@ class PlannedRasterizer:
         self.graph = None
 
     # ---- CUDA graph ----
-    def capture(self, settings, means3D, colors, opacity, scales, rots, cov3D_precomp=None):
-        """Capture one forward (fixed input pointers / camera) into a CUDA graph; replay() re-runs it."""
+    def capture(self, settings, means3D, colors, opacity, scales, rots, cov3D_precomp=None, antialiasing=False):
+        """Capture one forward (fixed input pointers / camera / mode) into a CUDA graph; replay() re-runs it."""
         if isinstance(settings, dict):
             settings = make_settings(settings)
         self._keep = (settings, means3D, colors, opacity, scales, rots, cov3D_precomp)
         s = torch.cuda.Stream(self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
         with torch.cuda.stream(s):
-            self.forward(*self._keep)                      # warm-up outside capture (lazy module loads etc.)
+            self.forward(*self._keep, antialiasing=antialiasing)   # warm-up outside capture (lazy module loads etc.)
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
-            self.forward(*self._keep)
+            self.forward(*self._keep, antialiasing=antialiasing)
         self.graph = g
         return g
 

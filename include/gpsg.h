@@ -256,6 +256,51 @@ GPSG_API int gpsg_rasterize_backward_maps_aux(const GpsgRasterSettings* settings
                                               float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
                                               int flags);
 
+/* ---- forward flags: the forwards above with a trailing `flags` word -----------------------------------------------
+ * Each _ex forward covers its aux form too (out_depth / out_alpha both NULL or both set, as for the _aux forwards).
+ * flags = 0 is exactly the entry point without _ex (those are these with 0).
+ * flags = GPSG_FWD_ANTIALIAS: opacity-compensated screen-space filter (upstream's `antialiasing` setting, the 2-D filter of
+ *   Mip-Splatting).  The 0.3 px^2 dilation of the screen covariance stays, so the conics, radii, tile lists and sort
+ *   keys are bit-identical to flags = 0; each splat's opacity is scaled by rho = sqrt(max(2.5e-5, det(Sigma2D) /
+ *   det(Sigma2D + 0.3 I))), so its integrated alpha no longer grows with the dilation (sub-pixel splats no longer turn
+ *   into >= 0.55 px blobs at full opacity).  The scaled opacity o * rho is what conic_opacity[P,4].w (gpsg_geom_view)
+ *   holds and what the compositing uses.
+ * The forward records its flags in its image buffer, on the device and in stream order (no host synchronisation, so the
+ * planned forms stay graph-capturable); every backward reads them from the image buffer it is given, so a backward
+ * always differentiates the mode of the forward whose buffers it receives, and the backward entry points, workspace
+ * sizes and GPSG_BWD_* flags are unchanged.  A reused planned image buffer carries the mode of its last forward.
+ * maps: only _begin takes flags (the projection runs there); _finish / _finish_aux are unchanged.
+ * Unknown flag bits return GPSG_E_INVALID before any other argument is checked. */
+#define GPSG_FWD_ANTIALIAS 1
+GPSG_API int gpsg_rasterize_forward_ex(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
+                                       const float* means3D, const float* colors_precomp, const float* shs,
+                                       const float* opacities, const float* scales, const float* rotations,
+                                       const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
+                                       int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
+                                       gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
+                                       void* image_user, int32_t* num_rendered, int flags);
+GPSG_API int gpsg_rasterize_forward_maps_begin_ex(const GpsgRasterSettings* settings, int device, void* stream,
+                                                  int pixels_per_view, const uint8_t* const* valid,
+                                                  const float* const* xyz, const float* const* img,
+                                                  const float* const* rot, const float* const* scale,
+                                                  const float* const* opacity, int32_t* radii, gpsg_alloc_fn geom_alloc,
+                                                  void* geom_user, gpsg_alloc_fn image_alloc, void* image_user,
+                                                  uint32_t* totals_host, int flags);
+GPSG_API int gpsg_rasterize_forward_planned_ex(const GpsgRasterSettings* settings, int device, void* stream, int P,
+                                               const float* means3D, const float* colors_precomp, const float* opacities,
+                                               const float* scales, const float* rotations, const float* cov3D_precomp,
+                                               float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                               void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
+                                               void* image_buffer, uint32_t* status_host, int flags);
+GPSG_API int gpsg_rasterize_forward_maps_planned_ex(const GpsgRasterSettings* settings, int device, void* stream,
+                                                    int pixels_per_view, const uint8_t* const* valid,
+                                                    const float* const* xyz, const float* const* img,
+                                                    const float* const* rot, const float* const* scale,
+                                                    const float* const* opacity, float* out_color, float* out_depth,
+                                                    float* out_alpha, int32_t* radii, void* geom_buffer,
+                                                    void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
+                                                    uint32_t* status_host, int flags);
+
 /* ---- replaces _C.mark_visible : present[P] (uint8) = view-space z > 0.2 ---------------------- */
 GPSG_API int gpsg_mark_visible(int device, void* stream, int P, const float* means3D, const float* viewmatrix_host16,
                       uint8_t* present);

@@ -33,6 +33,13 @@ RASTER_CASES = {            # name -> synth.random_cube_scene kwargs (same cases
     "saturating": dict(P=300, res=64, spread=0.3, scale_mul=12.0, bg=(1.0, 1.0, 1.0), seed=11),
     "wide_cloud": dict(P=2000, res=130, spread=3.0, scale_mul=1.0, bg=(0.0, 0.0, 0.0), seed=11),
 }
+# Anti-aliased cases (the upstream `antialiasing=True` setting, GPSG_FWD_ANTIALIAS here), recorded only when the installed
+# extension's GaussianRasterizationSettings accepts `antialiasing`.  They go to raster_aa_reference_<name>.npz, a name the
+# plain consumer's raster_reference_*.npz glob does not match; tests/test_raster_aa_cpu.py / _gpu.py consume them.
+RASTER_AA_CASES = {
+    "c1_antialias": dict(P=10_000, res=256),
+    "small_splats_antialias": dict(P=20_000, res=256, scale_mul=0.25, seed=11),
+}
 CORR_CASES = {"b2_h32_w16_d32": dict(B=2, D=32, H=16, W=32)}
 
 
@@ -42,32 +49,47 @@ def _require_real(mod, ours_marker="gps-gaussian_b200"):
                          "PYTHONPATH -- the point of this script is to record the REAL extension")
 
 
+def upstream_has_antialiasing(dgr):
+    """Whether the installed extension's settings take the `antialiasing` field (the later upstream API)."""
+    return "antialiasing" in getattr(dgr.GaussianRasterizationSettings, "_fields", ())
+
+
 def dump_raster(out_dir, device):
-    import torch
     import diff_gaussian_rasterization as dgr
     _require_real(dgr)
+    cases = [(name, kw, False, "raster_reference") for name, kw in RASTER_CASES.items()]
+    if upstream_has_antialiasing(dgr):
+        cases += [(name, kw, True, "raster_aa_reference") for name, kw in RASTER_AA_CASES.items()]
+    else:
+        print("the installed diff_gaussian_rasterization has no `antialiasing` setting: anti-aliased cases not recorded")
+    for name, kw, aa, prefix in cases:
+        _dump_raster_case(dgr, out_dir, device, name, kw, aa, prefix)
+
+
+def _dump_raster_case(dgr, out_dir, device, name, kw, aa, prefix):
+    import torch
     from gps_gaussian_b200 import synth
-    for name, kw in RASTER_CASES.items():
-        kw = dict(kw)
-        sc = synth.random_cube_scene(kw.pop("P"), kw.pop("res"), **kw)
-        T = lambda a: torch.tensor(np.asarray(a, np.float32), device=device, requires_grad=True)
-        m, c, op, s, r = T(sc["means3D"]), T(sc["colors"]), T(sc["opacity"]), T(sc["scales"]), T(sc["rots"])
-        m2d = torch.zeros_like(m, requires_grad=True)
-        cam = lambda k, shape: torch.tensor(np.asarray(sc[k], np.float32).reshape(shape), device=device)
-        rs = dgr.GaussianRasterizationSettings(
-            image_height=int(sc["H"]), image_width=int(sc["W"]), tanfovx=float(sc["tanfovx"]), tanfovy=float(sc["tanfovy"]),
-            bg=cam("bg", (3,)), scale_modifier=1.0, viewmatrix=cam("view", (4, 4)), projmatrix=cam("proj", (4, 4)),
-            sh_degree=3, campos=cam("campos", (3,)), prefiltered=False, debug=False)
-        img, radii = dgr.GaussianRasterizer(raster_settings=rs)(means3D=m, means2D=m2d, opacities=op, shs=None,
-                                                                colors_precomp=c, scales=s, rotations=r, cov3D_precomp=None)
-        g = np.random.default_rng(0).standard_normal(tuple(img.shape)).astype(np.float32)
-        img.backward(torch.from_numpy(g).to(device))
-        np.savez_compressed(os.path.join(out_dir, f"raster_reference_{name}.npz"), case=name,
-                            color=img.detach().cpu().numpy(), radii=radii.cpu().numpy().astype(np.int32), grad_out=g,
-                            dL_dmeans3D=m.grad.cpu().numpy(), dL_dmeans2D=m2d.grad.cpu().numpy(), dL_dcolors=c.grad.cpu().numpy(),
-                            dL_dopacity=op.grad.cpu().numpy(), dL_dscales=s.grad.cpu().numpy(), dL_drots=r.grad.cpu().numpy(),
-                            extension=str(getattr(dgr, "__file__", "?")))
-        print("wrote raster", name, tuple(img.shape), int((radii > 0).sum()), "visible")
+    kw = dict(kw)
+    sc = synth.random_cube_scene(kw.pop("P"), kw.pop("res"), **kw)
+    T = lambda a: torch.tensor(np.asarray(a, np.float32), device=device, requires_grad=True)
+    m, c, op, s, r = T(sc["means3D"]), T(sc["colors"]), T(sc["opacity"]), T(sc["scales"]), T(sc["rots"])
+    m2d = torch.zeros_like(m, requires_grad=True)
+    cam = lambda k, shape: torch.tensor(np.asarray(sc[k], np.float32).reshape(shape), device=device)
+    rs = dgr.GaussianRasterizationSettings(
+        image_height=int(sc["H"]), image_width=int(sc["W"]), tanfovx=float(sc["tanfovx"]), tanfovy=float(sc["tanfovy"]),
+        bg=cam("bg", (3,)), scale_modifier=1.0, viewmatrix=cam("view", (4, 4)), projmatrix=cam("proj", (4, 4)),
+        sh_degree=3, campos=cam("campos", (3,)), prefiltered=False, debug=False, **(dict(antialiasing=True) if aa else {}))
+    res = dgr.GaussianRasterizer(raster_settings=rs)(means3D=m, means2D=m2d, opacities=op, shs=None,
+                                                     colors_precomp=c, scales=s, rotations=r, cov3D_precomp=None)
+    img, radii = res[0], res[1]              # the later upstream API also returns an inverse-depth image
+    g = np.random.default_rng(0).standard_normal(tuple(img.shape)).astype(np.float32)
+    img.backward(torch.from_numpy(g).to(device))
+    np.savez_compressed(os.path.join(out_dir, f"{prefix}_{name}.npz"), case=name, antialiasing=aa,
+                        color=img.detach().cpu().numpy(), radii=radii.cpu().numpy().astype(np.int32), grad_out=g,
+                        dL_dmeans3D=m.grad.cpu().numpy(), dL_dmeans2D=m2d.grad.cpu().numpy(), dL_dcolors=c.grad.cpu().numpy(),
+                        dL_dopacity=op.grad.cpu().numpy(), dL_dscales=s.grad.cpu().numpy(), dL_drots=r.grad.cpu().numpy(),
+                        extension=str(getattr(dgr, "__file__", "?")))
+    print("wrote raster", prefix, name, tuple(img.shape), int((radii > 0).sum()), "visible")
 
 
 def dump_corr(out_dir, device):

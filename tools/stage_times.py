@@ -4,10 +4,13 @@ one stream) -- the quick loop used while tuning kernels:  python tools/stage_tim
 --deterministic times the deterministic backward (GPSG_BWD_DETERMINISTIC: render_backward_det, render_backward_det_reduce)
 instead of the default one and adds its workspace bytes per view.  --aux times aux mode (depth and alpha outputs, and the
 backward of all three images) under the same stage names.  --alternate R runs R rounds that alternate default and aux
-(same scenes, same process) and prints one line per round and mode."""
+(same scenes, same process) and prints one line per round and mode.  --antialias times the anti-aliased forward and
+backward (GPSG_FWD_ANTIALIAS); with --alternate R the rounds then alternate AA off and on instead.  Each line carries the
+GPU's name and power limit."""
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -25,6 +28,7 @@ ap.add_argument("--no-backward", action="store_true")
 ap.add_argument("--deterministic", action="store_true")
 ap.add_argument("--aux", action="store_true")
 ap.add_argument("--alternate", type=int, default=0)
+ap.add_argument("--antialias", action="store_true")
 a = ap.parse_args()
 dev = torch.device("cuda", 0)
 calls = [RasterCall(sc, to_device(sc, dev), dev) for sc in (synth.stereo_pair_scene(a.res, seed=s) for s in a.seeds)]
@@ -33,15 +37,27 @@ gD, gA = torch.randn(a.res, a.res, device=dev), torch.randn(a.res, a.res, device
 depth, alpha = torch.empty(a.res, a.res, device=dev), torch.empty(a.res, a.res, device=dev)
 
 
-def step(c, aux):
+def power_limit():
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception:
+        return "unknown"
+
+
+POWER = power_limit()
+
+
+def step(c, aux, aa=False):
+    c.antialiasing = aa
     c.forward(*((depth, alpha) if aux else (None, None)))
     if not a.no_backward:
         c.backward(g, deterministic=a.deterministic, **(dict(grad_depth=gD, grad_alpha=gA) if aux else {}))
 
 
-def run(aux):
+def run(aux, aa=False):
     for c in calls:
-        step(c, aux)
+        step(c, aux, aa)
     torch.cuda.synchronize()
     _lib.profile_enable(True)
     _lib.profile_read()
@@ -49,7 +65,7 @@ def run(aux):
     e0.record()
     for _ in range(a.reps):
         for c in calls:
-            step(c, aux)
+            step(c, aux, aa)
     e1.record()
     torch.cuda.synchronize()
     prof = _lib.profile_read()
@@ -61,13 +77,19 @@ def run(aux):
     size = _lib.lib.gpsg_rasterize_backward_aux_workspace_bytes if aux else _lib.lib.gpsg_rasterize_backward_workspace_bytes_ex
     out["bwd_workspace_bytes_mean"] = sum(size(c.P, c.num_rendered, flags) for c in calls) / len(calls)
     out["aux"] = aux
+    out["antialias"] = aa
     out["gpu"] = torch.cuda.get_device_name(0)
+    out["power_limit"] = POWER
     return out
 
 
-if a.alternate:
+if a.alternate and a.antialias:
+    for r in range(a.alternate):
+        for aa in (False, True):
+            print(json.dumps(dict(run(a.aux, aa), round=r)))
+elif a.alternate:
     for r in range(a.alternate):
         for aux in (False, True):
             print(json.dumps(dict(run(aux), round=r)))
 else:
-    print(json.dumps(run(a.aux)))
+    print(json.dumps(run(a.aux, a.antialias)))
