@@ -32,11 +32,11 @@ class GeomView(C.Structure):
 
 
 class BinningView(C.Structure):
-    _fields_ = [("point_list_keys", C.c_void_p), ("point_list", C.c_void_p)]
+    _fields_ = [("point_list_keys", C.c_void_p), ("point_list", C.c_void_p), ("slabA", C.c_void_p), ("block_lists", C.c_void_p)]
 
 
 class ImageView(C.Structure):
-    _fields_ = [("final_T", C.c_void_p), ("n_contrib", C.c_void_p), ("ranges", C.c_void_p)]
+    _fields_ = [("final_T", C.c_void_p), ("n_contrib", C.c_void_p), ("ranges", C.c_void_p), ("block_counts", C.c_void_p)]
 
 
 ALLOC_FN = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)

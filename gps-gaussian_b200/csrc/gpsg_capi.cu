@@ -78,6 +78,7 @@ static BinningState carve_binning(char* p, size_t N, size_t sort_bytes, char** e
     b.keys_unsorted = take<uint64_t>(p, n);
     b.bucket = reinterpret_cast<uint2*>(b.keys_unsorted);   // tile-bucket path: same bytes, never both in use
     b.vals_unsorted = take<uint32_t>(p, n);
+    b.blk_list = take<uint32_t>(p, 8 * n);
     b.sort_temp = p;
     b.sort_temp_bytes = sort_bytes;
     p += align_up(sort_bytes);
@@ -105,6 +106,7 @@ static ImageState carve_image(char* p, int W, int H, char** end) {
     im.tile_cursor = take<uint32_t>(p, tiles > 0 ? tiles : 1);
     im.big_tiles = take<uint32_t>(p, tiles > 0 ? tiles : 1);
     im.tile_order = take<uint32_t>(p, tiles > 0 ? tiles : 1);
+    im.blk_count = take<uint32_t>(p, 8 * (tiles > 0 ? tiles : 1));
     if (end) *end = p;
     return im;
 }
@@ -273,7 +275,7 @@ static int forward_exact_finish(const GpsgRasterSettings* s, int device, cudaStr
         if (rc) return rc;
         { StageTimer t(ST_SORT, stream, 2 + (end_bit + 7) / 8); rc = run_sort(b, N, end_bit, stream); }
         if (rc) return rc;
-        { StageTimer t(ST_GATHER, stream, 1); rc = launch_gather_ranges(cam, N, src, g, b, im, stream); }
+        { StageTimer t(ST_GATHER, stream, 2); rc = launch_gather_ranges(cam, N, src, g, b, im, stream); }
         if (rc) return rc;
     }
     { StageTimer t(ST_RENDER_FWD, stream, 1); rc = launch_render_forward(cam, b, im, out_color, g.depths, out_depth, out_alpha, stream); }
@@ -783,6 +785,8 @@ int gpsg_binning_view(const void* binning_buffer, int64_t num_rendered, GpsgBinn
     BinningState b = BinningState::carve(const_cast<void*>(binning_buffer), (size_t)num_rendered, 0);
     out->point_list_keys = b.keys;
     out->point_list = b.vals;
+    out->slabA = reinterpret_cast<const float*>(b.slabA);
+    out->block_lists = b.blk_list;
     return GPSG_OK;
 }
 int gpsg_image_view(const void* image_buffer, int W, int H, GpsgImageView* out) {
@@ -791,6 +795,7 @@ int gpsg_image_view(const void* image_buffer, int W, int H, GpsgImageView* out) 
     out->final_T = im.final_T;
     out->n_contrib = im.n_contrib;
     out->ranges = reinterpret_cast<const uint32_t*>(im.ranges);
+    out->block_counts = im.blk_count;
     return GPSG_OK;
 }
 

@@ -99,6 +99,14 @@ __device__ __forceinline__ void tile_rect(int grid_x, int grid_y, float2 p, int 
     rx1 = min(grid_x, max(0, (int)((p.x + rad + (float)(GPSG_TILE_X - 1)) / (float)GPSG_TILE_X)));
     ry1 = min(grid_y, max(0, (int)((p.y + rad + (float)(GPSG_TILE_Y - 1)) / (float)GPSG_TILE_Y)));
 }
+// The 8 warp blocks (8x4 pixels) of a 16x16 tile that the compositing forward renders, one warp each.  Block k sits at
+// x offset 8*((k>>1)&1), y offset 4*(2*(k>>2) + (k&1)): blocks 2c, 2c+1 form an 8x8 quarter tile, 4c..4c+3 a 16x8 half.
+__device__ __forceinline__ int fwd_block_col(int k) { return (k >> 1) & 1; }            // 8-pixel column of the tile
+__device__ __forceinline__ int fwd_block_row(int k) { return ((k >> 2) << 1) + (k & 1); }   // 4-pixel row of the tile
+__device__ __forceinline__ void fwd_block_origin(int tile_x, int tile_y, int k, int& bx0, int& by0) {
+    bx0 = tile_x * GPSG_TILE_X + (fwd_block_col(k) << 3);
+    by0 = tile_y * GPSG_TILE_Y + (fwd_block_row(k) << 2);
+}
 __device__ __forceinline__ void src_color(const GaussianSrc& s, uint32_t id, float& r, float& g, float& b) {
     if (s.S2 == 0) { r = s.colors[3 * id]; g = s.colors[3 * id + 1]; b = s.colors[3 * id + 2]; return; }
     const int v = (int)id >= s.S2 ? 1 : 0;
@@ -132,6 +140,8 @@ struct BinningState {
     float4* slabA;            // [N] (x, y, cull half-extent x, y)     sorted, tile-contiguous
     float4* slabB;            // [N] (-0.5*log2e*conic.x, -log2e*conic.y, -0.5*log2e*conic.z, opacity)
     float4* slabC;            // [N] (r, g, b, Gaussian id bits)
+    uint32_t* blk_list;       // [8N] per warp block of a tile with range [s, s+n): block k's survivors, as tile-local list
+                              //      positions in list order, at blk_list[8s + k*n ...] (count in ImageState::blk_count)
     void* sort_temp;
     size_t sort_temp_bytes;
     static size_t required(size_t N, size_t sort_temp_bytes);
@@ -147,6 +157,7 @@ struct ImageState {
                           //          [kFwdFlagsWord] the GPSG_FWD_* flags of the forward that wrote this state
     uint32_t* big_tiles;  // [tiles]  ids of tiles with more than kBigTile pairs
     uint32_t* tile_order; // [tiles]  all tile ids, longest list first (tile_scan.cuh): work order of the compositing kernels
+    uint32_t* blk_count;  // [8*tiles] survivors per warp block (BinningState::blk_list); only read for non-empty tiles
     static size_t required(int W, int H);
     static ImageState carve(void* base, int W, int H);
 };

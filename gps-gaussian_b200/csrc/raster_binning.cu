@@ -173,14 +173,92 @@ __device__ __forceinline__ void slab_entry(uint32_t id, const GaussianSrc& src, 
     C = make_float4(r, gg, bb, __uint_as_float(id));
 }
 
+constexpr int kSortThreads = 512;
+constexpr int kSortWarps = kSortThreads / 32;
+constexpr int kSortCTAsPerSM = 3;
+
+// ---- per-block survivor lists of the compositing forward (raster_render.cu) ------------------------------------------
+// For each of the 8 warp blocks of a tile (fwd_block_origin), the tile-local list positions of the entries whose cull box
+// (slabA: centre +- half-extents) meets the block, in list order.  The test is the expression the compositing kernel used
+// to evaluate per entry and block, on the same floats, so the forward composites exactly the entries it did before.
+// Built by a whole CTA of kSortThreads threads over chunks of kSortThreads consecutive positions: ballot ranks inside a
+// warp plus a CTA-wide prefix of the 8 per-warp counts.  Positions are 32-bit: tile lists exceed 65535 entries on the
+// radix path.
+struct BlockLists {
+    uint32_t cnt[kSortWarps][8];   // survivors of the chunk per (warp, block)
+    uint32_t off[kSortWarps][8];   // where each warp's survivors go in each block's list
+    uint32_t base[8];              // survivors of the earlier chunks per block
+};
+
+// Every thread of the CTA calls this, after the tile's slabA entries [0, n) are written (tileA = slabA + tile start; on the
+// sort path each thread reads back only entries it wrote itself).  list = blk_list + 8 * (tile start),
+// count = blk_count + 8 * tile.  The entries are read back (from L2) rather than taken from the gather loop's registers:
+// fused into that loop, the build pushes the sort kernel past its 40 registers into spills, and measured slower.
+__device__ __forceinline__ void build_block_lists(BlockLists& s, const float4* __restrict__ tileA, uint32_t n, int tile_x,
+                                                  int tile_y, uint32_t* __restrict__ list, uint32_t* __restrict__ count) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned lt = (1u << lane) - 1u;
+    // block k keeps an entry iff (a.x >= wx0 - a.z) && (a.x <= wx1 + a.z) && (a.y >= wy0 - a.w) && (a.y <= wy1 + a.w) for
+    // its window; the x half depends on the block's column only and the y half on its row only
+    float wx0[2], wx1[2], wy0[4], wy1[4];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        int bx0, by0;
+        fwd_block_origin(tile_x, tile_y, k, bx0, by0);
+        wx0[fwd_block_col(k)] = (float)bx0; wx1[fwd_block_col(k)] = (float)(bx0 + 7);
+        wy0[fwd_block_row(k)] = (float)by0; wy1[fwd_block_row(k)] = (float)(by0 + 3);
+    }
+    if (threadIdx.x < 8) s.base[threadIdx.x] = 0u;
+#pragma unroll 1
+    for (uint32_t c0 = 0; c0 < n; c0 += kSortThreads) {
+        const uint32_t r = c0 + threadIdx.x;
+        const bool valid = r < n;
+        const float4 a = valid ? tileA[r] : make_float4(0.f, 0.f, 0.f, 0.f);
+        bool hx[2], hy[4];
+#pragma unroll
+        for (int c = 0; c < 2; ++c) hx[c] = (a.x >= wx0[c] - a.z) && (a.x <= wx1[c] + a.z);
+#pragma unroll
+        for (int w = 0; w < 4; ++w) hy[w] = (a.y >= wy0[w] - a.w) && (a.y <= wy1[w] + a.w);
+        uint32_t hits = 0u;   // bit k: the entry survives block k's cull
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const bool hit = valid && hx[fwd_block_col(k)] && hy[fwd_block_row(k)];
+            hits |= (uint32_t)hit << k;
+            const unsigned m = __ballot_sync(0xffffffffu, hit);
+            if (lane == k) s.cnt[warp][k] = __popc(m);
+        }
+        __syncthreads();
+        if (threadIdx.x < kSortWarps * 8) {   // one 16-lane segment per block: exclusive scan over the warps
+            static_assert(kSortWarps == 16, "one 16-lane segment per block");
+            const int k = threadIdx.x >> 4, w = threadIdx.x & 15;
+            const uint32_t cw = s.cnt[w][k];
+            uint32_t incl = cw;
+#pragma unroll
+            for (int o = 1; o < 16; o <<= 1) {
+                const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o, 16);
+                if (w >= o) incl += u;
+            }
+            const uint32_t b = s.base[k];
+            s.off[w][k] = b + incl - cw;
+            __syncwarp();
+            if (w == 15) s.base[k] = b + incl;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const unsigned m = __ballot_sync(0xffffffffu, (hits >> k) & 1u);
+            if ((hits >> k) & 1u) list[(size_t)k * n + s.off[warp][k] + __popc(m & lt)] = r;
+        }
+    }
+    if (threadIdx.x < 8) count[threadIdx.x] = s.base[threadIdx.x];   // base was last written before the final barrier
+}
+
 // one CTA per tile: radix sort of the tile's bucket inside the CTA (cub::BlockRadixSort, keys in registers), then the
-// parameter slabs (and, on the exact entry point, the sorted keys and point list) are written coalesced -- the sort
-// and the gather never round-trip to HBM.  The CTA picks the smallest items-per-thread variant that fits.
-// 512 threads: a 2048-entry tile needs only 4 keys + 4 ids per thread, so three CTAs (1536 threads, 40 registers)
+// parameter slabs (and, on the exact entry point, the sorted keys and point list) and the per-block survivor lists are
+// written -- the sort and the gather never round-trip to HBM.  The CTA picks the smallest items-per-thread variant that
+// fits.  512 threads: a 2048-entry tile needs only 4 keys + 4 ids per thread, so three CTAs (1536 threads, 40 registers)
 // fit per SM without spills.  Not memoising cub's outer scan and keeping the fix-up and gather loops rolled is what
 // keeps the kernel inside 40 registers.
-constexpr int kSortThreads = 512;
-constexpr int kSortCTAsPerSM = 3;
 constexpr int kBigItems = (int)kMaxTileSort / kSortThreads;   // big-tile kernel: 8 keys per thread
 template <int ITEMS>
 struct TileSort {
@@ -191,7 +269,8 @@ struct TileSort {
         unsigned long long keys[kSortThreads * ITEMS];   // sorted (depth bits << 32 | id), for the equal-depth fix-up
     };
 
-    // Sorts the tile's entries in (depth bits << 32 | id) order and writes slabs (+ keys and point list if b.keys).
+    // Sorts the tile's entries in (depth bits << 32 | id) order and writes slabs (+ keys and point list if b.keys) and the
+    // per-block survivor lists.
     //  * only the depth window is radix-sorted: 32-bit keys `depth bits - tile minimum`, whose width is the bit length
     //    of the tile's depth span (block-wide min/max; about 20 bits on real scenes, at most 31 as depth > 0);
     //  * the Gaussian id rides along as the value and is NOT radix-sorted: equal-depth runs -- the only place it
@@ -199,8 +278,9 @@ struct TileSort {
     //    to the full (id, then depth) LSD radix sort, so degenerate inputs (thousands of identical depths) stay correct
     //    and bounded.
     static constexpr int kMaxRun = 16;
-    __device__ static void run(Smem& sm, uint32_t* flags, const uint2* __restrict__ src, int n, int id_bits, uint32_t tile,
-                               size_t out0, const GaussianSrc& src_in, const GeomState& g, const BinningState& b) {
+    __device__ static void run(Smem& sm, uint32_t* flags, BlockLists& bl, const uint2* __restrict__ src, int n, int id_bits,
+                               uint32_t tile, int grid_x, size_t out0, const GaussianSrc& src_in, const GeomState& g,
+                               const BinningState& b, uint32_t* __restrict__ blk_count) {
         uint32_t keys[ITEMS], ids[ITEMS];
         uint32_t dmin = ~0u, dmax = 0u;
 #pragma unroll
@@ -305,6 +385,9 @@ struct TileSort {
                 b.slabC[o] = C;
             }
         }
+        const int tile_y = (int)tile / grid_x;
+        build_block_lists(bl, b.slabA + out0, (uint32_t)n, (int)tile - tile_y * grid_x, tile_y, b.blk_list + 8 * out0,
+                          blk_count + 8 * (size_t)tile);
     }
 };
 
@@ -315,8 +398,10 @@ struct TileSort {
 // footprint of the rare one.
 template <bool BIG>
 __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_sort_gather_kernel(const GaussianSrc colors, GeomState g,
-                                                                            BinningState b, ImageState im, int id_bits) {
+                                                                            BinningState b, ImageState im, int id_bits,
+                                                                            int grid_x) {
     __shared__ uint32_t flags[4];
+    __shared__ BlockLists bl;
     if (im.totals[2]) return;                   // planned mode overflow
     if constexpr (BIG) {
         __shared__ typename TileSort<kBigItems>::Smem t16;
@@ -325,7 +410,8 @@ __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_s
             const uint32_t tile = im.big_tiles[k];
             const uint2 range = im.ranges[tile];
             const int n = (int)(range.y - range.x);
-            TileSort<kBigItems>::run(t16, flags, b.bucket + range.x, n, id_bits, tile, range.x, colors, g, b);
+            TileSort<kBigItems>::run(t16, flags, bl, b.bucket + range.x, n, id_bits, tile, grid_x, range.x, colors, g, b,
+                                     im.blk_count);
             __syncthreads();
         }
     } else {
@@ -340,10 +426,10 @@ __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_s
         const int n = (int)(range.y - range.x);
         if (n == 0 || n > (int)kBigTile) return;
         const uint2* __restrict__ src = b.bucket + range.x;
-        if (n <= 512) TileSort<1>::run(temp.t1, flags, src, n, id_bits, tile, range.x, colors, g, b);
-        else if (n <= 1024) TileSort<2>::run(temp.t2, flags, src, n, id_bits, tile, range.x, colors, g, b);
-        else if (n <= 1536) TileSort<3>::run(temp.t3, flags, src, n, id_bits, tile, range.x, colors, g, b);
-        else TileSort<4>::run(temp.t4, flags, src, n, id_bits, tile, range.x, colors, g, b);
+        if (n <= 512) TileSort<1>::run(temp.t1, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+        else if (n <= 1024) TileSort<2>::run(temp.t2, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+        else if (n <= 1536) TileSort<3>::run(temp.t3, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+        else TileSort<4>::run(temp.t4, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
     }
 }
 
@@ -354,10 +440,11 @@ int launch_tile_sort_gather(const Camera& cam, int P, uint32_t max_count, const 
     int id_bits = 1;
     while (id_bits < 32 && (1ll << id_bits) < (long long)P) ++id_bits;
     const int tiles = cam.grid_x * cam.grid_y;
-    tile_sort_gather_kernel<false><<<tiles, kSortThreads, 0, stream>>>(colors, g, b, im, id_bits);
+    tile_sort_gather_kernel<false><<<tiles, kSortThreads, 0, stream>>>(colors, g, b, im, id_bits, cam.grid_x);
     GPSG_LAUNCH_CHECK();
     if (max_count > kBigTile) {   // exact mode passes the real maximum; planned mode passes kMaxTileSort (always launch)
-        tile_sort_gather_kernel<true><<<min(tiles, kBigTileCTAs), kSortThreads, 0, stream>>>(colors, g, b, im, id_bits);
+        tile_sort_gather_kernel<true><<<min(tiles, kBigTileCTAs), kSortThreads, 0, stream>>>(colors, g, b, im, id_bits,
+                                                                                             cam.grid_x);
         GPSG_LAUNCH_CHECK();
     }
     return GPSG_OK;
@@ -388,11 +475,26 @@ __global__ void __launch_bounds__(256) gather_ranges_kernel(size_t N, const Gaus
     b.slabC[i] = C;
 }
 
+// One CTA per tile, after gather_ranges: the per-block survivor lists from the tile's slabs (any tile length).
+__global__ void __launch_bounds__(kSortThreads) block_lists_kernel(int grid_x, BinningState b, ImageState im) {
+    __shared__ BlockLists bl;
+    const uint32_t tile = blockIdx.x;
+    const uint2 range = im.ranges[tile];
+    const uint32_t n = range.y - range.x;
+    if (n == 0) return;
+    const int tile_y = (int)tile / grid_x;
+    build_block_lists(bl, b.slabA + range.x, n, (int)tile - tile_y * grid_x, tile_y, b.blk_list + 8 * (size_t)range.x,
+                      im.blk_count + 8 * (size_t)tile);
+}
+
 int launch_gather_ranges(const Camera& cam, size_t N, const GaussianSrc& colors, GeomState g, BinningState b, ImageState im,
                          cudaStream_t stream) {
-    GPSG_CUDA(cudaMemsetAsync(im.ranges, 0, sizeof(uint2) * (size_t)cam.grid_x * cam.grid_y, stream));
+    const int tiles = cam.grid_x * cam.grid_y;
+    GPSG_CUDA(cudaMemsetAsync(im.ranges, 0, sizeof(uint2) * (size_t)tiles, stream));
     if (N == 0) return GPSG_OK;
     gather_ranges_kernel<<<(unsigned)((N + 255) / 256), 256, 0, stream>>>(N, colors, g, b, im);
+    GPSG_LAUNCH_CHECK();
+    block_lists_kernel<<<tiles, kSortThreads, 0, stream>>>(cam.grid_x, b, im);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;
 }

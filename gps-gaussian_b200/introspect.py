@@ -90,7 +90,10 @@ class RasterCall:
             _lib.check(_lib.lib.gpsg_binning_view(C.c_void_p(binning.data_ptr()), N, C.byref(bv)), "gpsg_binning_view")
             st["keys"] = _sub(binning, bv.point_list_keys, 8 * N, torch.int64)
             st["point_list"] = _sub(binning, bv.point_list, 4 * N, torch.int32)
+            st["slabA"] = _sub(binning, bv.slabA, 16 * N, torch.float32).view(N, 4)
+            st["block_lists"] = _sub(binning, bv.block_lists, 32 * N, torch.int32)
         st["final_T"] = _sub(image, iv.final_T, 4 * H * W, torch.float32).view(H, W)
         st["n_contrib"] = _sub(image, iv.n_contrib, 4 * H * W, torch.int32).view(H, W)
         st["ranges"] = _sub(image, iv.ranges, 8 * tiles, torch.int32).view(tiles, 2)
+        st["block_counts"] = _sub(image, iv.block_counts, 32 * tiles, torch.int32).view(tiles, 8)
         return st

@@ -317,11 +317,15 @@ typedef struct GpsgGeomView {
 typedef struct GpsgBinningView {
     const uint64_t* point_list_keys; /* [N] sorted */
     const uint32_t* point_list;      /* [N] sorted Gaussian ids */
+    const float* slabA;              /* [N,4] (x, y, cull half-extent x, y), sorted */
+    const uint32_t* block_lists;     /* [8N] per 8x4 block of a tile with range [s, s+n): its survivors' tile-local list
+                                        positions at [8s + k*n, 8s + k*n + block_counts[8*tile + k]) */
 } GpsgBinningView;
 typedef struct GpsgImageView {
     const float* final_T;       /* [H*W] */
     const uint32_t* n_contrib;  /* [H*W] */
     const uint32_t* ranges;     /* [tiles,2] */
+    const uint32_t* block_counts; /* [tiles,8] survivors per block (valid for non-empty tiles) */
 } GpsgImageView;
 GPSG_API int gpsg_geom_view(const void* geom_buffer, int P, GpsgGeomView* out);
 GPSG_API int gpsg_binning_view(const void* binning_buffer, int64_t num_rendered, GpsgBinningView* out);
