@@ -153,6 +153,10 @@ lib.gpsg_l1_ssim_forward.restype = _i
 lib.gpsg_l1_ssim_forward.argtypes = [_i, _vp, _i, _i, _i, _vp, _vp, C.c_float, C.c_float, _vp, _vp, _vp]
 lib.gpsg_l1_ssim_backward.restype = _i
 lib.gpsg_l1_ssim_backward.argtypes = [_i, _vp, _i, _i, _i, _vp, _vp, _vp, C.c_float, C.c_float, _vp, _vp]
+lib.gpsg_point_splat_workspace_bytes.restype = _sz
+lib.gpsg_point_splat_workspace_bytes.argtypes = [_i, _i]
+lib.gpsg_point_splat.restype = _i
+lib.gpsg_point_splat.argtypes = [_i, _vp, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -176,7 +180,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_rasterize_forward_maps_planned_aux", "gpsg_rasterize_backward_aux_workspace_bytes",
             "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
             "gpsg_rasterize_backward_maps_aux", "gpsg_rasterize_forward_ex", "gpsg_rasterize_forward_maps_begin_ex",
-            "gpsg_rasterize_forward_planned_ex", "gpsg_rasterize_forward_maps_planned_ex"]
+            "gpsg_rasterize_forward_planned_ex", "gpsg_rasterize_forward_maps_planned_ex",
+            "gpsg_point_splat_workspace_bytes", "gpsg_point_splat"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

@@ -31,6 +31,7 @@ SOURCES = {
     "sh.cu": [],
     "unproject.cu": [],
     "loss.cu": [],
+    "point_splat.cu": [],
 }
 
 

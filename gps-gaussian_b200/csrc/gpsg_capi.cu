@@ -897,6 +897,23 @@ int gpsg_unproject_backward(int device, void* stream_, int B, int S, const float
                                 dL_ddepth, dL_dflow, (cudaStream_t)stream_);
 }
 
+size_t gpsg_point_splat_workspace_bytes(int B, int res) {
+    return (B > 0 && res > 0 && (int64_t)res * res < (int64_t(1) << 31)) ? point_splat_workspace_bytes(B, res) : 0;
+}
+
+int gpsg_point_splat(int device, void* stream_, int B, int N, int res, int64_t rows_per_batch, const float* pts,
+                     const float* mask, float* depth, float* color, void* workspace) {
+    GPSG_REQUIRE(B >= 0 && N >= 0 && rows_per_batch >= 0, "point_splat: negative size");
+    GPSG_REQUIRE(res >= 1, "point_splat: res must be >= 1");
+    GPSG_REQUIRE(N <= rows_per_batch, "point_splat: N > rows_per_batch");
+    GPSG_REQUIRE((int64_t)res * res < (int64_t(1) << 31), "point_splat: res^2 must be < 2^31");
+    if ((int64_t)B * N == 0) return GPSG_OK;
+    GPSG_REQUIRE(pts && mask && depth && color && workspace, "NULL pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 8 == 0, "point_splat: workspace must be 8-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_point_splat(B, N, res, rows_per_batch, pts, mask, depth, color, workspace, (cudaStream_t)stream_);
+}
+
 size_t gpsg_l1_ssim_workspace_bytes(int planes, int H, int W) {
     return (planes > 0 && H > 0 && W > 0) ? l1_ssim_workspace_bytes(planes, H, W) : 256;
 }

@@ -227,6 +227,10 @@ int launch_unproject_fwd(int B, int S, const float* flow, const float* mask, int
 int launch_unproject_bwd(int B, int S, const float* depth, const float* mask, int64_t mask_bs, const float* intr,
                          const float* extr, int extr_rows, const float* ref_intr, const float* Tf_x,
                          const float* dL_dxyz, const float* dL_ddepth, float* dL_dflow, cudaStream_t stream);
+// point_splat.cu
+size_t point_splat_workspace_bytes(int B, int res);
+int launch_point_splat(int B, int N, int res, int64_t rows, const float* pts, const float* mask, float* depth, float* color,
+                       void* workspace, cudaStream_t stream);
 // corr.cu
 int corr_build_mode();            // 0 = wgmma when possible, 1 = FFMA kernels
 void set_corr_build_mode(int m);

@@ -43,13 +43,15 @@ def add_reference_to_path():
     return ref
 
 
-def stage2_yaml(data_root, src_res=512, num_steps=3, batch_size=2, corr_implementation=None, use_processed_data=True):
+def stage2_yaml(data_root, src_res=512, num_steps=3, batch_size=2, corr_implementation=None, use_processed_data=True,
+                stage1_ckpt=None):
     """The reference's own config/stage2.yaml with only the user-facing knobs changed (data_root and stage1_ckpt are
-    placeholders upstream: 'PATH/TO/...')."""
+    placeholders upstream: 'PATH/TO/...').  stage1_ckpt: the stage-1 checkpoint stage 2 warm-starts from
+    (train_stage2.py:50-52); None leaves it unset."""
     import yaml
     with open(os.path.join(staged_reference(), "config", "stage2.yaml")) as f:
         y = yaml.safe_load(f)
-    y["stage1_ckpt"] = "None"
+    y["stage1_ckpt"] = "None" if stage1_ckpt is None else str(stage1_ckpt)
     y["num_steps"] = int(num_steps)
     y["batch_size"] = int(batch_size)
     y["dataset"]["src_res"] = int(src_res)
@@ -60,9 +62,28 @@ def stage2_yaml(data_root, src_res=512, num_steps=3, batch_size=2, corr_implemen
     return yaml.safe_dump(y, sort_keys=False)
 
 
-def make_workdir(path, data_root, **cfg):
+def stage1_yaml(data_root, src_res=512, num_steps=3, batch_size=2, eval_freq=2, loss_freq=2, use_processed_data=True):
+    """The reference's own config/stage1.yaml with only the user-facing knobs changed.  train_stage1.py evaluates (and
+    writes its preview JPEG) at every nonzero step that is a multiple of record.eval_freq, and saves `_latest.pth` at
+    multiples of record.loss_freq (:63-65, :76): the defaults make a 3-step run reach both at step 2.  Its eval draws
+    from int(len(val_loader) / val_boost) batches of 2, so the val split needs at least 2 samples."""
+    import yaml
+    with open(os.path.join(staged_reference(), "config", "stage1.yaml")) as f:
+        y = yaml.safe_load(f)
+    y["num_steps"] = int(num_steps)
+    y["batch_size"] = int(batch_size)
+    y["dataset"]["src_res"] = int(src_res)
+    y["dataset"]["data_root"] = str(data_root)
+    y["dataset"]["use_processed_data"] = bool(use_processed_data)
+    y["record"]["eval_freq"] = int(eval_freq)
+    y["record"]["loss_freq"] = int(loss_freq)
+    return yaml.safe_dump(y, sort_keys=False)
+
+
+def make_workdir(path, data_root, stage1=None, **cfg):
     """A working copy of the staged tree (the scripts resolve 'config/stage2.yaml', 'core', 'lib', ... relative to the
-    cwd and write experiments/ into it) with our config/stage2.yaml in place of the placeholder one."""
+    cwd and write experiments/ into it) with our config/stage2.yaml in place of the placeholder one.  stage1: a dict of
+    `stage1_yaml` keywords; when given, config/stage1.yaml is replaced as well."""
     ref = staged_reference()
     if ref is None:
         raise FileNotFoundError("oracle/_ref is not staged")
@@ -72,6 +93,9 @@ def make_workdir(path, data_root, **cfg):
     make_writable(path)                 # a read-only checkout keeps its modes through the copies
     with open(os.path.join(path, "config", "stage2.yaml"), "w") as f:
         f.write(stage2_yaml(data_root, **cfg))
+    if stage1 is not None:
+        with open(os.path.join(path, "config", "stage1.yaml"), "w") as f:
+            f.write(stage1_yaml(data_root, **stage1))
     return path
 
 
@@ -110,13 +134,14 @@ def run_script(workdir, script, args=(), patch=False, timeout=900):
 # in-process: the reference's own model, loader and optimisation step
 # ----------------------------------------------------------------------------------------------------------------
 
-def load_cfg(data_root, **kw):
+def load_cfg(data_root, stage=2, **kw):
+    """The reference's config object loaded from our stage2.yaml (stage=2) or stage1.yaml (stage=1)."""
     add_reference_to_path()
     import tempfile
     from config.stereo_human_config import ConfigStereoHuman
     c = ConfigStereoHuman()
     with tempfile.NamedTemporaryFile("w", suffix=".yaml", delete=False) as f:
-        f.write(stage2_yaml(data_root, **kw))
+        f.write((stage1_yaml if stage == 1 else stage2_yaml)(data_root, **kw))
     try:
         c.load(f.name)
     finally:
@@ -213,3 +238,58 @@ def c3_step(st, data, pts2render=None, timers=None, allreduce=None):
         for (_, a), (name, b) in zip(ev[:-1], ev[1:]):
             timers[name] = timers.get(name, 0.0) + a.elapsed_time(b)
     return out
+
+
+class Stage1State(C3State):
+    """What train_stage1.py's Trainer.__init__ builds (:30-52), minus logger / val set / checkpoint I/O: the depth-only
+    model (no Gaussian head), fp32 RAFT (config/stage1.yaml: mixed_precision False, so the GradScaler is disabled) and
+    the preview renderer `TaichiRenderBatch(bs=1, res=src_res)` (through the `taichi` stand-in in dropin/)."""
+
+    def __init__(self, cfg, seed=1314, device="cuda"):
+        import numpy as np
+        import torch
+        import torch.optim as optim
+        from torch.cuda.amp import GradScaler
+        from lib.human_loader import StereoHumanDataset
+        from lib.network import RtStereoHumanModel
+        from lib.TaichiRender import TaichiRenderBatch
+        torch.manual_seed(seed)                                                     # train_stage1.py:186-187
+        np.random.seed(seed)
+        self.cfg = cfg
+        self.device = device
+        self.model = RtStereoHumanModel(cfg, with_gs_render=False)
+        self.train_set = StereoHumanDataset(cfg.dataset, phase='train')
+        self.optimizer = optim.AdamW(self.model.parameters(), lr=cfg.lr, weight_decay=cfg.wdecay, eps=1e-8)
+        self.scheduler = optim.lr_scheduler.OneCycleLR(self.optimizer, cfg.lr, 100100, pct_start=0.01,
+                                                       cycle_momentum=False, anneal_strategy='linear')
+        self.model.to(device)
+        self.model.train()
+        self.model.raft_stereo.freeze_bn()
+        self.scaler = GradScaler(enabled=cfg.raft.mixed_precision)
+        self.render = TaichiRenderBatch(bs=1, res=cfg.dataset.src_res)
+
+    def batch(self, first=0):
+        """`batch_size` training samples collated like the reference DataLoader, source views moved to the GPU like
+        Trainer.fetch_data (train_stage1.py:135-137).  Stage-1 samples have no novel view."""
+        from torch.utils.data import default_collate
+        data = default_collate([self.train_set[first + k] for k in range(self.cfg.batch_size)])
+        for view in ('lmain', 'rmain'):
+            for item in data[view].keys():
+                data[view][item] = data[view][item].to(self.device)
+        return data
+
+
+def stage1_step(st, data):
+    """One optimisation step, statement for statement train_stage1.py:56-74 (logging / checkpointing left out)."""
+    import torch
+    st.optimizer.zero_grad()                                                          # :56
+    _, flow_loss, metrics = st.model(data)                                            # :60
+    loss = flow_loss                                                                  # :61
+    st.scaler.scale(loss).backward()                                                  # :68
+    st.scaler.unscale_(st.optimizer)                                                  # :69
+    gnorm = torch.nn.utils.clip_grad_norm_(st.model.parameters(), 1.0)                # :70
+    st.scaler.step(st.optimizer)                                                      # :72
+    st.scheduler.step()
+    st.scaler.update()                                                                # :74
+    return {"loss": loss.detach(), "flow_loss": flow_loss.detach(), "metrics": metrics,
+            "grad_norm": gnorm.detach() if torch.is_tensor(gnorm) else gnorm}

@@ -377,7 +377,23 @@ GPSG_API int gpsg_unproject_backward(int device, void* stream, int B, int S, con
                                      const float* ref_intr, const float* Tf_x, const float* dL_dxyz,
                                      const float* dL_ddepth, float* dL_dflow);
 
-/* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4) -----------------------------------------------
+/* ---- point splat: the stage-1 preview's 1-pixel z-buffer on inverse depth (reference lib/TaichiRender.py:13-24) ------
+ * One call = one call of `render_respective_color` over the loop domain (B, N):
+ *   pts[Bp, rows_per_batch, 6] = (x_pix, y_pix, inverse depth, r, g, b), mask[Bp, rows_per_batch] (point skipped when
+ *   mask < 0.5), depth[Bp, 1, res, res] and color[Bp, 3, res, res] in/out, Bp >= B, rows_per_batch >= N.  Batches b >= B
+ *   and rows i >= N are not read or written.
+ * The result is the serial reading of the reference kernel (points in index order), race-free and bit-exact: per pixel,
+ * with M the largest z landing there, colour <- rgb of the highest index with z == M when M >= old depth, and depth <-
+ * M (the first such point's value) when M > old depth.  NaN z is skipped; x, y truncate towards zero with saturation
+ * (NaN -> 0) and clamp to [0, res-1].
+ * workspace: gpsg_point_splat_workspace_bytes(B, res) bytes, 8-byte aligned; the call zeroes it on the stream.
+ * B == 0 or N == 0 is a no-op.  Refused (GPSG_E_INVALID): negative sizes, res < 1, N > rows_per_batch, res^2 >= 2^31,
+ * NULL pointers when there is work. */
+GPSG_API size_t gpsg_point_splat_workspace_bytes(int B, int res);
+GPSG_API int gpsg_point_splat(int device, void* stream, int B, int N, int res, int64_t rows_per_batch, const float* pts,
+                              const float* mask, float* depth, float* color, void* workspace);
+
+/* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.
  * img, gt: [planes, H, W] fp32 (planes = B*C).  out3 (device float[3]) = { w_l1*L1 + w_ssim*(1-SSIM), L1, SSIM }.
