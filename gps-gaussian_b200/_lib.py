@@ -157,6 +157,23 @@ lib.gpsg_point_splat_workspace_bytes.restype = _sz
 lib.gpsg_point_splat_workspace_bytes.argtypes = [_i, _i]
 lib.gpsg_point_splat.restype = _i
 lib.gpsg_point_splat.argtypes = [_i, _vp, _i, _i, _i, _i64, _vp, _vp, _vp, _vp, _vp]
+
+
+class RectifyCamera(C.Structure):
+    """GpsgRectifyCamera (include/gpsg.h): source K, rectifying R and P[:3,:3], fp64 row-major."""
+    _fields_ = [("K", C.c_double * 9), ("R", C.c_double * 9), ("P", C.c_double * 9)]
+
+
+class RectifyPlanes(C.Structure):
+    """GpsgRectifyPlanes (include/gpsg.h): one view's device pointers, NULL where absent."""
+    _fields_ = [(n, C.c_void_p) for n in ("img", "mask", "depth", "img_out", "mask_out", "depth_out", "img_tensor",
+                                          "mask_tensor")]
+
+
+lib.gpsg_rectify_remap.restype = _i
+lib.gpsg_rectify_remap.argtypes = [_i, _vp, C.POINTER(RectifyCamera), _i, _i, _i, _i, _i, _i, C.POINTER(RectifyPlanes)]
+lib.gpsg_rectify_flow.restype = _i
+lib.gpsg_rectify_flow.argtypes = [_i, _vp, _i, _i, _i, C.c_double, C.c_double, C.c_double, _pp, _pp, _pp, _pp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -181,7 +198,7 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
             "gpsg_rasterize_backward_maps_aux", "gpsg_rasterize_forward_ex", "gpsg_rasterize_forward_maps_begin_ex",
             "gpsg_rasterize_forward_planned_ex", "gpsg_rasterize_forward_maps_planned_ex",
-            "gpsg_point_splat_workspace_bytes", "gpsg_point_splat"]
+            "gpsg_point_splat_workspace_bytes", "gpsg_point_splat", "gpsg_rectify_remap", "gpsg_rectify_flow"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

@@ -4,7 +4,8 @@
 
 Output: gps-gaussian_b200/lib/libgpsg_sm90.so (git-ignored build product).
 raster_preprocess.cu is compiled with -fmad=false (see its header): the fp32 op order that decides
-radii / tile rectangles must not be FMA-contracted.
+radii / tile rectangles must not be FMA-contracted.  rectify.cu likewise: its fp32 / fp64 op order is what makes
+the rectified images and flow bit-identical to OpenCV.
 """
 import os
 import subprocess
@@ -32,6 +33,7 @@ SOURCES = {
     "unproject.cu": [],
     "loss.cu": [],
     "point_splat.cu": [],
+    "rectify.cu": ["-fmad=false"],
 }
 
 

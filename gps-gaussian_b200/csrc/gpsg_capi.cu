@@ -914,6 +914,36 @@ int gpsg_point_splat(int device, void* stream_, int B, int N, int res, int64_t r
     return launch_point_splat(B, N, res, rows_per_batch, pts, mask, depth, color, workspace, (cudaStream_t)stream_);
 }
 
+int gpsg_rectify_remap(int device, void* stream_, const GpsgRectifyCamera* cams, int Hin, int Win, int C, int Cm, int H,
+                       int W, const GpsgRectifyPlanes* planes) {
+    GPSG_REQUIRE(cams && planes, "rectify_remap: NULL cams / planes");
+    GPSG_REQUIRE(Hin >= 1 && Win >= 1 && H >= 1 && W >= 1, "rectify_remap: sizes must be >= 1");
+    GPSG_REQUIRE((int64_t)Hin * Win < (int64_t(1) << 31) && (int64_t)H * W < (int64_t(1) << 31),
+                 "rectify_remap: planes must have < 2^31 pixels");
+    GPSG_REQUIRE(C == 1 || C == 3 || C == 4, "rectify_remap: C must be 1, 3 or 4");
+    GPSG_REQUIRE(Cm == 1 || Cm == 3 || Cm == 4, "rectify_remap: Cm must be 1, 3 or 4");
+    for (int k = 0; k < 2; ++k) {
+        const GpsgRectifyPlanes& p = planes[k];
+        GPSG_REQUIRE(p.img, "rectify_remap: NULL img");
+        GPSG_REQUIRE(!p.depth || p.depth_out, "rectify_remap: depth without depth_out");
+        GPSG_REQUIRE(p.mask || (!p.mask_out && !p.mask_tensor && !p.img_tensor),
+                     "rectify_remap: mask outputs and img_tensor need the mask");
+        GPSG_REQUIRE(!p.img_tensor || Cm == 1 || Cm == C, "rectify_remap: img_tensor needs Cm == 1 or Cm == C");
+    }
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_rectify_remap(cams, Hin, Win, C, Cm, H, W, planes, (cudaStream_t)stream_);
+}
+
+int gpsg_rectify_flow(int device, void* stream_, int H, int W, int Cm, double Tf_x, double cx0, double cx1,
+                      const float* const* depth, const uint8_t* const* mask, double* const* flow, uint8_t* const* valid) {
+    GPSG_REQUIRE(H >= 1 && W >= 1 && (int64_t)H * W < (int64_t(1) << 31), "rectify_flow: bad size");
+    GPSG_REQUIRE(Cm == 1 || Cm == 3 || Cm == 4, "rectify_flow: Cm must be 1, 3 or 4");
+    GPSG_REQUIRE(depth && mask && flow && valid, "NULL pointer");
+    for (int k = 0; k < 2; ++k) GPSG_REQUIRE(depth[k] && mask[k] && flow[k] && valid[k], "NULL pointer");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_rectify_flow(H, W, Cm, Tf_x, cx0, cx1, depth, mask, flow, valid, (cudaStream_t)stream_);
+}
+
 size_t gpsg_l1_ssim_workspace_bytes(int planes, int H, int W) {
     return (planes > 0 && H > 0 && W > 0) ? l1_ssim_workspace_bytes(planes, H, W) : 256;
 }

@@ -227,6 +227,26 @@ int launch_unproject_fwd(int B, int S, const float* flow, const float* mask, int
 int launch_unproject_bwd(int B, int S, const float* depth, const float* mask, int64_t mask_bs, const float* intr,
                          const float* extr, int extr_rows, const float* ref_intr, const float* Tf_x,
                          const float* dL_dxyz, const float* dL_ddepth, float* dL_dflow, cudaStream_t stream);
+// rectify.cu
+struct RectifyView {
+    double iR[9];                        // inv(P3 R), row-major
+    double fx, fy, cx, cy;               // source intrinsics
+    const uint8_t* img; const uint8_t* mask; const float* depth;
+    uint8_t* img_out; uint8_t* mask_out; float* depth_out; float* img_tensor; float* mask_tensor;
+};
+struct RectifyArgs {
+    RectifyView v[2];
+    int Hin, Win, C, Cm, H, W;
+};
+struct RectifyFlowArgs {
+    const float* depth[2]; const uint8_t* mask[2]; double* flow[2]; uint8_t* valid[2];
+    double offset[2], tf[2];
+    int H, W, Cm;
+};
+int launch_rectify_remap(const GpsgRectifyCamera* cams, int Hin, int Win, int C, int Cm, int H, int W,
+                         const GpsgRectifyPlanes* planes, cudaStream_t stream);
+int launch_rectify_flow(int H, int W, int Cm, double Tf_x, double cx0, double cx1, const float* const* depth,
+                        const uint8_t* const* mask, double* const* flow, uint8_t* const* valid, cudaStream_t stream);
 // point_splat.cu
 size_t point_splat_workspace_bytes(int B, int res);
 int launch_point_splat(int B, int N, int res, int64_t rows, const float* pts, const float* mask, float* depth, float* color,

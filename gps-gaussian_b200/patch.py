@@ -16,14 +16,26 @@ the stage-2 step both ways).  `install()` / `uninstall()` do the same for module
 `GPSG_ANTIALIAS=1`, read once by `install()`, makes the rebound `pts2render` render with the opacity-compensated
 screen-space filter (`pts2render_ex(..., antialiasing=True)`, forward and backward), so the unmodified training and
 novel-view scripts train and render anti-aliased; unset or any other value keeps the reference's image.
+
+`GPSG_RECTIFY=1`, read once by `install()`, also hooks `lib.human_loader` and rebinds two methods of its
+`StereoHumanDataset` to the rectification kernels (gps_gaussian_b200.rectify, csrc/rectify.cu), with identical results:
+
+    get_rectified_stereo_data -> rectify.rectify_stereo    (every main-process caller, the rectified_local/ cache included)
+    get_test_item             -> rectify.stereo_item_cuda  (test_real_data.py: lmain/rmain img and mask arrive on the GPU)
+
+Inside a DataLoader worker (forked, no CUDA) or without CUDA both call the reference's own method.  Unset or any other
+value leaves `lib.human_loader` alone: it is then not even hooked.
 """
 import importlib.abc
 import importlib.machinery
+import logging
 import os
 import sys
 
 _ORIG = {}            # (module name, attribute) -> original object
+_ORIG_METHODS = {}    # (class, attribute) -> original function
 _ANTIALIAS = False    # GPSG_ANTIALIAS=1 at install()
+_RECTIFY = False      # GPSG_RECTIFY=1 at install()
 
 
 def _set(mod, attr, new):
@@ -53,7 +65,59 @@ def _patch_render(mod):
     _set(mod, "pts2render", _pts2render_antialiased if _ANTIALIAS else ours.pts2render)
 
 
+def _on_device():
+    """The GPU route runs in the main process with CUDA; a DataLoader worker is forked and must not touch CUDA."""
+    import torch
+    return torch.utils.data.get_worker_info() is None and torch.cuda.is_available()
+
+
+def _rectified_stereo_data(orig, mod):
+    def get_rectified_stereo_data(self, main_view_data, ref_view_data):
+        if not _on_device():
+            return orig(self, main_view_data, ref_view_data)
+        from gps_gaussian_b200 import rectify
+        return rectify.rectify_stereo(main_view_data, ref_view_data, self.opt.src_res, pts2depth=mod.pts2depth)
+    return get_rectified_stereo_data
+
+
+def _test_item(orig, mod):
+    """get_test_item with the rectified pair made on the GPU: load both views, then stereo_item_cuda, then the original
+    intrinsics / extrinsics and the novel-view size, as the reference's method (lib/human_loader.py:390-419)."""
+    def get_test_item(self, index, source_id):
+        if not _on_device():
+            return orig(self, index, source_id)
+        import torch
+        from gps_gaussian_b200 import rectify
+        sample_name = self.sample_list[index % len(self.sample_list)]
+        if self.use_processed_data:
+            logging.error('test data loader not support processed data')
+        views = [self.load_single_view(sample_name, sid, hr_img=False, require_mask=True, require_pts=False)
+                 for sid in source_id[:2]]
+        item = rectify.stereo_item_cuda(views[0], views[1], self.opt.src_res, sample_name, pts2depth=mod.pts2depth)
+        for key, which in (('intr_ori', 2), ('extr_ori', 3)):
+            item['lmain'][key] = torch.FloatTensor(views[0][which])
+            item['rmain'][key] = torch.FloatTensor(views[1][which])
+        size = self.opt.src_res * 2 if self.opt.use_hr_img else self.opt.src_res
+        item['novel_view'] = {'height': torch.IntTensor([size]), 'width': torch.IntTensor([size])}
+        return item
+    return get_test_item
+
+
+def _patch_loader(mod):
+    cls = mod.StereoHumanDataset
+    for attr, wrap in (("get_rectified_stereo_data", _rectified_stereo_data), ("get_test_item", _test_item)):
+        key = (cls, attr)
+        if key not in _ORIG_METHODS:
+            _ORIG_METHODS[key] = cls.__dict__[attr]
+        setattr(cls, attr, wrap(_ORIG_METHODS[key], mod))
+
+
 _TARGETS = {"core.corr": _patch_corr, "lib.GaussianRender": _patch_render}
+_RECTIFY_TARGETS = {"lib.human_loader": _patch_loader}
+
+
+def _targets():
+    return {**_TARGETS, **_RECTIFY_TARGETS} if _RECTIFY else _TARGETS
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -70,7 +134,7 @@ class _PatchingLoader(importlib.abc.Loader):
 
 class _Finder(importlib.abc.MetaPathFinder):
     def find_spec(self, name, path=None, target=None):
-        hook = _TARGETS.get(name)
+        hook = _targets().get(name)
         if hook is None:
             return None
         for finder in sys.meta_path:
@@ -87,12 +151,14 @@ _FINDER = _Finder()
 
 
 def install():
-    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS here, once."""
-    global _ANTIALIAS
+    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS and GPSG_RECTIFY here,
+    once."""
+    global _ANTIALIAS, _RECTIFY
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
+    _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
-    for name, hook in _TARGETS.items():
+    for name, hook in _targets().items():
         if name in sys.modules:
             hook(sys.modules[name])
 
@@ -105,6 +171,9 @@ def uninstall():
         if mod is not None and orig is not None:
             setattr(mod, attr, orig)
     _ORIG.clear()
+    for (cls, attr), orig in list(_ORIG_METHODS.items()):
+        setattr(cls, attr, orig)
+    _ORIG_METHODS.clear()
 
 
 def active():
@@ -114,3 +183,8 @@ def active():
 def antialiasing():
     """Whether the installed patch renders with the screen-space filter (GPSG_ANTIALIAS=1 at install())."""
     return _ANTIALIAS
+
+
+def rectify():
+    """Whether the installed patch rectifies on the GPU (GPSG_RECTIFY=1 at install())."""
+    return _RECTIFY

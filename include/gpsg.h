@@ -393,6 +393,47 @@ GPSG_API size_t gpsg_point_splat_workspace_bytes(int B, int res);
 GPSG_API int gpsg_point_splat(int device, void* stream, int B, int N, int res, int64_t rows_per_batch, const float* pts,
                               const float* mask, float* depth, float* color, void* workspace);
 
+/* ---- stereo rectification of the real-data loader (reference lib/human_loader.py:245-366) ----------------------------
+ * gpsg_rectify_remap: cv2.initUndistortRectifyMap(K, 0, R, P, (W, H), CV_32FC1) + cv2.remap(INTER_LINEAR,
+ *   BORDER_CONSTANT 0) of both views of a pair in one launch, bit-identical to OpenCV 4.x (DESIGN.md §2).  cams[2] are
+ *   HOST structs passed to the kernel by value: the source intrinsics K, the rectifying rotation R and P[:3,:3] of
+ *   cv2.stereoRectify, all fp64 row-major.  Per view, planes[k] (HOST struct of device pointers):
+ *     img [Hin,Win,C] uint8 (C in {1,3,4}); mask [Hin,Win,Cm] uint8 (Cm in {1,3,4}) or NULL; depth [Hin,Win] fp32 or NULL;
+ *     numpy contract (what cv2.remap returns): img_out [H,W,C], mask_out [H,W,Cm] uint8, depth_out [H,W] fp32 (required
+ *       with depth);
+ *     tensor contract (stereo_to_dict_tensor, :319-331): img_tensor fp32 = (2*(v/255) - 1) * m_soft with m_soft =
+ *       mask/255 (channel c of the mask, or channel 0 when Cm == 1; needs Cm == 1 or Cm == C), mask_tensor fp32 =
+ *       (m_soft >= 0.5); both stored [H,W,C] / [H,W,Cm], i.e. the [C,H,W] tensors of that function with its strides
+ *       (1, W*C, C), which it inherits from permuting the numpy image;
+ *   any output may be NULL.  Refused: sizes < 1, unsupported C / Cm, NULL img, depth without depth_out, a tensor output
+ *   that needs the mask without one.
+ * gpsg_rectify_flow: the ground truth of stereo_pts2flow (:74-85) and the eroded valid mask (:298-315) of both views in
+ *   one launch.  depth[k] [H,W] fp32 is the rectified depth (depth_out above), mask[k] [H,W,Cm] the rectified mask;
+ *   flow[k] [H,W] fp64 = (cx_other - cx_self) - (-depth * Tf_x) (Tf_x -> -Tf_x for view 1), 0 where depth < 0.05, times
+ *   valid; valid is the 3x3 erode (border +inf) of fp32(mask[...,0] / 255.0) thresholded at 0.66; valid[k] [H,W] uint8 =
+ *   255 * valid.  cx0 / cx1 are P0[0,2] / P1[0,2].  Pointer arrays are host arrays of device pointers.
+ * Both enqueue one kernel on `stream` and do not synchronise. */
+typedef struct GpsgRectifyCamera {
+    double K[9];
+    double R[9];
+    double P[9];
+} GpsgRectifyCamera;
+typedef struct GpsgRectifyPlanes {
+    const uint8_t* img;
+    const uint8_t* mask;
+    const float* depth;
+    uint8_t* img_out;
+    uint8_t* mask_out;
+    float* depth_out;
+    float* img_tensor;
+    float* mask_tensor;
+} GpsgRectifyPlanes;
+GPSG_API int gpsg_rectify_remap(int device, void* stream, const GpsgRectifyCamera* cams, int Hin, int Win, int C, int Cm,
+                                int H, int W, const GpsgRectifyPlanes* planes);
+GPSG_API int gpsg_rectify_flow(int device, void* stream, int H, int W, int Cm, double Tf_x, double cx0, double cx1,
+                               const float* const* depth, const uint8_t* const* mask, double* const* flow,
+                               uint8_t* const* valid);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.
