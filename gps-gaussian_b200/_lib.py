@@ -174,6 +174,25 @@ lib.gpsg_rectify_remap.restype = _i
 lib.gpsg_rectify_remap.argtypes = [_i, _vp, C.POINTER(RectifyCamera), _i, _i, _i, _i, _i, _i, C.POINTER(RectifyPlanes)]
 lib.gpsg_rectify_flow.restype = _i
 lib.gpsg_rectify_flow.argtypes = [_i, _vp, _i, _i, _i, C.c_double, C.c_double, C.c_double, _pp, _pp, _pp, _pp]
+class SeqLossArgs(C.Structure):
+    """GpsgSeqLossArgs (include/gpsg.h), passed by value: prediction / gradient pointers and fp32 weights."""
+    _fields_ = [("pred", C.c_void_p * 32), ("grad", C.c_void_p * 32), ("weight", C.c_float * 32), ("gt", C.c_void_p),
+                ("valid", C.c_void_p), ("numel", C.c_int64), ("n_pred", C.c_int), ("gt_dtype", C.c_int)]
+
+
+SEQ_LOSS_MAX_PRED = 32    # GPSG_SEQ_LOSS_MAX_PRED (include/gpsg.h)
+lib.gpsg_convex_upsample_forward.restype = _i
+lib.gpsg_convex_upsample_forward.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]
+lib.gpsg_convex_upsample_backward_workspace_bytes.restype = _sz
+lib.gpsg_convex_upsample_backward_workspace_bytes.argtypes = [_i, _i, _i, _i]
+lib.gpsg_convex_upsample_backward.restype = _i
+lib.gpsg_convex_upsample_backward.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]
+lib.gpsg_sequence_loss_workspace_bytes.restype = _sz
+lib.gpsg_sequence_loss_workspace_bytes.argtypes = []
+lib.gpsg_sequence_loss_forward.restype = _i
+lib.gpsg_sequence_loss_forward.argtypes = [_i, _vp, SeqLossArgs, _vp, _vp]
+lib.gpsg_sequence_loss_backward.restype = _i
+lib.gpsg_sequence_loss_backward.argtypes = [_i, _vp, SeqLossArgs, _vp, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -198,7 +217,10 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
             "gpsg_rasterize_backward_maps_aux", "gpsg_rasterize_forward_ex", "gpsg_rasterize_forward_maps_begin_ex",
             "gpsg_rasterize_forward_planned_ex", "gpsg_rasterize_forward_maps_planned_ex",
-            "gpsg_point_splat_workspace_bytes", "gpsg_point_splat", "gpsg_rectify_remap", "gpsg_rectify_flow"]
+            "gpsg_point_splat_workspace_bytes", "gpsg_point_splat", "gpsg_rectify_remap", "gpsg_rectify_flow",
+            "gpsg_convex_upsample_forward", "gpsg_convex_upsample_backward_workspace_bytes",
+            "gpsg_convex_upsample_backward", "gpsg_sequence_loss_workspace_bytes", "gpsg_sequence_loss_forward",
+            "gpsg_sequence_loss_backward"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

@@ -34,6 +34,7 @@ SOURCES = {
     "loss.cu": [],
     "point_splat.cu": [],
     "rectify.cu": ["-fmad=false"],
+    "flow_head.cu": [],
 }
 
 

@@ -964,6 +964,70 @@ int gpsg_l1_ssim_backward(int device, void* stream_, int planes, int H, int W, c
     return launch_l1_ssim_bwd(planes, H, W, img, gt, dmaps, w_l1, w_ssim, grad_loss, dimg, (cudaStream_t)stream_);
 }
 
+static int check_upsample(int mask_dtype, int factor, int N, int D, int H, int W) {
+    GPSG_REQUIRE(mask_dtype == 0 || mask_dtype == 1, "convex_upsample: mask_dtype must be 0 (fp32) or 1 (fp16)");
+    GPSG_REQUIRE(factor == 2 || factor == 4 || factor == 8, "convex_upsample: factor must be 2, 4 or 8");
+    GPSG_REQUIRE(D == 1 || D == 2, "convex_upsample: D must be 1 or 2");
+    GPSG_REQUIRE(N >= 0 && H >= 0 && W >= 0 && N <= 65535 && H <= 65535, "convex_upsample: bad shape");
+    GPSG_REQUIRE((int64_t)N * 9 * factor * factor * H * W < (int64_t(1) << 40), "convex_upsample: mask too large");
+    return GPSG_OK;
+}
+
+int gpsg_convex_upsample_forward(int device, void* stream_, int mask_dtype, int factor, int N, int D, int H, int W,
+                                 const float* flow, const void* mask, float* out) {
+    if (int rc = check_upsample(mask_dtype, factor, N, D, H, W)) return rc;
+    if ((int64_t)N * H * W == 0) return GPSG_OK;
+    GPSG_REQUIRE(flow && mask && out, "NULL pointer");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_convex_upsample_fwd(mask_dtype, factor, N, D, H, W, flow, mask, out, (cudaStream_t)stream_);
+}
+
+size_t gpsg_convex_upsample_backward_workspace_bytes(int N, int D, int H, int W) {
+    return (N > 0 && D > 0 && H > 0 && W > 0) ? convex_upsample_workspace_bytes(N, D, H, W) : 0;
+}
+
+int gpsg_convex_upsample_backward(int device, void* stream_, int mask_dtype, int factor, int N, int D, int H, int W,
+                                  const float* flow, const void* mask, const float* grad_out, void* grad_mask,
+                                  float* grad_flow, void* workspace) {
+    if (int rc = check_upsample(mask_dtype, factor, N, D, H, W)) return rc;
+    if ((int64_t)N * H * W == 0) return GPSG_OK;
+    GPSG_REQUIRE(flow && mask && grad_out && (grad_mask || grad_flow), "NULL pointer");
+    GPSG_REQUIRE(!grad_flow || workspace, "convex_upsample_backward: grad_flow needs the workspace");
+    GPSG_REQUIRE((uintptr_t)workspace % 4 == 0, "convex_upsample_backward: workspace must be 4-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_convex_upsample_bwd(mask_dtype, factor, N, D, H, W, flow, mask, grad_out, grad_mask, grad_flow, workspace,
+                                      (cudaStream_t)stream_);
+}
+
+static int check_seq_loss(const GpsgSeqLossArgs& a) {
+    GPSG_REQUIRE(a.n_pred >= 1 && a.n_pred <= GPSG_SEQ_LOSS_MAX_PRED, "sequence_loss: n_pred must be in [1, 32]");
+    GPSG_REQUIRE(a.numel >= 0, "sequence_loss: negative numel");
+    GPSG_REQUIRE(a.gt_dtype == 0 || a.gt_dtype == 1, "sequence_loss: gt_dtype must be 0 (fp32) or 1 (fp16)");
+    GPSG_REQUIRE(a.numel == 0 || (a.gt && a.valid), "NULL pointer");
+    for (int i = 0; i < a.n_pred; ++i) GPSG_REQUIRE(a.numel == 0 || a.pred[i], "NULL pointer");
+    return GPSG_OK;
+}
+
+size_t gpsg_sequence_loss_workspace_bytes(void) { return sequence_loss_workspace_bytes(); }
+
+int gpsg_sequence_loss_forward(int device, void* stream_, GpsgSeqLossArgs args, float* stats, void* workspace) {
+    if (int rc = check_seq_loss(args)) return rc;
+    GPSG_REQUIRE(stats && workspace, "NULL pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 8 == 0, "sequence_loss: workspace must be 8-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_sequence_loss_fwd(args, stats, workspace, (cudaStream_t)stream_);
+}
+
+int gpsg_sequence_loss_backward(int device, void* stream_, GpsgSeqLossArgs args, const float* grad_loss,
+                                const float* stats) {
+    if (int rc = check_seq_loss(args)) return rc;
+    GPSG_REQUIRE(stats, "NULL pointer");
+    for (int i = 0; i < args.n_pred; ++i) GPSG_REQUIRE(args.numel == 0 || args.grad[i], "NULL pointer");
+    if (args.numel == 0) return GPSG_OK;
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_sequence_loss_bwd(args, grad_loss, stats, (cudaStream_t)stream_);
+}
+
 int gpsg_set_corr_build(int mode) {
     set_corr_build_mode(mode);
     return GPSG_OK;

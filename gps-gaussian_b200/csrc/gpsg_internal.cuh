@@ -251,6 +251,16 @@ int launch_rectify_flow(int H, int W, int Cm, double Tf_x, double cx0, double cx
 size_t point_splat_workspace_bytes(int B, int res);
 int launch_point_splat(int B, int N, int res, int64_t rows, const float* pts, const float* mask, float* depth, float* color,
                        void* workspace, cudaStream_t stream);
+// flow_head.cu (dtype: 0 = fp32 mask, 1 = fp16 mask)
+int launch_convex_upsample_fwd(int dtype, int f, int N, int D, int H, int W, const float* flow, const void* mask, float* out,
+                               cudaStream_t stream);
+size_t convex_upsample_workspace_bytes(int N, int D, int H, int W);
+int launch_convex_upsample_bwd(int dtype, int f, int N, int D, int H, int W, const float* flow, const void* mask,
+                               const float* grad_out, void* grad_mask, float* grad_flow, void* workspace,
+                               cudaStream_t stream);
+size_t sequence_loss_workspace_bytes();
+int launch_sequence_loss_fwd(const GpsgSeqLossArgs& a, float* stats, void* workspace, cudaStream_t stream);
+int launch_sequence_loss_bwd(const GpsgSeqLossArgs& a, const float* grad_loss, const float* stats, cudaStream_t stream);
 // corr.cu
 int corr_build_mode();            // 0 = wgmma when possible, 1 = FFMA kernels
 void set_corr_build_mode(int m);

@@ -25,6 +25,16 @@ novel-view scripts train and render anti-aliased; unset or any other value keeps
 
 Inside a DataLoader worker (forked, no CUDA) or without CUDA both call the reference's own method.  Unset or any other
 value leaves `lib.human_loader` alone: it is then not even hooked.
+
+`GPSG_FLOW_HEAD=1`, read once by `install()`, also hooks the disparity head of both training stages
+(gps_gaussian_b200.flow_head, csrc/flow_head.cu):
+
+    core.raft_stereo_human.FlowUpdateModule.upsample_flow -> fused convex upsampling (a class method, kept in _ORIG_METHODS)
+    lib.loss.sequence_loss (and lib.network's copy)        -> flow_head.sequence_loss (one host synchronisation)
+
+Inputs the kernels do not cover (CPU tensors, other dtypes or factors) reach the reference's own function.  The results
+differ from the op chain's by fp32 re-association and by where fp16 rounding falls in the backward, which is why the
+switch is opt-in.  Unset or any other value hooks neither.
 """
 import importlib.abc
 import importlib.machinery
@@ -36,6 +46,7 @@ _ORIG = {}            # (module name, attribute) -> original object
 _ORIG_METHODS = {}    # (class, attribute) -> original function
 _ANTIALIAS = False    # GPSG_ANTIALIAS=1 at install()
 _RECTIFY = False      # GPSG_RECTIFY=1 at install()
+_FLOW_HEAD = False    # GPSG_FLOW_HEAD=1 at install()
 
 
 def _set(mod, attr, new):
@@ -112,12 +123,40 @@ def _patch_loader(mod):
         setattr(cls, attr, wrap(_ORIG_METHODS[key], mod))
 
 
+def _patch_upsample(mod):
+    from gps_gaussian_b200 import flow_head
+    cls = mod.FlowUpdateModule
+    key = (cls, "upsample_flow")
+    if key not in _ORIG_METHODS:
+        _ORIG_METHODS[key] = cls.__dict__["upsample_flow"]
+    cls.upsample_flow = flow_head.make_upsample_flow(_ORIG_METHODS[key])
+
+
+def _patch_loss(mod):
+    from gps_gaussian_b200 import flow_head
+    _set(mod, "sequence_loss", flow_head.sequence_loss)
+    user = sys.modules.get("lib.network")                     # `from lib.loss import sequence_loss` copies the binding
+    if user is not None and hasattr(user, "sequence_loss"):
+        _set(user, "sequence_loss", flow_head.sequence_loss)
+
+
+# Modules whose `from <module> import <attr>` made after install() copies the rebound object without _set seeing it;
+# uninstall() puts the original back there too.
+_COPIES = {("lib.loss", "sequence_loss"): ("lib.network",)}
+
+
+def original(mod, attr):
+    """The object `mod.attr` had before the patch rebound it (itself when it was never rebound)."""
+    return _ORIG.get((mod.__name__, attr)) or getattr(mod, attr)
+
+
 _TARGETS = {"core.corr": _patch_corr, "lib.GaussianRender": _patch_render}
 _RECTIFY_TARGETS = {"lib.human_loader": _patch_loader}
+_FLOW_HEAD_TARGETS = {"core.raft_stereo_human": _patch_upsample, "lib.loss": _patch_loss}
 
 
 def _targets():
-    return {**_TARGETS, **_RECTIFY_TARGETS} if _RECTIFY else _TARGETS
+    return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {})}
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -151,11 +190,12 @@ _FINDER = _Finder()
 
 
 def install():
-    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS and GPSG_RECTIFY here,
-    once."""
-    global _ANTIALIAS, _RECTIFY
+    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY and
+    GPSG_FLOW_HEAD here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
+    _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -169,6 +209,9 @@ def uninstall():
     for (modname, attr), orig in list(_ORIG.items()):
         mod = sys.modules.get(modname)
         if mod is not None and orig is not None:
+            for user in filter(None, map(sys.modules.get, _COPIES.get((modname, attr), ()))):
+                if getattr(user, attr, None) is getattr(mod, attr):
+                    setattr(user, attr, orig)
             setattr(mod, attr, orig)
     _ORIG.clear()
     for (cls, attr), orig in list(_ORIG_METHODS.items()):
@@ -188,3 +231,8 @@ def antialiasing():
 def rectify():
     """Whether the installed patch rectifies on the GPU (GPSG_RECTIFY=1 at install())."""
     return _RECTIFY
+
+
+def flow_head():
+    """Whether the installed patch runs the disparity head on the fused kernels (GPSG_FLOW_HEAD=1 at install())."""
+    return _FLOW_HEAD

@@ -434,6 +434,47 @@ GPSG_API int gpsg_rectify_flow(int device, void* stream, int H, int W, int Cm, d
                                const float* const* depth, const uint8_t* const* mask, double* const* flow,
                                uint8_t* const* valid);
 
+/* ---- disparity head of both training stages (reference core/raft_stereo_human.py:69-81 and lib/loss.py:8-33) -----------
+ * gpsg_convex_upsample_forward: FlowUpdateModule.upsample_flow.  flow [N,D,H,W] fp32, mask [N,9*f*f,H,W] of `mask_dtype`
+ *   (0 = fp32, 1 = fp16), both contiguous; out [N,D,f*H,f*W] fp32.  With tap k = 3*ky + kx and mask channel
+ *   k*f^2 + i*f + j: w = softmax over k of the 9 logits, computed in fp32 (max-subtracted exp over their sum) and rounded
+ *   to the mask dtype; out[n,d,h*f+i,w*f+j] = sum_{k=0..8} w * f*flow[n,d,h+ky-1,w+kx-1] with fp32 products and sum,
+ *   zero padding (padded taps keep their weight).  f in {2, 4, 8}, D in {1, 2}.
+ * gpsg_convex_upsample_backward: grad_out [N,D,f*H,f*W] fp32 -> grad_mask (mask dtype; the weights are recomputed from
+ *   the mask, dL/dweight is rounded to the mask dtype before the softmax backward) and grad_flow [N,D,H,W] fp32; either may
+ *   be NULL, not both.  workspace: gpsg_convex_upsample_backward_workspace_bytes bytes, 4-byte aligned (the per-pixel tap
+ *   sums, gathered into grad_flow without atomics, so the result is deterministic).
+ * gpsg_sequence_loss_forward: args->pred[0..n_pred) and valid: `numel` fp32 elements each (the [N,1,H,W] tensors); gt:
+ *   `numel` elements of `gt_dtype` (0 = fp32, 1 = fp16: the training cache's flow, widened exactly to fp32);
+ *   stats (device float[6]) = { loss, EPE mean, fraction of EPE < 1, fraction of EPE < 3, 1 if gt is inf at a valid
+ *   pixel else 0, float(valid count) }, with valid = (valid >= 0.5), loss = sum_i weight[i] * mean_valid |pred_i - gt| and
+ *   EPE = sqrt((pred_last - gt)^2) in fp32.  Reductions run in a fixed order: bit-reproducible.  workspace:
+ *   gpsg_sequence_loss_workspace_bytes() bytes, 8-byte aligned.
+ * gpsg_sequence_loss_backward: args->grad[i] (numel fp32 each) = d(grad_loss * loss)/d(pred_i), reading the count from
+ *   the forward's stats; grad_loss is a DEVICE pointer to one float (NULL = 1).  No host synchronisation.
+ * All enqueue on `stream` and do not synchronise. */
+#define GPSG_SEQ_LOSS_MAX_PRED 32
+typedef struct GpsgSeqLossArgs {
+    const float* pred[GPSG_SEQ_LOSS_MAX_PRED];
+    float* grad[GPSG_SEQ_LOSS_MAX_PRED];
+    float weight[GPSG_SEQ_LOSS_MAX_PRED];
+    const void* gt;
+    const float* valid;
+    int64_t numel;
+    int n_pred;
+    int gt_dtype;
+} GpsgSeqLossArgs;
+GPSG_API int gpsg_convex_upsample_forward(int device, void* stream, int mask_dtype, int factor, int N, int D, int H, int W,
+                                          const float* flow, const void* mask, float* out);
+GPSG_API size_t gpsg_convex_upsample_backward_workspace_bytes(int N, int D, int H, int W);
+GPSG_API int gpsg_convex_upsample_backward(int device, void* stream, int mask_dtype, int factor, int N, int D, int H,
+                                           int W, const float* flow, const void* mask, const float* grad_out,
+                                           void* grad_mask, float* grad_flow, void* workspace);
+GPSG_API size_t gpsg_sequence_loss_workspace_bytes(void);
+GPSG_API int gpsg_sequence_loss_forward(int device, void* stream, GpsgSeqLossArgs args, float* stats, void* workspace);
+GPSG_API int gpsg_sequence_loss_backward(int device, void* stream, GpsgSeqLossArgs args, const float* grad_loss,
+                                         const float* stats);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.
