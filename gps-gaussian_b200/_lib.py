@@ -170,6 +170,35 @@ class RectifyPlanes(C.Structure):
                                           "mask_tensor")]
 
 
+MESH_MAX_CAMERAS = 8      # GPSG_MESH_MAX_CAMERAS (include/gpsg.h)
+MESH_MAX_LIGHTS = 16      # GPSG_MESH_MAX_LIGHTS (include/gpsg.h)
+
+
+class Mesh(C.Structure):
+    """GpsgMesh (include/gpsg.h), passed by value: device pointers of the mesh and its texture, NULL where absent."""
+    _fields_ = [("verts", C.c_void_p), ("face_verts", C.c_void_p), ("uvs", C.c_void_p), ("face_uvs", C.c_void_p),
+                ("tex", C.c_void_p), ("num_verts", C.c_int32), ("num_faces", C.c_int32), ("num_uvs", C.c_int32),
+                ("tex_w", C.c_int32), ("tex_h", C.c_int32)]
+
+
+class MeshCamera(C.Structure):
+    """GpsgMeshCamera (include/gpsg.h): res, intrinsics, position, trans^-1 (row-major) and the device outputs."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float),
+                ("cy", C.c_float), ("pos", C.c_float * 3), ("inv_rot", C.c_float * 9), ("img", C.c_void_p),
+                ("zbuf", C.c_void_p), ("mask", C.c_void_p)]
+
+
+class MeshScene(C.Structure):
+    """GpsgMeshScene (include/gpsg.h), passed by value: the cameras of one render and the lights."""
+    _fields_ = [("cameras", MeshCamera * MESH_MAX_CAMERAS), ("light_dir", (C.c_float * 3) * MESH_MAX_LIGHTS),
+                ("light_color", (C.c_float * 3) * MESH_MAX_LIGHTS), ("num_cameras", C.c_int32),
+                ("num_lights", C.c_int32)]
+
+
+lib.gpsg_mesh_render_workspace_bytes.restype = _sz
+lib.gpsg_mesh_render_workspace_bytes.argtypes = [_i, _i64]
+lib.gpsg_mesh_render.restype = _i
+lib.gpsg_mesh_render.argtypes = [_i, _vp, Mesh, MeshScene, _vp, _sz]
 lib.gpsg_rectify_remap.restype = _i
 lib.gpsg_rectify_remap.argtypes = [_i, _vp, C.POINTER(RectifyCamera), _i, _i, _i, _i, _i, _i, C.POINTER(RectifyPlanes)]
 lib.gpsg_rectify_flow.restype = _i
@@ -220,7 +249,7 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_point_splat_workspace_bytes", "gpsg_point_splat", "gpsg_rectify_remap", "gpsg_rectify_flow",
             "gpsg_convex_upsample_forward", "gpsg_convex_upsample_backward_workspace_bytes",
             "gpsg_convex_upsample_backward", "gpsg_sequence_loss_workspace_bytes", "gpsg_sequence_loss_forward",
-            "gpsg_sequence_loss_backward"]
+            "gpsg_sequence_loss_backward", "gpsg_mesh_render_workspace_bytes", "gpsg_mesh_render"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

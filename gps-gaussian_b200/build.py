@@ -5,7 +5,7 @@
 Output: gps-gaussian_b200/lib/libgpsg_sm90.so (git-ignored build product).
 raster_preprocess.cu is compiled with -fmad=false (see its header): the fp32 op order that decides
 radii / tile rectangles must not be FMA-contracted.  rectify.cu likewise: its fp32 / fp64 op order is what makes
-the rectified images and flow bit-identical to OpenCV.
+the rectified images and flow bit-identical to OpenCV.  mesh_render.cu likewise: its fp32 op order is the mesh oracle's.
 """
 import os
 import subprocess
@@ -35,6 +35,7 @@ SOURCES = {
     "point_splat.cu": [],
     "rectify.cu": ["-fmad=false"],
     "flow_head.cu": [],
+    "mesh_render.cu": ["-fmad=false"],
 }
 
 

@@ -914,6 +914,38 @@ int gpsg_point_splat(int device, void* stream_, int B, int N, int res, int64_t r
     return launch_point_splat(B, N, res, rows_per_batch, pts, mask, depth, color, workspace, (cudaStream_t)stream_);
 }
 
+size_t gpsg_mesh_render_workspace_bytes(int num_faces, int64_t max_pixels) {
+    return (num_faces >= 0 && max_pixels >= 1 && max_pixels < (int64_t(1) << 31))
+               ? mesh_render_workspace_bytes(num_faces, max_pixels) : 0;
+}
+
+int gpsg_mesh_render(int device, void* stream_, GpsgMesh mesh, GpsgMeshScene scene, void* workspace,
+                     size_t workspace_bytes) {
+    GPSG_REQUIRE(mesh.num_verts >= 0 && mesh.num_faces >= 0 && mesh.num_uvs >= 0, "mesh_render: negative count");
+    GPSG_REQUIRE(scene.num_cameras >= 1 && scene.num_cameras <= GPSG_MESH_MAX_CAMERAS,
+                 "mesh_render: num_cameras must be in [1, GPSG_MESH_MAX_CAMERAS]");
+    GPSG_REQUIRE(scene.num_lights >= 0 && scene.num_lights <= GPSG_MESH_MAX_LIGHTS,
+                 "mesh_render: num_lights must be in [0, GPSG_MESH_MAX_LIGHTS]");
+    GPSG_REQUIRE(!mesh.uvs == !mesh.face_uvs, "mesh_render: uvs and face_uvs go together");
+    GPSG_REQUIRE(!mesh.tex || (mesh.tex_w >= 1 && mesh.tex_h >= 1), "mesh_render: texture sizes must be >= 1");
+    GPSG_REQUIRE(mesh.num_faces == 0 || (mesh.face_verts && (mesh.num_verts == 0 || mesh.verts)), "NULL pointer");
+    int64_t max_pixels = 0;
+    for (int c = 0; c < scene.num_cameras; ++c) {
+        const GpsgMeshCamera& cam = scene.cameras[c];
+        GPSG_REQUIRE(cam.width >= 1 && cam.height >= 1, "mesh_render: camera size must be >= 1");
+        const int64_t px = (int64_t)cam.width * cam.height;
+        GPSG_REQUIRE(px < (int64_t(1) << 31), "mesh_render: a camera must have < 2^31 pixels");
+        GPSG_REQUIRE(cam.img && cam.zbuf && cam.mask, "NULL pointer");
+        max_pixels = px > max_pixels ? px : max_pixels;
+    }
+    GPSG_REQUIRE(workspace, "NULL pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 256 == 0, "mesh_render: workspace must be 256-byte aligned");
+    GPSG_REQUIRE(workspace_bytes >= mesh_render_workspace_bytes(mesh.num_faces, max_pixels),
+                 "mesh_render: workspace smaller than gpsg_mesh_render_workspace_bytes");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_mesh_render(mesh, scene, workspace, (cudaStream_t)stream_);
+}
+
 int gpsg_rectify_remap(int device, void* stream_, const GpsgRectifyCamera* cams, int Hin, int Win, int C, int Cm, int H,
                        int W, const GpsgRectifyPlanes* planes) {
     GPSG_REQUIRE(cams && planes, "rectify_remap: NULL cams / planes");

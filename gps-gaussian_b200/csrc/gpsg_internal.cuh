@@ -251,6 +251,9 @@ int launch_rectify_flow(int H, int W, int Cm, double Tf_x, double cx0, double cx
 size_t point_splat_workspace_bytes(int B, int res);
 int launch_point_splat(int B, int N, int res, int64_t rows, const float* pts, const float* mask, float* depth, float* color,
                        void* workspace, cudaStream_t stream);
+// mesh_render.cu (compiled with -fmad=false: the fp32 op order is the oracle's)
+size_t mesh_render_workspace_bytes(int num_faces, int64_t max_pixels);
+int launch_mesh_render(const GpsgMesh& mesh, const GpsgMeshScene& scene, void* workspace, cudaStream_t stream);
 // flow_head.cu (dtype: 0 = fp32 mask, 1 = fp16 mask)
 int launch_convex_upsample_fwd(int dtype, int f, int N, int D, int H, int W, const float* flow, const void* mask, float* out,
                                cudaStream_t stream);

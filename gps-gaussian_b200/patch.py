@@ -35,6 +35,10 @@ value leaves `lib.human_loader` alone: it is then not even hooked.
 Inputs the kernels do not cover (CPU tensors, other dtypes or factors) reach the reference's own function.  The results
 differ from the op chain's by fp32 re-association and by where fp16 rounding falls in the backward, which is why the
 switch is opt-in.  Unset or any other value hooks neither.
+
+`taichi_three` and its submodules always resolve to the stand-in in dropin/taichi_three (the dataset renderer on
+csrc/mesh_render.cu).  `python prepare_data/render_data.py` puts prepare_data/ first on sys.path, where the reference's
+own package, which cannot import without Taichi, would shadow anything on PYTHONPATH.
 """
 import importlib.abc
 import importlib.machinery
@@ -171,8 +175,23 @@ class _PatchingLoader(importlib.abc.Loader):
         self._hook(module)
 
 
+_STANDINS = ("taichi_three",)    # packages always taken from dropin/, whatever shadows them on sys.path
+_DROPIN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "dropin")
+
+
+def _standin_spec(name):
+    top = name.split(".", 1)[0]
+    if top not in _STANDINS:
+        return None
+    where = [_DROPIN] if name == top else [os.path.join(_DROPIN, *name.split(".")[:-1])]
+    return importlib.machinery.PathFinder.find_spec(name, where)
+
+
 class _Finder(importlib.abc.MetaPathFinder):
     def find_spec(self, name, path=None, target=None):
+        spec = _standin_spec(name)
+        if spec is not None:
+            return spec
         hook = _targets().get(name)
         if hook is None:
             return None

@@ -393,6 +393,60 @@ GPSG_API size_t gpsg_point_splat_workspace_bytes(int B, int res);
 GPSG_API int gpsg_point_splat(int device, void* stream, int B, int N, int res, int64_t rows_per_batch, const float* pts,
                               const float* mask, float* depth, float* color, void* workspace);
 
+/* ---- textured triangle mesh renderer of the dataset script (reference prepare_data/taichi_three) ---------------------
+ * gpsg_mesh_render: one `Scene.render()` of the reference: every camera of `scene` is cleared and the mesh drawn into it,
+ * in one launch chain on `stream`, without host synchronisation.  The result is the serial reading of the reference's
+ * `render_triangle` (faces in index order): per pixel the face with the largest zindex = 1 / (screen-affine depth) wins,
+ * the highest face index among equal zindex; the fp32 formulation is written down in csrc/mesh_render.cu.
+ *   mesh (HOST struct of device pointers, by value):
+ *     verts [num_verts,3] fp32; face_verts [num_faces,3] int32 (vertex indices);
+ *     uvs [num_uvs,2] fp32 and face_uvs [num_faces,3] int32, or both NULL (every corner samples uv = (0, 0));
+ *     tex [tex_w,tex_h,3] fp32 (the reference's texture field: tex[i,j] at uv*(tex_w, tex_h) = (i, j)), or NULL (the
+ *     sample is 1).  A face with an index outside its array draws nothing.
+ *   scene (HOST struct, by value): cameras[0..num_cameras), lights[0..num_lights).  Per camera: res = (width, height)
+ *     (the reference's field shape (res[0], res[1])), fx, fy, cx, cy, pos, inv_rot = trans^-1 (row-major fp32; the caller
+ *     inverts `trans` in fp64), and device outputs img [height,width,3], zbuf [height,width], mask [height,width,3] fp32
+ *     (the reference's fields transposed to [y, x]; every pixel is written).  Per light: light_dir = the unit vector
+ *     towards the light (-normalize(dir)), light_color.  A NaN img value is written as the canonical NaN 0x7fffffff.
+ *   workspace: gpsg_mesh_render_workspace_bytes(num_faces, max over cameras of width*height) bytes, 256-byte aligned.
+ * Refused (GPSG_E_INVALID): negative counts, num_cameras outside [1, GPSG_MESH_MAX_CAMERAS], num_lights outside
+ * [0, GPSG_MESH_MAX_LIGHTS], a camera size < 1 or with >= 2^31 pixels, uvs without face_uvs (or the reverse), texture
+ * sizes < 1, NULL pointers where there is data, a workspace smaller than the query or misaligned. */
+#define GPSG_MESH_MAX_CAMERAS 8
+#define GPSG_MESH_MAX_LIGHTS 16
+typedef struct GpsgMesh {
+    const float* verts;
+    const int32_t* face_verts;
+    const float* uvs;
+    const int32_t* face_uvs;
+    const float* tex;
+    int32_t num_verts;
+    int32_t num_faces;
+    int32_t num_uvs;
+    int32_t tex_w;
+    int32_t tex_h;
+} GpsgMesh;
+typedef struct GpsgMeshCamera {
+    int32_t width;
+    int32_t height;
+    float fx, fy, cx, cy;
+    float pos[3];
+    float inv_rot[9];
+    float* img;
+    float* zbuf;
+    float* mask;
+} GpsgMeshCamera;
+typedef struct GpsgMeshScene {
+    GpsgMeshCamera cameras[GPSG_MESH_MAX_CAMERAS];
+    float light_dir[GPSG_MESH_MAX_LIGHTS][3];
+    float light_color[GPSG_MESH_MAX_LIGHTS][3];
+    int32_t num_cameras;
+    int32_t num_lights;
+} GpsgMeshScene;
+GPSG_API size_t gpsg_mesh_render_workspace_bytes(int num_faces, int64_t max_pixels);
+GPSG_API int gpsg_mesh_render(int device, void* stream, GpsgMesh mesh, GpsgMeshScene scene, void* workspace,
+                              size_t workspace_bytes);
+
 /* ---- stereo rectification of the real-data loader (reference lib/human_loader.py:245-366) ----------------------------
  * gpsg_rectify_remap: cv2.initUndistortRectifyMap(K, 0, R, P, (W, H), CV_32FC1) + cv2.remap(INTER_LINEAR,
  *   BORDER_CONSTANT 0) of both views of a pair in one launch, bit-identical to OpenCV 4.x (DESIGN.md §2).  cams[2] are
