@@ -36,6 +36,7 @@ SOURCES = {
     "rectify.cu": ["-fmad=false"],
     "flow_head.cu": [],
     "mesh_render.cu": ["-fmad=false"],
+    "jpeg_decode.cu": [],
 }
 
 

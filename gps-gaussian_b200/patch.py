@@ -26,6 +26,11 @@ novel-view scripts train and render anti-aliased; unset or any other value keeps
 Inside a DataLoader worker (forked, no CUDA) or without CUDA both call the reference's own method.  Unset or any other
 value leaves `lib.human_loader` alone: it is then not even hooked.
 
+`GPSG_DECODE=1`, read once by `install()` and effective together with `GPSG_RECTIFY=1`, makes the rebound
+`get_test_item` decode the two source JPEGs on the GPU (gps_gaussian_b200.jpeg, csrc/jpeg_decode.cu: Pillow's bytes) and
+hand the device images to the rectification kernels without a host round trip.  The masks stay PNG on Pillow.  Unset or
+any other value decodes with the reference's `read_img`, as before.
+
 `GPSG_FLOW_HEAD=1`, read once by `install()`, also hooks the disparity head of both training stages
 (gps_gaussian_b200.flow_head, csrc/flow_head.cu):
 
@@ -51,6 +56,7 @@ _ORIG_METHODS = {}    # (class, attribute) -> original function
 _ANTIALIAS = False    # GPSG_ANTIALIAS=1 at install()
 _RECTIFY = False      # GPSG_RECTIFY=1 at install()
 _FLOW_HEAD = False    # GPSG_FLOW_HEAD=1 at install()
+_DECODE = False       # GPSG_DECODE=1 at install()
 
 
 def _set(mod, attr, new):
@@ -95,6 +101,16 @@ def _rectified_stereo_data(orig, mod):
     return get_rectified_stereo_data
 
 
+def _views_cuda(self, mod, sample_name, source_ids):
+    """load_single_view(sample_name, sid, hr_img=False, require_mask=True, require_pts=False) of both views, with the
+    two images decoded on the GPU in one call (lib/human_loader.py:190-211)."""
+    import numpy as np
+    from gps_gaussian_b200 import jpeg
+    imgs = jpeg.read_img_cuda([self.img_path % (sample_name, sid) for sid in source_ids])
+    return [(img, mod.read_img(self.mask_path % (sample_name, sid)), np.load(self.intr_path % (sample_name, sid)),
+             np.load(self.extr_path % (sample_name, sid)), None) for img, sid in zip(imgs, source_ids)]
+
+
 def _test_item(orig, mod):
     """get_test_item with the rectified pair made on the GPU: load both views, then stereo_item_cuda, then the original
     intrinsics / extrinsics and the novel-view size, as the reference's method (lib/human_loader.py:390-419)."""
@@ -106,8 +122,11 @@ def _test_item(orig, mod):
         sample_name = self.sample_list[index % len(self.sample_list)]
         if self.use_processed_data:
             logging.error('test data loader not support processed data')
-        views = [self.load_single_view(sample_name, sid, hr_img=False, require_mask=True, require_pts=False)
-                 for sid in source_id[:2]]
+        if _DECODE:
+            views = _views_cuda(self, mod, sample_name, source_id[:2])
+        else:
+            views = [self.load_single_view(sample_name, sid, hr_img=False, require_mask=True, require_pts=False)
+                     for sid in source_id[:2]]
         item = rectify.stereo_item_cuda(views[0], views[1], self.opt.src_res, sample_name, pts2depth=mod.pts2depth)
         for key, which in (('intr_ori', 2), ('extr_ori', 3)):
             item['lmain'][key] = torch.FloatTensor(views[0][which])
@@ -209,12 +228,13 @@ _FINDER = _Finder()
 
 
 def install():
-    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY and
-    GPSG_FLOW_HEAD here, once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD
+    """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
+    GPSG_FLOW_HEAD and GPSG_DECODE here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
+    _DECODE = os.environ.get("GPSG_DECODE", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -250,6 +270,11 @@ def antialiasing():
 def rectify():
     """Whether the installed patch rectifies on the GPU (GPSG_RECTIFY=1 at install())."""
     return _RECTIFY
+
+
+def decode():
+    """Whether the rebound get_test_item decodes the source JPEGs on the GPU (GPSG_DECODE=1 at install())."""
+    return _DECODE
 
 
 def flow_head():

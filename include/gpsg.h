@@ -488,6 +488,52 @@ GPSG_API int gpsg_rectify_flow(int device, void* stream, int H, int W, int Cm, d
                                const float* const* depth, const uint8_t* const* mask, double* const* flow,
                                uint8_t* const* valid);
 
+/* ---- baseline JPEG decoding (the loader's source frames; rules in DESIGN.md §2 "JPEG decoding") ----------------------
+ * gpsg_jpeg_parse: reads the markers of one JPEG file (host memory, `size` bytes) into `info`.  Returns 0 when the image
+ *   is decoded natively, else a refusal code GPSG_JPEG_E_* (> 0; `info` is then partial), or GPSG_E_INVALID for NULL
+ *   pointers.  Every length field is checked against `size`; nothing past it is read.  Decoded natively: SOF0 / SOF1,
+ *   8-bit, one scan holding every component in frame order, Huffman coded; one component (Pillow mode L), or three
+ *   YCbCr components with chroma 1x1 and luma 1x1, 2x1 or 2x2.
+ * gpsg_jpeg_decode_workspace_bytes: the workspace of one gpsg_jpeg_decode over these infos (0 when they are refused).
+ * gpsg_jpeg_decode: decodes n <= GPSG_JPEG_MAX_BATCH parsed images in one launch chain on `stream`.  data[i]: DEVICE
+ *   pointer to the whole file of image i (the bytes gpsg_jpeg_parse read); out[i]: DEVICE [H,W] (one component) or
+ *   [H,W,3] uint8, what Pillow's np.array(Image.open(f)) holds; status: DEVICE uint32[n], set to 0 and then to the
+ *   GPSG_JPEG_ST_* bits of whatever made image i undecodable (its `out` is then unspecified).  The caller reads the
+ *   status words after the stream reaches this call.  workspace: gpsg_jpeg_decode_workspace_bytes bytes, 256-byte
+ *   aligned.  Refused: bad n, NULL pointers, infos that gpsg_jpeg_parse would refuse, a batch whose scans reach
+ *   GPSG_JPEG_MAX_SCAN_BYTES (gpsg_jpeg_decode_workspace_bytes then returns 0), a short workspace. */
+#define GPSG_JPEG_MAX_BATCH 64
+#define GPSG_JPEG_MAX_SCAN_BYTES (1 << 28)   /* entropy-coded bytes of one gpsg_jpeg_decode, summed over its images */
+#define GPSG_JPEG_E_TRUNCATED 1     /* a length field, the scan or the EOI marker lies past the end of the buffer */
+#define GPSG_JPEG_E_MALFORMED 2     /* a marker or table that T.81 does not allow, or a table the scan needs is missing */
+#define GPSG_JPEG_E_PROGRESSIVE 3   /* SOF2 */
+#define GPSG_JPEG_E_ARITHMETIC 4    /* SOF9 / SOF10 / DAC */
+#define GPSG_JPEG_E_LOSSLESS 5      /* SOF3 / SOF7 / SOF11 / SOF15 */
+#define GPSG_JPEG_E_HIERARCHICAL 6  /* SOF5 / SOF6 / SOF13 / SOF14 */
+#define GPSG_JPEG_E_PRECISION 7     /* sample precision other than 8 bits */
+#define GPSG_JPEG_E_COLORSPACE 8    /* 2 or 4 components (CMYK), or RGB (Adobe transform 0, or R/G/B component ids) */
+#define GPSG_JPEG_E_SAMPLING 9      /* sampling factors other than the three layouts above */
+#define GPSG_JPEG_E_MULTISCAN 10    /* more than one scan, or a scan without every component in frame order */
+#define GPSG_JPEG_E_DNL 11          /* height 0 / a DNL marker */
+#define GPSG_JPEG_ST_BAD_CODE 1u    /* a Huffman code no table holds */
+#define GPSG_JPEG_ST_OVERRUN 2u     /* a code or its bits run past the end of the restart segment */
+#define GPSG_JPEG_ST_MCU_COUNT 4u   /* a restart segment (or the image) holds the wrong number of MCUs, or bad padding */
+#define GPSG_JPEG_ST_RST 8u         /* an RSTn marker out of sequence */
+#define GPSG_JPEG_ST_MARKER 16u     /* a marker other than RSTn or a stuffed 0xFF inside the scan */
+#define GPSG_JPEG_ST_COEF 32u       /* a coefficient past index 63, or a magnitude category beyond 8-bit baseline */
+typedef struct GpsgJpegInfo {
+    int32_t width, height, num_components, restart_interval;
+    int32_t h_samp[3], v_samp[3], quant_id[3], dc_id[3], ac_id[3];
+    uint16_t quant[4][64];                      /* zigzag order */
+    uint8_t dc_bits[4][16], ac_bits[4][16];     /* codes of length 1..16 */
+    uint8_t dc_vals[4][256], ac_vals[4][256];
+    int64_t ecs_offset, ecs_length;             /* the entropy-coded segment (RSTn markers included) in the file */
+} GpsgJpegInfo;
+GPSG_API int gpsg_jpeg_parse(const uint8_t* data, size_t size, GpsgJpegInfo* info);
+GPSG_API size_t gpsg_jpeg_decode_workspace_bytes(int n, const GpsgJpegInfo* infos);
+GPSG_API int gpsg_jpeg_decode(int device, void* stream, int n, const GpsgJpegInfo* infos, const uint8_t* const* data,
+                              uint8_t* const* out, uint32_t* status, void* workspace, size_t workspace_bytes);
+
 /* ---- disparity head of both training stages (reference core/raft_stereo_human.py:69-81 and lib/loss.py:8-33) -----------
  * gpsg_convex_upsample_forward: FlowUpdateModule.upsample_flow.  flow [N,D,H,W] fp32, mask [N,9*f*f,H,W] of `mask_dtype`
  *   (0 = fp32, 1 = fp16), both contiguous; out [N,D,f*H,f*W] fp32.  With tap k = 3*ky + kx and mask channel
