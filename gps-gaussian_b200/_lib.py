@@ -250,7 +250,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_convex_upsample_forward", "gpsg_convex_upsample_backward_workspace_bytes",
             "gpsg_convex_upsample_backward", "gpsg_sequence_loss_workspace_bytes", "gpsg_sequence_loss_forward",
             "gpsg_sequence_loss_backward", "gpsg_mesh_render_workspace_bytes", "gpsg_mesh_render", "gpsg_jpeg_parse",
-            "gpsg_jpeg_decode_workspace_bytes", "gpsg_jpeg_decode"]
+            "gpsg_jpeg_decode_workspace_bytes", "gpsg_jpeg_decode", "gpsg_jpeg_encode_max_bytes",
+            "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

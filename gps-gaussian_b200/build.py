@@ -37,6 +37,7 @@ SOURCES = {
     "flow_head.cu": [],
     "mesh_render.cu": ["-fmad=false"],
     "jpeg_decode.cu": [],
+    "jpeg_encode.cu": [],
 }
 
 

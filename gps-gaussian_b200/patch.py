@@ -31,6 +31,14 @@ value leaves `lib.human_loader` alone: it is then not even hooked.
 hand the device images to the rectification kernels without a host round trip.  The masks stay PNG on Pillow.  Unset or
 any other value decodes with the reference's `read_img`, as before.
 
+`GPSG_ENCODE=1`, read once by `install()`, also hooks `cv2` and rebinds `cv2.imwrite` to the GPU JPEG encoder
+(gps_gaussian_b200.jpeg, csrc/jpeg_encode.cu: cv2's bytes), which covers every JPEG the entry scripts write.  A call goes
+to the GPU when the extension is .jpg / .jpeg / .jpe (any case), the params are empty or only IMWRITE_JPEG_QUALITY (0..100)
+and IMWRITE_JPEG_SAMPLING_FACTOR (4:4:4, 4:2:2, 4:2:0), the array is uint8 [H,W], [H,W,1] or [H,W,3] of at least
+_MIN_NATIVE_PIXELS pixels (any strides), its directory exists, and it runs in the main process with CUDA.  Every other
+call reaches cv2's own function with the same arguments.  Unset or any other value leaves `cv2` alone: it is then not
+even hooked.
+
 `GPSG_FLOW_HEAD=1`, read once by `install()`, also hooks the disparity head of both training stages
 (gps_gaussian_b200.flow_head, csrc/flow_head.cu):
 
@@ -57,6 +65,7 @@ _ANTIALIAS = False    # GPSG_ANTIALIAS=1 at install()
 _RECTIFY = False      # GPSG_RECTIFY=1 at install()
 _FLOW_HEAD = False    # GPSG_FLOW_HEAD=1 at install()
 _DECODE = False       # GPSG_DECODE=1 at install()
+_ENCODE = False       # GPSG_ENCODE=1 at install()
 
 
 def _set(mod, attr, new):
@@ -163,6 +172,99 @@ def _patch_loss(mod):
         _set(user, "sequence_loss", flow_head.sequence_loss)
 
 
+_JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
+_JPEG_SAMPLING = {0x111111: "444", 0x211111: "422", 0x221111: "420"}   # cv2.IMWRITE_JPEG_SAMPLING_FACTOR_444/422/420
+_IMWRITE_JPEG_QUALITY, _IMWRITE_JPEG_SAMPLING_FACTOR = 1, 7
+# Below this many pixels cv2 on the host is faster than the upload, the launch chain and the download: on an H100 at 700 W,
+# q95 4:2:0, the GPU route took 1.85 ms against cv2's 1.38 ms at 256^2 and 4.34 ms against 4.98 ms at 512^2 (DESIGN.md §5).
+_MIN_NATIVE_PIXELS = 512 * 512
+
+
+def _jpeg_route(args, kwargs):
+    """(filename, array, quality, subsampling) when cv2.imwrite(*args, **kwargs) is encoded on the GPU, else None."""
+    import numpy as np
+    names = ("filename", "img", "params")
+    if len(args) > 3 or any(k not in names[len(args):] for k in kwargs):
+        return None
+    bound = dict(zip(names, args), **kwargs)
+    filename, img, params = bound.get("filename"), bound.get("img"), bound.get("params")
+    if not isinstance(filename, str) or os.path.splitext(filename)[1].lower() not in _JPEG_EXTS:
+        return None
+    if type(img) is not np.ndarray or img.dtype != np.uint8:
+        return None
+    if not (img.ndim == 2 or (img.ndim == 3 and img.shape[2] in (1, 3))):
+        return None
+    H, W = img.shape[:2]
+    if not (1 <= H <= 65500 and 1 <= W <= 65500) or H * W < _MIN_NATIVE_PIXELS:
+        return None
+    quality, subsampling = 95, "420"                   # cv2's defaults
+    if params is not None:
+        if not isinstance(params, (list, tuple)) or len(params) % 2:
+            return None
+        for key, val in zip(params[0::2], params[1::2]):
+            if not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in (key, val)):
+                return None
+            if key == _IMWRITE_JPEG_QUALITY and 0 <= val <= 100:
+                quality = max(int(val), 1)             # quality 0 is libjpeg's 1
+            elif key == _IMWRITE_JPEG_SAMPLING_FACTOR and int(val) in _JPEG_SAMPLING:
+                subsampling = _JPEG_SAMPLING[int(val)]
+            else:
+                return None
+    if not os.path.isdir(os.path.dirname(os.path.abspath(filename))) or not _in_main_process() or not _on_device():
+        return None
+    from gps_gaussian_b200 import jpeg
+    if not jpeg.fits_one_call(H, W, 1 if img.ndim == 2 or img.shape[2] == 1 else 3, subsampling):
+        return None                                    # too large for one launch chain: cv2 writes it
+    return filename, img, quality, subsampling
+
+
+def _in_main_process():
+    """cv2.imwrite in a child process (a DataLoader worker, a multiprocessing.Pool of writers) stays on cv2: a forked
+    child of a process that has used CUDA cannot use it again."""
+    import multiprocessing
+    return multiprocessing.parent_process() is None
+
+
+def _make_imwrite(orig):
+    def imwrite(*args, **kwargs):
+        from gps_gaussian_b200 import jpeg
+        route = _jpeg_route(args, kwargs)
+        if route is not None:
+            filename, img, quality, subsampling = route
+            import torch
+            try:
+                data = jpeg.encode_host(img, quality, subsampling, order="bgr")
+                with open(filename, "wb") as f:
+                    f.write(data)
+                return True
+            except (OSError, torch.cuda.OutOfMemoryError):
+                pass                                   # an unwritable path, or no device memory left: cv2 decides
+        jpeg._ENC_COUNTS["fallback"] += 1
+        return orig(*args, **kwargs)
+    imwrite.__doc__ = orig.__doc__
+    imwrite._gpsg_original = orig
+    return imwrite
+
+
+_CV2_MODULES = []     # module objects whose imwrite the patch rebound (see _patch_cv2)
+
+
+def _patch_cv2(mod):
+    """cv2.imwrite -> the GPU JPEG route.
+
+    Imported after install(), cv2's package (cv2/__init__.py) imports its native extension under the same name "cv2",
+    so this hook fires twice: first on the extension module, whose imwrite it wraps, then on the package, which by then
+    has copied the wrapper from the extension.  Both module objects are kept in _CV2_MODULES and uninstall() restores
+    imwrite on each of them, not only on whichever one sys.modules["cv2"] holds."""
+    cur = getattr(mod, "imwrite", None)
+    if cur is None:
+        return
+    if not hasattr(cur, "_gpsg_original"):
+        _set(mod, "imwrite", _make_imwrite(cur))
+    if not any(m is mod for m in _CV2_MODULES):
+        _CV2_MODULES.append(mod)
+
+
 # Modules whose `from <module> import <attr>` made after install() copies the rebound object without _set seeing it;
 # uninstall() puts the original back there too.
 _COPIES = {("lib.loss", "sequence_loss"): ("lib.network",)}
@@ -176,10 +278,12 @@ def original(mod, attr):
 _TARGETS = {"core.corr": _patch_corr, "lib.GaussianRender": _patch_render}
 _RECTIFY_TARGETS = {"lib.human_loader": _patch_loader}
 _FLOW_HEAD_TARGETS = {"core.raft_stereo_human": _patch_upsample, "lib.loss": _patch_loss}
+_ENCODE_TARGETS = {"cv2": _patch_cv2}
 
 
 def _targets():
-    return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {})}
+    return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {}),
+            **(_ENCODE_TARGETS if _ENCODE else {})}
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -229,12 +333,13 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD and GPSG_DECODE here, once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE
+    GPSG_FLOW_HEAD, GPSG_DECODE and GPSG_ENCODE here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
     _DECODE = os.environ.get("GPSG_DECODE", "") == "1"
+    _ENCODE = os.environ.get("GPSG_ENCODE", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -256,6 +361,11 @@ def uninstall():
     for (cls, attr), orig in list(_ORIG_METHODS.items()):
         setattr(cls, attr, orig)
     _ORIG_METHODS.clear()
+    for mod in _CV2_MODULES:
+        wrapper = getattr(mod, "imwrite", None)
+        if hasattr(wrapper, "_gpsg_original"):
+            mod.imwrite = wrapper._gpsg_original
+    _CV2_MODULES.clear()
 
 
 def active():
@@ -275,6 +385,11 @@ def rectify():
 def decode():
     """Whether the rebound get_test_item decodes the source JPEGs on the GPU (GPSG_DECODE=1 at install())."""
     return _DECODE
+
+
+def encode():
+    """Whether cv2.imwrite writes JPEGs through the GPU encoder (GPSG_ENCODE=1 at install())."""
+    return _ENCODE
 
 
 def flow_head():

@@ -534,6 +534,31 @@ GPSG_API size_t gpsg_jpeg_decode_workspace_bytes(int n, const GpsgJpegInfo* info
 GPSG_API int gpsg_jpeg_decode(int device, void* stream, int n, const GpsgJpegInfo* infos, const uint8_t* const* data,
                               uint8_t* const* out, uint32_t* status, void* workspace, size_t workspace_bytes);
 
+/* ---- baseline JPEG encoding (the output JPEGs; rules in DESIGN.md §2 "JPEG encoding") ---------------------------------
+ * The file cv2.imencode('.jpg') and Pillow's save('JPEG') write with libjpeg-turbo's defaults at `quality`: Annex K
+ * tables, islow FDCT, no Huffman optimisation, no restart markers, one interleaved scan, JFIF APP0.
+ * GpsgJpegEncodeDesc: width, height in 1..65500; channels 1 (grayscale; `sampling` is then ignored but must be valid) or
+ *   3 (interleaved, channel order GPSG_JPEG_ORDER_RGB or _BGR); pitch: bytes between rows, >= width * channels;
+ *   quality 1..100; sampling 444, 422 or 420 (4:4:4, 4:2:2, 4:2:0 chroma).
+ * gpsg_jpeg_encode_max_bytes: an upper bound on the file of one image (0 for a refused descriptor).
+ * gpsg_jpeg_encode_workspace_bytes: the workspace of one gpsg_jpeg_encode over these descriptors (0 when refused, also
+ *   for a batch too large for one call: 2^31 blocks or 2^30 32-bit words of 1664 bits per block).
+ * gpsg_jpeg_encode: encodes n <= GPSG_JPEG_MAX_BATCH images in one launch chain on `stream`.  src[i]: DEVICE rows of
+ *   image i; out[i]: DEVICE buffer of gpsg_jpeg_encode_max_bytes(descs + i) bytes, of which the first out_sizes[i]
+ *   (DEVICE int64[n]) hold the complete file; nothing past them is written.  The caller reads out_sizes after the stream
+ *   reaches this call.  workspace: gpsg_jpeg_encode_workspace_bytes bytes, 256-byte aligned.  Refused before any launch:
+ *   bad n, NULL pointers, a refused descriptor, a short or misaligned workspace. */
+#define GPSG_JPEG_ORDER_RGB 0
+#define GPSG_JPEG_ORDER_BGR 1
+typedef struct GpsgJpegEncodeDesc {
+    int32_t width, height, channels, order, quality, sampling;
+    int64_t pitch;
+} GpsgJpegEncodeDesc;
+GPSG_API size_t gpsg_jpeg_encode_max_bytes(const GpsgJpegEncodeDesc* desc);
+GPSG_API size_t gpsg_jpeg_encode_workspace_bytes(int n, const GpsgJpegEncodeDesc* descs);
+GPSG_API int gpsg_jpeg_encode(int device, void* stream, int n, const GpsgJpegEncodeDesc* descs, const uint8_t* const* src,
+                              uint8_t* const* out, int64_t* out_sizes, void* workspace, size_t workspace_bytes);
+
 /* ---- disparity head of both training stages (reference core/raft_stereo_human.py:69-81 and lib/loss.py:8-33) -----------
  * gpsg_convex_upsample_forward: FlowUpdateModule.upsample_flow.  flow [N,D,H,W] fp32, mask [N,9*f*f,H,W] of `mask_dtype`
  *   (0 = fp32, 1 = fp16), both contiguous; out [N,D,f*H,f*W] fp32.  With tap k = 3*ky + kx and mask channel
