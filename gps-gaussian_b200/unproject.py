@@ -16,9 +16,19 @@ class _Unproject(torch.autograd.Function):
         dev = flow_pred.device
         f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
         flow, m, K, E, Kr, tf = f32(flow_pred), f32(mask), f32(intr), f32(extr), f32(ref_intr), f32(tf_x).reshape(-1)
-        B, _, S, S2 = flow.shape
-        if S != S2 or m.shape[0] != B or m.shape[-1] != S or E.shape[-1] != 4 or E.shape[-2] < 3:
-            raise RuntimeError("unproject (gpsg): unexpected input shapes")
+        # the kernels index every input by batch item and pixel without bounds: refuse any shape they would read past
+        if flow.dim() != 4 or flow.shape[1] != 1 or flow.shape[2] != flow.shape[3]:
+            raise RuntimeError(f"unproject (gpsg): flow_pred must be [B,1,S,S], got {tuple(flow.shape)}")
+        B, _, S, _ = flow.shape
+        if m.dim() != 4 or m.shape[0] != B or m.shape[1] < 1 or m.shape[2] != S or m.shape[3] != S:
+            raise RuntimeError(f"unproject (gpsg): mask must be [{B},C,{S},{S}], got {tuple(m.shape)}")
+        for name, t in (("intr", K), ("ref_intr", Kr)):
+            if tuple(t.shape) != (B, 3, 3):
+                raise RuntimeError(f"unproject (gpsg): {name} must be [{B},3,3], got {tuple(t.shape)}")
+        if E.dim() != 3 or E.shape[0] != B or E.shape[1] < 3 or E.shape[2] != 4:
+            raise RuntimeError(f"unproject (gpsg): extr must be [{B},>=3,4], got {tuple(E.shape)}")
+        if tf.numel() != B:
+            raise RuntimeError(f"unproject (gpsg): Tf_x must have {B} elements, got {tf.numel()}")
         depth = torch.empty((B, 1, S, S), dtype=torch.float32, device=dev)
         xyz = torch.empty((B, S * S, 3), dtype=torch.float32, device=dev)
         valid = torch.empty((B, S * S), dtype=torch.bool, device=dev)
