@@ -413,7 +413,9 @@ __device__ __forceinline__ unsigned long long block_sum_u(unsigned long long v, 
 
 // stats[0] = loss = ((0 + w_0*m_0) + w_1*m_1) + ..., m_i = float(sum_i) * (1/float(count)) (torch's mean: sum times
 // the fp32 reciprocal of the count); stats[1..3] = EPE mean, fraction < 1, fraction < 3 of the last prediction;
-// stats[4] = 1 when flow_gt is inf at a valid pixel; stats[5] = float(count), read by the backward.
+// stats[4] = 1 when flow_gt is inf at a valid pixel; stats[5] = the reciprocal of the exact count rounded once to fp32,
+// read by the backward.  torch's mean backward divides by the integer count and takes that reciprocal; it equals
+// 1/float(count) up to 2^24 valid pixels, where float(count) is exact, and not above (a stage-1 batch of 8 at 1024^2).
 __global__ void __launch_bounds__(kLossThreads) sequence_loss_fwd_kernel(const __grid_constant__ GpsgSeqLossArgs a,
                                                                         double* __restrict__ pd,
                                                                         unsigned long long* __restrict__ pu,
@@ -494,19 +496,19 @@ __global__ void __launch_bounds__(kLossThreads) sequence_loss_fwd_kernel(const _
         stats[2] = __fmul_rn((float)totu[1], inv);
         stats[3] = __fmul_rn((float)totu[2], inv);
         stats[4] = totu[3] ? 1.f : 0.f;
-        stats[5] = cf;
+        stats[5] = (float)(1.0 / (double)totu[0]);
         *ticket = 0;                                                // re-arm for the next call on this workspace
     }
 }
 
-// grad_i = (valid ? 0 + (g*w_i) * (1/count) : 0) * sign(p_i - gt): the op order of torch's mean -> boolean-index -> abs
-// backward (the mean's division by the count runs as a multiplication by its fp32 reciprocal, the index backward
-// accumulates into zeros), so the gradient is bit-identical; sign(0) = sign(NaN) = 0.
+// grad_i = (valid ? 0 + (g*w_i) * (1/count) : 0) * sign(p_i - gt) with 1/count = stats[5]: the op order of torch's
+// mean -> boolean-index -> abs backward (the mean's division by the count runs as a multiplication by its fp32
+// reciprocal, the index backward accumulates into zeros), so the gradient is bit-identical; sign(0) = sign(NaN) = 0.
 __global__ void __launch_bounds__(256) sequence_loss_bwd_kernel(const __grid_constant__ GpsgSeqLossArgs a,
                                                                const float* __restrict__ grad_loss,
                                                                const float* __restrict__ stats) {
     const float g = grad_loss ? __ldg(grad_loss) : 1.f;
-    const float inv = __fdiv_rn(1.f, __ldg(stats + 5));
+    const float inv = __ldg(stats + 5);
     for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < a.numel; e += (int64_t)gridDim.x * blockDim.x) {
         const bool v = __ldg(a.valid + e) >= 0.5f;
         const float gt = load_gt(a, e);

@@ -572,10 +572,10 @@ GPSG_API int gpsg_jpeg_encode(int device, void* stream, int n, const GpsgJpegEnc
  * gpsg_sequence_loss_forward: args->pred[0..n_pred) and valid: `numel` fp32 elements each (the [N,1,H,W] tensors); gt:
  *   `numel` elements of `gt_dtype` (0 = fp32, 1 = fp16: the training cache's flow, widened exactly to fp32);
  *   stats (device float[6]) = { loss, EPE mean, fraction of EPE < 1, fraction of EPE < 3, 1 if gt is inf at a valid
- *   pixel else 0, float(valid count) }, with valid = (valid >= 0.5), loss = sum_i weight[i] * mean_valid |pred_i - gt| and
- *   EPE = sqrt((pred_last - gt)^2) in fp32.  Reductions run in a fixed order: bit-reproducible.  workspace:
+ *   pixel else 0, 1 / valid count (in fp64, rounded once to fp32) }, with valid = (valid >= 0.5),
+ *   loss = sum_i weight[i] * mean_valid |pred_i - gt| and EPE = sqrt((pred_last - gt)^2) in fp32.  Reductions run in a fixed order: bit-reproducible.  workspace:
  *   gpsg_sequence_loss_workspace_bytes() bytes, 8-byte aligned.
- * gpsg_sequence_loss_backward: args->grad[i] (numel fp32 each) = d(grad_loss * loss)/d(pred_i), reading the count from
+ * gpsg_sequence_loss_backward: args->grad[i] (numel fp32 each) = d(grad_loss * loss)/d(pred_i), reading 1 / count from
  *   the forward's stats; grad_loss is a DEVICE pointer to one float (NULL = 1).  No host synchronisation.
  * All enqueue on `stream` and do not synchronise. */
 #define GPSG_SEQ_LOSS_MAX_PRED 32
