@@ -71,30 +71,30 @@ def _maps_forward(ctx, settings_list, flags, maps, aux):
         _lib.begin_alloc(dev)
         try:
             with torch.cuda.device(dev):
-                rc = _lib.lib.gpsg_rasterize_forward_maps_begin_ex(
+                rc = _lib.lib.gpsg_rasterize_forward_maps_begin(
                     C.byref(st), idx, sptr, S2, *ptrs, C.c_void_p(radii.data_ptr()), _lib.ALLOC_CB, C.c_void_p(1),
                     _lib.ALLOC_CB, C.c_void_p(3), C.c_void_p(totals[b].data_ptr()), int(flags))
         finally:
             bufs = _lib.end_alloc()
-        _lib.check(rc, "gpsg_rasterize_forward_maps_begin_ex")
+        _lib.check(rc, "gpsg_rasterize_forward_maps_begin")
         per.append(dict(S2=S2, tensors=tensors, ptrs=ptrs, radii=radii, geom=bufs.get(1), image=bufs.get(3)))
     torch.cuda.current_stream(dev).synchronize()           # the ONE host synchronisation of the batch
     ctx.per = []
     for b in range(B):
         p = per[b]
         n = C.c_int32(0)
-        fn = _lib.lib.gpsg_rasterize_forward_maps_finish_aux if aux else _lib.lib.gpsg_rasterize_forward_maps_finish
-        extra = [C.c_void_p(depth[b].data_ptr()), C.c_void_p(alpha[b].data_ptr())] if aux else []
+        extra = [C.c_void_p(depth[b].data_ptr()), C.c_void_p(alpha[b].data_ptr())] if aux else [None, None]
         _lib.begin_alloc(dev)
         try:
             with torch.cuda.device(dev):
-                rc = fn(C.byref(settings_list[b]), idx, sptr, p["S2"], *p["ptrs"], C.c_void_p(out[b].data_ptr()), *extra,
-                        C.c_void_p(p["radii"].data_ptr()), C.c_void_p(p["geom"].data_ptr()),
-                        C.c_void_p(p["image"].data_ptr()), _lib.ALLOC_CB, C.c_void_p(2),
-                        C.c_void_p(totals[b].data_ptr()), C.byref(n))
+                rc = _lib.lib.gpsg_rasterize_forward_maps_finish(
+                    C.byref(settings_list[b]), idx, sptr, p["S2"], *p["ptrs"], C.c_void_p(out[b].data_ptr()), *extra,
+                    C.c_void_p(p["radii"].data_ptr()), C.c_void_p(p["geom"].data_ptr()),
+                    C.c_void_p(p["image"].data_ptr()), _lib.ALLOC_CB, C.c_void_p(2),
+                    C.c_void_p(totals[b].data_ptr()), C.byref(n))
         finally:
             bufs = _lib.end_alloc()
-        _lib.check(rc, fn.__name__)
+        _lib.check(rc, "gpsg_rasterize_forward_maps_finish")
         ctx.per.append(dict(S2=p["S2"], n=int(n.value), tensors=p["tensors"], radii=p["radii"],
                             bufs=(p["geom"], bufs.get(2), p["image"])))
     ctx.settings_list = settings_list
@@ -104,8 +104,8 @@ def _maps_forward(ctx, settings_list, flags, maps, aux):
 
 
 def _maps_backward(ctx, grad_out, grad_depth=None, grad_alpha=None):
-    """Backward of both map Functions: gradients in map layout; with grad_depth / grad_alpha [B,1,H,W] the aux entry
-    point on the aux forward's own buffers."""
+    """Backward of both map Functions: gradients in map layout; with grad_depth / grad_alpha [B,1,H,W] also the aux
+    gradients, on the aux forward's own buffers."""
     aux = grad_depth is not None
     grads = [None, None]                                   # settings_list, flags
     flags = _lib.backward_flags()
@@ -114,19 +114,18 @@ def _maps_backward(ctx, grad_out, grad_depth=None, grad_alpha=None):
     for b, p in enumerate(ctx.per):
         new = lambda ref: [torch.empty_like(ref[0]), torch.empty_like(ref[1])]
         dxyz, dimg, drot, dscale, dopac = (new(t) for t in p["tensors"][1:])
-        L = _lib.lib
-        size_fn = L.gpsg_rasterize_backward_maps_aux_workspace_bytes if aux else L.gpsg_rasterize_backward_maps_workspace_bytes_ex
-        fn = L.gpsg_rasterize_backward_maps_aux if aux else L.gpsg_rasterize_backward_maps_ex
-        ws = torch.empty(int(size_fn(p["S2"], p["n"], flags)), dtype=torch.uint8, device=dev)
+        ws = torch.empty(int(_lib.lib.gpsg_rasterize_backward_maps_workspace_bytes(p["S2"], p["n"], flags, int(aux))),
+                         dtype=torch.uint8, device=dev)
         g = _f32(grad_out[b].detach())
-        gaux = [_f32(grad_depth[b].detach()), _f32(grad_alpha[b].detach())] if aux else []
+        gaux = [_f32(grad_depth[b].detach()), _f32(grad_alpha[b].detach())] if aux else [None, None]
         geom, binning, image = p["bufs"]
         with torch.cuda.device(dev):
-            rc = fn(C.byref(ctx.settings_list[b]), idx, sptr, p["S2"], p["n"], *(_ptrs(t) for t in p["tensors"]),
-                    C.c_void_p(p["radii"].data_ptr()), C.c_void_p(geom.data_ptr()), C.c_void_p(binning.data_ptr()),
-                    C.c_void_p(image.data_ptr()), C.c_void_p(g.data_ptr()), *(C.c_void_p(t.data_ptr()) for t in gaux),
-                    _ptrs(dxyz), _ptrs(dimg), _ptrs(drot), _ptrs(dscale), _ptrs(dopac), C.c_void_p(ws.data_ptr()), flags)
-        _lib.check(rc, fn.__name__)
+            rc = _lib.lib.gpsg_rasterize_backward_maps(
+                C.byref(ctx.settings_list[b]), idx, sptr, p["S2"], p["n"], *(_ptrs(t) for t in p["tensors"]),
+                C.c_void_p(p["radii"].data_ptr()), C.c_void_p(geom.data_ptr()), C.c_void_p(binning.data_ptr()),
+                C.c_void_p(image.data_ptr()), C.c_void_p(g.data_ptr()), *map(_lib._ptr, gaux), _ptrs(dxyz), _ptrs(dimg),
+                _ptrs(drot), _ptrs(dscale), _ptrs(dopac), C.c_void_p(ws.data_ptr()), flags)
+        _lib.check(rc, "gpsg_rasterize_backward_maps")
         sh = ctx.shapes[12 * b:12 * b + 12]
         grads += [None, dxyz[0].view(sh[1]), dimg[0].view(sh[2]), drot[0].view(sh[3]), dscale[0].view(sh[4]),
                   dopac[0].view(sh[5]), None, dxyz[1].view(sh[7]), dimg[1].view(sh[8]), drot[1].view(sh[9]),

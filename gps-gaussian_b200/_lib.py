@@ -52,17 +52,29 @@ _vp, _i, _i64, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_size_t
 lib.gpsg_last_error.restype = C.c_char_p
 lib.gpsg_last_error.argtypes = []
 lib.gpsg_version.restype = _i
+_pp = C.POINTER(C.c_void_p)
+_rs = C.POINTER(RasterSettings)
 lib.gpsg_rasterize_forward.restype = _i
-lib.gpsg_rasterize_forward.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                       _vp, _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, C.POINTER(C.c_int32)]
+lib.gpsg_rasterize_forward.argtypes = [_rs, _i, _vp, _i, _i] + [_vp] * 11 + [
+    ALLOC_FN, _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, C.POINTER(C.c_int32), _i]
+lib.gpsg_rasterize_forward_maps_begin.restype = _i
+lib.gpsg_rasterize_forward_maps_begin.argtypes = [_rs, _i, _vp, _i] + [_pp] * 6 + [
+    _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, _vp, _i]
+lib.gpsg_rasterize_forward_maps_finish.restype = _i
+lib.gpsg_rasterize_forward_maps_finish.argtypes = [_rs, _i, _vp, _i] + [_pp] * 6 + [_vp] * 6 + [
+    ALLOC_FN, _vp, _vp, C.POINTER(C.c_int32)]
+lib.gpsg_rasterize_forward_planned.restype = _i
+lib.gpsg_rasterize_forward_planned.argtypes = [_rs, _i, _vp, _i] + [_vp] * 12 + [_i64, _vp, _vp, _i]
+lib.gpsg_rasterize_forward_maps_planned.restype = _i
+lib.gpsg_rasterize_forward_maps_planned.argtypes = [_rs, _i, _vp, _i] + [_pp] * 6 + [_vp] * 6 + [_i64, _vp, _vp, _i]
 lib.gpsg_rasterize_backward_workspace_bytes.restype = _sz
-lib.gpsg_rasterize_backward_workspace_bytes.argtypes = [_i]
+lib.gpsg_rasterize_backward_workspace_bytes.argtypes = [_i, _i64, _i, _i]
 lib.gpsg_rasterize_backward.restype = _i
-lib.gpsg_rasterize_backward.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, C.c_int32] + [_vp] * 21
-lib.gpsg_rasterize_backward_workspace_bytes_ex.restype = _sz
-lib.gpsg_rasterize_backward_workspace_bytes_ex.argtypes = [_i, _i64, _i]
-lib.gpsg_rasterize_backward_ex.restype = _i
-lib.gpsg_rasterize_backward_ex.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, C.c_int32] + [_vp] * 21 + [_i]
+lib.gpsg_rasterize_backward.argtypes = [_rs, _i, _vp, _i, _i, C.c_int32] + [_vp] * 23 + [_i]
+lib.gpsg_rasterize_backward_maps_workspace_bytes.restype = _sz
+lib.gpsg_rasterize_backward_maps_workspace_bytes.argtypes = [_i, _i64, _i, _i]
+lib.gpsg_rasterize_backward_maps.restype = _i
+lib.gpsg_rasterize_backward_maps.argtypes = [_rs, _i, _vp, _i, C.c_int32] + [_pp] * 6 + [_vp] * 7 + [_pp] * 5 + [_vp, _i]
 lib.gpsg_mark_visible.restype = _i
 lib.gpsg_mark_visible.argtypes = [_i, _vp, _i, _vp, C.POINTER(C.c_float), _vp]
 lib.gpsg_geom_view.restype = _i
@@ -82,57 +94,6 @@ lib.gpsg_raster_binning_bytes.restype = _sz
 lib.gpsg_raster_binning_bytes.argtypes = [_i64]
 lib.gpsg_raster_image_bytes.restype = _sz
 lib.gpsg_raster_image_bytes.argtypes = [_i, _i]
-lib.gpsg_raster_status_ptr.restype = _vp
-lib.gpsg_raster_status_ptr.argtypes = [_vp, _i, _i]
-lib.gpsg_rasterize_forward_planned.restype = _i
-lib.gpsg_rasterize_forward_planned.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_vp] * 10 + [_i64, _vp, _vp]
-_pp = C.POINTER(C.c_void_p)
-lib.gpsg_rasterize_forward_maps_planned.restype = _i
-lib.gpsg_rasterize_forward_maps_planned.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _pp, _pp, _pp, _pp, _pp, _pp, _vp, _vp,
-                                                    _vp, _vp, _i64, _vp, _vp]
-lib.gpsg_rasterize_forward_maps_begin.restype = _i
-lib.gpsg_rasterize_forward_maps_begin.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _pp, _pp, _pp, _pp, _pp, _pp, _vp,
-                                                  ALLOC_FN, _vp, ALLOC_FN, _vp, _vp]
-lib.gpsg_rasterize_forward_maps_finish.restype = _i
-lib.gpsg_rasterize_forward_maps_finish.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _pp, _pp, _pp, _pp, _pp, _pp, _vp, _vp,
-                                                   _vp, _vp, ALLOC_FN, _vp, _vp, C.POINTER(C.c_int32)]
-lib.gpsg_rasterize_backward_maps_workspace_bytes.restype = _sz
-lib.gpsg_rasterize_backward_maps_workspace_bytes.argtypes = [_i]
-lib.gpsg_rasterize_backward_maps.restype = _i
-lib.gpsg_rasterize_backward_maps.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, C.c_int32, _pp, _pp, _pp, _pp, _pp, _pp,
-                                             _vp, _vp, _vp, _vp, _vp, _pp, _pp, _pp, _pp, _pp, _vp]
-lib.gpsg_rasterize_backward_maps_workspace_bytes_ex.restype = _sz
-lib.gpsg_rasterize_backward_maps_workspace_bytes_ex.argtypes = [_i, _i64, _i]
-lib.gpsg_rasterize_backward_maps_ex.restype = _i
-lib.gpsg_rasterize_backward_maps_ex.argtypes = lib.gpsg_rasterize_backward_maps.argtypes + [_i]
-lib.gpsg_rasterize_forward_aux.restype = _i
-lib.gpsg_rasterize_forward_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i] + [_vp] * 11 + [
-    ALLOC_FN, _vp, ALLOC_FN, _vp, ALLOC_FN, _vp, C.POINTER(C.c_int32)]
-lib.gpsg_rasterize_forward_maps_finish_aux.restype = _i
-lib.gpsg_rasterize_forward_maps_finish_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_pp] * 6 + [_vp] * 6 + [
-    ALLOC_FN, _vp, _vp, C.POINTER(C.c_int32)]
-lib.gpsg_rasterize_forward_planned_aux.restype = _i
-lib.gpsg_rasterize_forward_planned_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_vp] * 12 + [_i64, _vp, _vp]
-lib.gpsg_rasterize_forward_maps_planned_aux.restype = _i
-lib.gpsg_rasterize_forward_maps_planned_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i] + [_pp] * 6 + [_vp] * 6 + [
-    _i64, _vp, _vp]
-lib.gpsg_rasterize_backward_aux_workspace_bytes.restype = _sz
-lib.gpsg_rasterize_backward_aux_workspace_bytes.argtypes = [_i, _i64, _i]
-lib.gpsg_rasterize_backward_aux.restype = _i
-lib.gpsg_rasterize_backward_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, _i, C.c_int32] + [_vp] * 23 + [_i]
-lib.gpsg_rasterize_backward_maps_aux_workspace_bytes.restype = _sz
-lib.gpsg_rasterize_backward_maps_aux_workspace_bytes.argtypes = [_i, _i64, _i]
-lib.gpsg_rasterize_backward_maps_aux.restype = _i
-lib.gpsg_rasterize_backward_maps_aux.argtypes = [C.POINTER(RasterSettings), _i, _vp, _i, C.c_int32] + [_pp] * 6 + [
-    _vp] * 7 + [_pp] * 5 + [_vp, _i]
-lib.gpsg_rasterize_forward_ex.restype = _i
-lib.gpsg_rasterize_forward_ex.argtypes = lib.gpsg_rasterize_forward_aux.argtypes + [_i]
-lib.gpsg_rasterize_forward_maps_begin_ex.restype = _i
-lib.gpsg_rasterize_forward_maps_begin_ex.argtypes = lib.gpsg_rasterize_forward_maps_begin.argtypes + [_i]
-lib.gpsg_rasterize_forward_planned_ex.restype = _i
-lib.gpsg_rasterize_forward_planned_ex.argtypes = lib.gpsg_rasterize_forward_planned_aux.argtypes + [_i]
-lib.gpsg_rasterize_forward_maps_planned_ex.restype = _i
-lib.gpsg_rasterize_forward_maps_planned_ex.argtypes = lib.gpsg_rasterize_forward_maps_planned_aux.argtypes + [_i]
 lib.gpsg_corr_build_pyramid.restype = _i
 lib.gpsg_corr_build_pyramid.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, C.POINTER(C.c_void_p), _i]
 lib.gpsg_corr_build_backward.restype = _i
@@ -229,23 +190,16 @@ lib.gpsg_profile_read.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_int32), C.
 lib.gpsg_profile_stage_name.restype = C.c_char_p
 lib.gpsg_profile_stage_name.argtypes = [_i]
 
-EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_rasterize_backward_workspace_bytes",
-            "gpsg_rasterize_backward", "gpsg_mark_visible", "gpsg_geom_view", "gpsg_binning_view", "gpsg_image_view",
-            "gpsg_corr_sampler_forward", "gpsg_corr_sampler_backward", "gpsg_corr_build_pyramid", "gpsg_corr_build_backward",
-            "gpsg_corr_lookup_pyramid_forward", "gpsg_corr_lookup_pyramid_backward", "gpsg_raster_geom_bytes",
-            "gpsg_raster_binning_bytes", "gpsg_raster_image_bytes", "gpsg_raster_status_ptr",
-            "gpsg_rasterize_forward_planned", "gpsg_rasterize_forward_maps_planned", "gpsg_rasterize_forward_maps_begin", "gpsg_rasterize_forward_maps_finish",
-            "gpsg_rasterize_backward_maps_workspace_bytes",
-            "gpsg_rasterize_backward_maps", "gpsg_unproject_forward", "gpsg_unproject_backward", "gpsg_l1_ssim_workspace_bytes", "gpsg_l1_ssim_forward",
-            "gpsg_l1_ssim_backward", "gpsg_set_corr_build", "gpsg_profile_enable",
-            "gpsg_profile_read",
-            "gpsg_profile_stage_name", "gpsg_rasterize_backward_workspace_bytes_ex", "gpsg_rasterize_backward_ex",
-            "gpsg_rasterize_backward_maps_workspace_bytes_ex", "gpsg_rasterize_backward_maps_ex",
-            "gpsg_rasterize_forward_aux", "gpsg_rasterize_forward_maps_finish_aux", "gpsg_rasterize_forward_planned_aux",
-            "gpsg_rasterize_forward_maps_planned_aux", "gpsg_rasterize_backward_aux_workspace_bytes",
-            "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
-            "gpsg_rasterize_backward_maps_aux", "gpsg_rasterize_forward_ex", "gpsg_rasterize_forward_maps_begin_ex",
-            "gpsg_rasterize_forward_planned_ex", "gpsg_rasterize_forward_maps_planned_ex",
+EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_rasterize_forward_maps_begin",
+            "gpsg_rasterize_forward_maps_finish", "gpsg_raster_geom_bytes", "gpsg_raster_binning_bytes",
+            "gpsg_raster_image_bytes", "gpsg_rasterize_forward_planned", "gpsg_rasterize_forward_maps_planned",
+            "gpsg_rasterize_backward_workspace_bytes", "gpsg_rasterize_backward",
+            "gpsg_rasterize_backward_maps_workspace_bytes", "gpsg_rasterize_backward_maps", "gpsg_mark_visible",
+            "gpsg_geom_view", "gpsg_binning_view", "gpsg_image_view", "gpsg_corr_sampler_forward",
+            "gpsg_corr_sampler_backward", "gpsg_corr_build_pyramid", "gpsg_corr_build_backward",
+            "gpsg_corr_lookup_pyramid_forward", "gpsg_corr_lookup_pyramid_backward", "gpsg_unproject_forward",
+            "gpsg_unproject_backward", "gpsg_l1_ssim_workspace_bytes", "gpsg_l1_ssim_forward", "gpsg_l1_ssim_backward",
+            "gpsg_set_corr_build", "gpsg_profile_enable", "gpsg_profile_read", "gpsg_profile_stage_name",
             "gpsg_point_splat_workspace_bytes", "gpsg_point_splat", "gpsg_rectify_remap", "gpsg_rectify_flow",
             "gpsg_convex_upsample_forward", "gpsg_convex_upsample_backward_workspace_bytes",
             "gpsg_convex_upsample_backward", "gpsg_sequence_loss_workspace_bytes", "gpsg_sequence_loss_forward",
@@ -258,7 +212,7 @@ FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)
 
 
 def forward_flags(antialiasing=False):
-    """The `flags` word of the gpsg_*_forward*_ex entry points: GPSG_FWD_ANTIALIAS when `antialiasing`, else 0."""
+    """The `flags` word of the gpsg_rasterize_forward* entry points: GPSG_FWD_ANTIALIAS when `antialiasing`, else 0."""
     return FWD_ANTIALIAS if antialiasing else 0
 
 
@@ -311,15 +265,15 @@ def rasterize_forward(settings, out_color, radii, means3D, opacities, colors_pre
     """One forward through the exact entry point gpsg_rasterize_forward: one host synchronisation, and the global radix
     fallback takes tile lists of any length.  Inputs are contiguous fp32 tensors on one CUDA device, absent ones None.
     Writes out_color [3,H,W] and radii [P]; returns (num_rendered, (geom, binning, image)), the buffers the backward
-    reads.  out_depth / out_alpha ([H,W] fp32, both or neither): aux mode (gpsg_rasterize_forward_aux), which also writes
-    the expected depth and the accumulated opacity.  antialiasing: the opacity-compensated screen-space filter
-    (GPSG_FWD_ANTIALIAS); the backward of these buffers follows it without being told.  Runs gpsg_rasterize_forward_ex."""
+    reads.  out_depth / out_alpha ([H,W] fp32, both or neither): aux mode, which also writes the expected depth and the
+    accumulated opacity.  antialiasing: the opacity-compensated screen-space filter (GPSG_FWD_ANTIALIAS); the backward of
+    these buffers follows it without being told."""
     if (out_depth is None) != (out_alpha is None):
         raise ValueError("out_depth and out_alpha must be given together")
     dev = means3D.device
     idx, stream = device_stream(dev)
     n = C.c_int32(0)
-    fn = lib.gpsg_rasterize_forward_ex
+    fn = lib.gpsg_rasterize_forward
     begin_alloc(dev)
     try:
         with torch.cuda.device(dev):
@@ -335,7 +289,7 @@ def rasterize_forward(settings, out_color, radii, means3D, opacities, colors_pre
 
 
 def backward_flags(deterministic=None):
-    """The `flags` word of the gpsg_*_backward_ex entry points.  deterministic=None follows PyTorch's switch,
+    """The `flags` word of the gpsg_rasterize_backward* entry points.  deterministic=None follows PyTorch's switch,
     torch.use_deterministic_algorithms(True), read when the backward runs (as PyTorch's own kernels read it); True / False
     force the mode.  Deterministic mode gives bit-identical gradients on reruns (include/gpsg.h)."""
     if deterministic is None:
@@ -350,7 +304,7 @@ def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D,
     dL_dmeans2D [P,3], dL_dcolors [P,3], dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dscales [P,3], dL_drots [P,4],
     dL_dcov3D [P,6] and dL_dsh [P,M,3].  dL_dcolors is None on the SH path, dL_dsh is None without shs and dL_dcov3D
     is None unless want_cov3D.  `deterministic`: see `backward_flags`.  grad_depth / grad_alpha ([H,W], both or
-    neither): the aux backward (gpsg_rasterize_backward_aux); the buffers must then come from an aux forward."""
+    neither): the aux gradients; the buffers must then come from an aux forward."""
     if (grad_depth is None) != (grad_alpha is None):
         raise ValueError("grad_depth and grad_alpha must be given together")
     aux = grad_depth is not None
@@ -362,12 +316,12 @@ def rasterize_backward(settings, num_rendered, bufs, radii, grad_color, means3D,
                dL_dopacity=new(P, 1), dL_dmeans3D=new(P, 3), dL_dscales=new(P, 3), dL_drots=new(P, 4),
                dL_dcov3D=new(P, 6) if want_cov3D else None,
                dL_dsh=new(P, int(shs.shape[1]), 3) if shs is not None else None)
-    size_fn = lib.gpsg_rasterize_backward_aux_workspace_bytes if aux else lib.gpsg_rasterize_backward_workspace_bytes_ex
-    ws = torch.empty(int(size_fn(P, num_rendered, flags)), dtype=torch.uint8, device=dev)
+    ws = torch.empty(int(lib.gpsg_rasterize_backward_workspace_bytes(P, num_rendered, flags, int(aux))), dtype=torch.uint8,
+                     device=dev)
     f32 = lambda t: t.detach().to(torch.float32).contiguous()
     g = f32(grad_color)
-    gaux = [f32(grad_depth), f32(grad_alpha)] if aux else []
-    fn = lib.gpsg_rasterize_backward_aux if aux else lib.gpsg_rasterize_backward_ex
+    gaux = [f32(grad_depth), f32(grad_alpha)] if aux else [None, None]
+    fn = lib.gpsg_rasterize_backward
     idx, stream = device_stream(dev)
     geom, binning, image = bufs
     with torch.cuda.device(dev):

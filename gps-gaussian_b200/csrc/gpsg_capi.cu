@@ -297,32 +297,10 @@ static int check_aux_outputs(const float* out_depth, const float* out_alpha) {
 int gpsg_rasterize_forward(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
                            const float* means3D, const float* colors_precomp, const float* shs,
                            const float* opacities, const float* scales, const float* rotations,
-                           const float* cov3D_precomp, float* out_color, int32_t* radii, gpsg_alloc_fn geom_alloc,
-                           void* geom_user, gpsg_alloc_fn binning_alloc, void* binning_user,
-                           gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered) {
-    return gpsg_rasterize_forward_aux(s, device, stream_, P, sh_M, means3D, colors_precomp, shs, opacities, scales, rotations,
-                                      cov3D_precomp, out_color, nullptr, nullptr, radii, geom_alloc, geom_user, binning_alloc,
-                                      binning_user, image_alloc, image_user, num_rendered);
-}
-
-int gpsg_rasterize_forward_aux(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
-                               const float* means3D, const float* colors_precomp, const float* shs,
-                               const float* opacities, const float* scales, const float* rotations,
-                               const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
-                               int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
-                               void* binning_user, gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered) {
-    return gpsg_rasterize_forward_ex(s, device, stream_, P, sh_M, means3D, colors_precomp, shs, opacities, scales, rotations,
-                                     cov3D_precomp, out_color, out_depth, out_alpha, radii, geom_alloc, geom_user,
-                                     binning_alloc, binning_user, image_alloc, image_user, num_rendered, 0);
-}
-
-int gpsg_rasterize_forward_ex(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
-                              const float* means3D, const float* colors_precomp, const float* shs,
-                              const float* opacities, const float* scales, const float* rotations,
-                              const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
-                              int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
-                              void* binning_user, gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered,
-                              int flags) {
+                           const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
+                           int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
+                           void* binning_user, gpsg_alloc_fn image_alloc, void* image_user, int32_t* num_rendered,
+                           int flags) {
     if (int rc_f = check_fwd_flags(flags)) return rc_f;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(P >= 0, "P < 0");
@@ -378,17 +356,8 @@ static GaussianSrc maps_src(int S2, const uint8_t* const* valid, const float* co
 int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
                                       const uint8_t* const* valid, const float* const* xyz, const float* const* img,
                                       const float* const* rot, const float* const* scale, const float* const* opacity,
-                                      int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn image_alloc,
-                                      void* image_user, uint32_t* totals_host) {
-    return gpsg_rasterize_forward_maps_begin_ex(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity, radii,
-                                                geom_alloc, geom_user, image_alloc, image_user, totals_host, 0);
-}
-
-int gpsg_rasterize_forward_maps_begin_ex(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                         const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                         const float* const* rot, const float* const* scale, const float* const* opacity,
-                                         int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
-                                         gpsg_alloc_fn image_alloc, void* image_user, uint32_t* totals_host, int flags) {
+                                      int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
+                                      gpsg_alloc_fn image_alloc, void* image_user, uint32_t* totals_host, int flags) {
     if (int rc_f = check_fwd_flags(flags)) return rc_f;
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(s->image_width > 0 && s->image_height > 0, "image size must be positive");
@@ -403,20 +372,9 @@ int gpsg_rasterize_forward_maps_begin_ex(const GpsgRasterSettings* s, int device
 int gpsg_rasterize_forward_maps_finish(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
                                        const uint8_t* const* valid, const float* const* xyz, const float* const* img,
                                        const float* const* rot, const float* const* scale, const float* const* opacity,
-                                       float* out_color, int32_t* radii, void* geom_buffer, void* image_buffer,
-                                       gpsg_alloc_fn binning_alloc, void* binning_user, const uint32_t* totals_host,
-                                       int32_t* num_rendered) {
-    return gpsg_rasterize_forward_maps_finish_aux(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity,
-                                                  out_color, nullptr, nullptr, radii, geom_buffer, image_buffer, binning_alloc,
-                                                  binning_user, totals_host, num_rendered);
-}
-
-int gpsg_rasterize_forward_maps_finish_aux(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                           const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                           const float* const* rot, const float* const* scale, const float* const* opacity,
-                                           float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
-                                           void* geom_buffer, void* image_buffer, gpsg_alloc_fn binning_alloc,
-                                           void* binning_user, const uint32_t* totals_host, int32_t* num_rendered) {
+                                       float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                       void* geom_buffer, void* image_buffer, gpsg_alloc_fn binning_alloc,
+                                       void* binning_user, const uint32_t* totals_host, int32_t* num_rendered) {
     GPSG_REQUIRE(s != nullptr, "settings is NULL");
     GPSG_REQUIRE(out_color && radii && geom_buffer && image_buffer && binning_alloc && totals_host, "a required pointer is NULL");
     int rc = check_aux_outputs(out_depth, out_alpha);
@@ -432,11 +390,6 @@ int gpsg_rasterize_forward_maps_finish_aux(const GpsgRasterSettings* s, int devi
 size_t gpsg_raster_geom_bytes(int P) { return GeomState::required(P > 0 ? P : 0, scan_temp_bytes(P > 0 ? P : 0)); }
 size_t gpsg_raster_binning_bytes(int64_t capacity_pairs) { return BinningState::required((size_t)(capacity_pairs > 0 ? capacity_pairs : 0), 0); }
 size_t gpsg_raster_image_bytes(int W, int H) { return ImageState::required(W, H); }
-const uint32_t* gpsg_raster_status_ptr(const void* image_buffer, int W, int H) {
-    if (!image_buffer || W <= 0 || H <= 0) return nullptr;
-    return ImageState::carve(const_cast<void*>(image_buffer), W, H).totals;
-}
-
 static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, const GaussianSrc& src,
                                   float* out_color, float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
                                   void* binning_buffer, int64_t capacity_pairs, void* image_buffer, uint32_t* status_host,
@@ -470,31 +423,10 @@ static int forward_planned_common(const GpsgRasterSettings* s, int device, cudaS
 
 int gpsg_rasterize_forward_planned(const GpsgRasterSettings* s, int device, void* stream_, int P, const float* means3D,
                                    const float* colors_precomp, const float* opacities, const float* scales,
-                                   const float* rotations, const float* cov3D_precomp, float* out_color, int32_t* radii,
-                                   void* geom_buffer, void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
-                                   uint32_t* status_host) {
-    return gpsg_rasterize_forward_planned_aux(s, device, stream_, P, means3D, colors_precomp, opacities, scales, rotations,
-                                              cov3D_precomp, out_color, nullptr, nullptr, radii, geom_buffer, binning_buffer,
-                                              capacity_pairs, image_buffer, status_host);
-}
-
-int gpsg_rasterize_forward_planned_aux(const GpsgRasterSettings* s, int device, void* stream_, int P, const float* means3D,
-                                       const float* colors_precomp, const float* opacities, const float* scales,
-                                       const float* rotations, const float* cov3D_precomp, float* out_color,
-                                       float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
-                                       void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
-                                       uint32_t* status_host) {
-    return gpsg_rasterize_forward_planned_ex(s, device, stream_, P, means3D, colors_precomp, opacities, scales, rotations,
-                                             cov3D_precomp, out_color, out_depth, out_alpha, radii, geom_buffer,
-                                             binning_buffer, capacity_pairs, image_buffer, status_host, 0);
-}
-
-int gpsg_rasterize_forward_planned_ex(const GpsgRasterSettings* s, int device, void* stream_, int P, const float* means3D,
-                                      const float* colors_precomp, const float* opacities, const float* scales,
-                                      const float* rotations, const float* cov3D_precomp, float* out_color,
-                                      float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
-                                      void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
-                                      uint32_t* status_host, int flags) {
+                                   const float* rotations, const float* cov3D_precomp, float* out_color,
+                                   float* out_depth, float* out_alpha, int32_t* radii, void* geom_buffer,
+                                   void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
+                                   uint32_t* status_host, int flags) {
     if (int rc_f = check_fwd_flags(flags)) return rc_f;
     GPSG_REQUIRE(means3D && colors_precomp && opacities, "a required pointer is NULL");
     GPSG_REQUIRE(((scales != nullptr && rotations != nullptr) != (cov3D_precomp != nullptr)),
@@ -509,30 +441,9 @@ int gpsg_rasterize_forward_planned_ex(const GpsgRasterSettings* s, int device, v
 int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
                                         const uint8_t* const* valid, const float* const* xyz, const float* const* img,
                                         const float* const* rot, const float* const* scale, const float* const* opacity,
-                                        float* out_color, int32_t* radii, void* geom_buffer, void* binning_buffer,
-                                        int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
-    return gpsg_rasterize_forward_maps_planned_aux(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity,
-                                                   out_color, nullptr, nullptr, radii, geom_buffer, binning_buffer,
-                                                   capacity_pairs, image_buffer, status_host);
-}
-
-int gpsg_rasterize_forward_maps_planned_aux(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                            const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                            const float* const* rot, const float* const* scale,
-                                            const float* const* opacity, float* out_color, float* out_depth,
-                                            float* out_alpha, int32_t* radii, void* geom_buffer, void* binning_buffer,
-                                            int64_t capacity_pairs, void* image_buffer, uint32_t* status_host) {
-    return gpsg_rasterize_forward_maps_planned_ex(s, device, stream_, pixels_per_view, valid, xyz, img, rot, scale, opacity,
-                                                  out_color, out_depth, out_alpha, radii, geom_buffer, binning_buffer,
-                                                  capacity_pairs, image_buffer, status_host, 0);
-}
-
-int gpsg_rasterize_forward_maps_planned_ex(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                           const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                           const float* const* rot, const float* const* scale, const float* const* opacity,
-                                           float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
-                                           void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
-                                           void* image_buffer, uint32_t* status_host, int flags) {
+                                        float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                        void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
+                                        void* image_buffer, uint32_t* status_host, int flags) {
     if (int rc_f = check_fwd_flags(flags)) return rc_f;
     int rc = check_maps(pixels_per_view, valid, xyz, img, rot, scale, opacity);
     if (rc) return rc;
@@ -557,20 +468,17 @@ static int check_bwd_flags(int flags) {
     return GPSG_OK;
 }
 
-static size_t bwd_workspace_bytes(size_t n, size_t slack, int64_t num_rendered, int flags, bool aux) {
+static size_t bwd_workspace_bytes(size_t n, size_t slack, int64_t num_rendered, int flags, int aux) {
     if (check_bwd_flags(flags)) return 0;
+    if (aux != 0 && aux != 1) { set_error("aux must be 0 or 1"); return 0; }
     if (!(flags & GPSG_BWD_DETERMINISTIC)) return bwd_base_bytes(n) + slack;
     if (num_rendered < 0 || num_rendered >= (1ll << 31)) { set_error("num_rendered out of range"); return 0; }
-    return bwd_base_bytes(n) + slack + bwd_det_bytes((size_t)num_rendered, aux);
+    return bwd_base_bytes(n) + slack + bwd_det_bytes((size_t)num_rendered, aux == 1);
 }
 
-size_t gpsg_rasterize_backward_workspace_bytes_ex(int P, int64_t num_rendered, int flags) {
-    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags, false);
+size_t gpsg_rasterize_backward_workspace_bytes(int P, int64_t num_rendered, int flags, int aux) {
+    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags, aux);
 }
-size_t gpsg_rasterize_backward_aux_workspace_bytes(int P, int64_t num_rendered, int flags) {
-    return bwd_workspace_bytes((size_t)(P > 0 ? P : 1), 256, num_rendered, flags, true);
-}
-size_t gpsg_rasterize_backward_workspace_bytes(int P) { return gpsg_rasterize_backward_workspace_bytes_ex(P, 0, 0); }
 
 static int backward_common(const GpsgRasterSettings* s, int device, cudaStream_t stream, int P, int sh_M,
                            int32_t num_rendered, const GaussianSrc& src, const float* shs, const int32_t* radii,
@@ -624,28 +532,14 @@ static int check_aux_grads(const float* dL_dout_depth, const float* dL_dout_alph
     return GPSG_OK;
 }
 
-int gpsg_rasterize_backward_ex(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
-                               int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
-                               const float* opacities, const float* scales, const float* rotations,
-                               const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
-                               const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                               float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                               float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                               void* workspace, int flags) {
-    return gpsg_rasterize_backward_aux(s, device, stream_, P, sh_M, num_rendered, means3D, colors_precomp, shs, opacities,
-                                       scales, rotations, cov3D_precomp, radii, geom_buffer, binning_buffer, image_buffer,
-                                       dL_dout_color, nullptr, nullptr, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D,
-                                       dL_dcov3D, dL_dsh, dL_dscales, dL_drotations, workspace, flags);
-}
-
-int gpsg_rasterize_backward_aux(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
-                                int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
-                                const float* opacities, const float* scales, const float* rotations,
-                                const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
-                                const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                                const float* dL_dout_depth, const float* dL_dout_alpha, float* dL_dmeans2D,
-                                float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
-                                float* dL_dscales, float* dL_drotations, void* workspace, int flags) {
+int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
+                            int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
+                            const float* opacities, const float* scales, const float* rotations,
+                            const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
+                            const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                            const float* dL_dout_depth, const float* dL_dout_alpha, float* dL_dmeans2D,
+                            float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
+                            float* dL_dscales, float* dL_drotations, void* workspace, int flags) {
     int rc = check_bwd_flags(flags);
     if (rc) return rc;
     rc = check_aux_grads(dL_dout_depth, dL_dout_alpha);
@@ -678,50 +572,18 @@ int gpsg_rasterize_backward_aux(const GpsgRasterSettings* s, int device, void* s
     return GPSG_OK;
 }
 
-int gpsg_rasterize_backward(const GpsgRasterSettings* s, int device, void* stream_, int P, int sh_M,
-                            int32_t num_rendered, const float* means3D, const float* colors_precomp, const float* shs,
-                            const float* opacities, const float* scales, const float* rotations,
-                            const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
-                            const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                            float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                            float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                            void* workspace) {
-    return gpsg_rasterize_backward_ex(s, device, stream_, P, sh_M, num_rendered, means3D, colors_precomp, shs, opacities,
-                                      scales, rotations, cov3D_precomp, radii, geom_buffer, binning_buffer, image_buffer,
-                                      dL_dout_color, dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh,
-                                      dL_dscales, dL_drotations, workspace, 0);
+size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view, int64_t num_rendered, int flags, int aux) {
+    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags, aux);
 }
 
-size_t gpsg_rasterize_backward_maps_workspace_bytes_ex(int pixels_per_view, int64_t num_rendered, int flags) {
-    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags, false);
-}
-size_t gpsg_rasterize_backward_maps_aux_workspace_bytes(int pixels_per_view, int64_t num_rendered, int flags) {
-    return bwd_workspace_bytes((size_t)(pixels_per_view > 0 ? 2 * (size_t)pixels_per_view : 1), 512, num_rendered, flags, true);
-}
-size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view) {
-    return gpsg_rasterize_backward_maps_workspace_bytes_ex(pixels_per_view, 0, 0);
-}
-
-int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                    int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
-                                    const float* const* img, const float* const* rot, const float* const* scale,
-                                    const float* const* opacity, const int32_t* radii, const void* geom_buffer,
-                                    const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                                    float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
-                                    float* const* dL_dscale, float* const* dL_dopacity, void* workspace, int flags) {
-    return gpsg_rasterize_backward_maps_aux(s, device, stream_, pixels_per_view, num_rendered, valid, xyz, img, rot, scale,
-                                            opacity, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, nullptr,
-                                            nullptr, dL_dxyz, dL_dimg, dL_drot, dL_dscale, dL_dopacity, workspace, flags);
-}
-
-int gpsg_rasterize_backward_maps_aux(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                     int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
-                                     const float* const* img, const float* const* rot, const float* const* scale,
-                                     const float* const* opacity, const int32_t* radii, const void* geom_buffer,
-                                     const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                                     const float* dL_dout_depth, const float* dL_dout_alpha, float* const* dL_dxyz,
-                                     float* const* dL_dimg, float* const* dL_drot, float* const* dL_dscale,
-                                     float* const* dL_dopacity, void* workspace, int flags) {
+int gpsg_rasterize_backward_maps(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
+                                 int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
+                                 const float* const* img, const float* const* rot, const float* const* scale,
+                                 const float* const* opacity, const int32_t* radii, const void* geom_buffer,
+                                 const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                                 const float* dL_dout_depth, const float* dL_dout_alpha, float* const* dL_dxyz,
+                                 float* const* dL_dimg, float* const* dL_drot, float* const* dL_dscale,
+                                 float* const* dL_dopacity, void* workspace, int flags) {
     int rc = check_bwd_flags(flags);
     if (rc) return rc;
     rc = check_aux_grads(dL_dout_depth, dL_dout_alpha);
@@ -747,18 +609,6 @@ int gpsg_rasterize_backward_maps_aux(const GpsgRasterSettings* s, int device, vo
                            maps_src(pixels_per_view, valid, xyz, img, rot, scale, opacity), nullptr, radii, geom_buffer,
                            binning_buffer, image_buffer, dL_dout_color, dL_dout_depth, dL_dout_alpha, dmeans2D, nullptr,
                            nullptr, out, workspace, flags);
-}
-
-int gpsg_rasterize_backward_maps(const GpsgRasterSettings* s, int device, void* stream_, int pixels_per_view,
-                                 int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
-                                 const float* const* img, const float* const* rot, const float* const* scale,
-                                 const float* const* opacity, const int32_t* radii, const void* geom_buffer,
-                                 const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                                 float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
-                                 float* const* dL_dscale, float* const* dL_dopacity, void* workspace) {
-    return gpsg_rasterize_backward_maps_ex(s, device, stream_, pixels_per_view, num_rendered, valid, xyz, img, rot, scale,
-                                           opacity, radii, geom_buffer, binning_buffer, image_buffer, dL_dout_color, dL_dxyz,
-                                           dL_dimg, dL_drot, dL_dscale, dL_dopacity, workspace, 0);
 }
 
 int gpsg_mark_visible(int device, void* stream_, int P, const float* means3D, const float* viewmatrix_host16,

@@ -236,8 +236,9 @@ class _RasterizeGaussians(torch.autograd.Function):
 
 
 class _RasterizeGaussiansAux(torch.autograd.Function):
-    """Aux mode: (color, depth, alpha, radii).  The backward runs the aux entry point on this forward's own buffers (the
-    precondition of gpsg_rasterize_backward_aux); an output that received no gradient gets zeros from autograd."""
+    """Aux mode: (color, depth, alpha, radii).  The backward passes the aux gradients on this forward's own buffers (the
+    precondition of gpsg_rasterize_backward's dL_dout_depth / dL_dout_alpha); an output that received no gradient gets
+    zeros from autograd."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,

@@ -18,10 +18,10 @@ from .introspect import make_settings
 
 
 def _aux_args(depth, alpha):
-    """The (out_depth, out_alpha) pointer arguments of the _aux planned entry points, or [] without aux outputs."""
+    """The (out_depth, out_alpha) pointer arguments of the planned entry points: (NULL, NULL) without aux outputs."""
     if (depth is None) != (alpha is None):
         raise ValueError("depth and alpha must be given together")
-    return [] if depth is None else [C.c_void_p(depth.data_ptr()), C.c_void_p(alpha.data_ptr())]
+    return (None, None) if depth is None else (C.c_void_p(depth.data_ptr()), C.c_void_p(alpha.data_ptr()))
 
 
 class PlannedRasterizer:
@@ -46,10 +46,9 @@ class PlannedRasterizer:
         """Enqueue one forward on the current stream (P = means3D.shape[0] may be smaller than the P the scratch was
         sized for; `out` / `status_host` redirect the image / deferred status words, as in forward_maps).  Inputs: contiguous fp32 CUDA tensors; `settings`: a
         `_lib.RasterSettings` (see introspect.make_settings) or a synth scene dict.  Returns self.color (valid once the
-        stream has run AND ok() holds).  depth / alpha ([H,W] fp32, both or neither): aux mode
-        (gpsg_rasterize_forward_planned_aux), which also writes the expected depth and the alpha matte.  antialiasing: the
-        opacity-compensated screen-space filter (GPSG_FWD_ANTIALIAS); the image buffer then carries that mode to the
-        backward.  Runs gpsg_rasterize_forward_planned_ex."""
+        stream has run AND ok() holds).  depth / alpha ([H,W] fp32, both or neither): aux mode, which also writes the
+        expected depth and the alpha matte.  antialiasing: the opacity-compensated screen-space filter
+        (GPSG_FWD_ANTIALIAS); the image buffer then carries that mode to the backward."""
         if isinstance(settings, dict):
             settings = make_settings(settings)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
@@ -57,8 +56,8 @@ class PlannedRasterizer:
         if P > self.P:
             raise ValueError(f"PlannedRasterizer scratch holds P<={self.P}, got {P}")
         color = self.color if out is None else out
-        aux = _aux_args(depth, alpha) or [None, None]       # the _ex forwards take both pointers, NULL without aux
-        fn = _lib.lib.gpsg_rasterize_forward_planned_ex
+        aux = _aux_args(depth, alpha)
+        fn = _lib.lib.gpsg_rasterize_forward_planned
         rc = fn(C.byref(settings), *_lib.device_stream(self.dev), P, p(means3D),
                 p(colors), p(opacity), p(scales), p(rots), p(cov3D_precomp), p(color), *aux, p(self.radii), p(self.geom),
                 p(self.binning), self.capacity, p(self.image),
@@ -73,16 +72,15 @@ class PlannedRasterizer:
         each argument is a pair (lmain, rmain) of contiguous CUDA tensors -- valid uint8/bool [S2], xyz [S2,3], img
         [3,S2] in [-1,1], rot [4,S2], scale [3,S2], opacity [1,S2]; self.P must be 2*S2.  `out` optionally redirects
         the image to another [3,H,W] tensor (e.g. a slice of a batch); `status_host` optionally redirects the deferred
-        status words to another pinned int32[>=3] tensor (one per in-flight job).  depth / alpha: aux mode, as in
-        forward (gpsg_rasterize_forward_maps_planned_aux).  antialiasing: as in forward
-        (gpsg_rasterize_forward_maps_planned_ex)."""
+        status words to another pinned int32[>=3] tensor (one per in-flight job).  depth / alpha, antialiasing: as in
+        forward."""
         S2 = int(valid[0].numel())
         if 2 * S2 != self.P:
             raise ValueError(f"PlannedRasterizer built for P={self.P}, maps hold 2*{S2} candidates")
         pp = lambda ts: (C.c_void_p * 2)(*[t.data_ptr() for t in ts])
         color = self.color if out is None else out
-        aux = _aux_args(depth, alpha) or [None, None]       # the _ex forwards take both pointers, NULL without aux
-        fn = _lib.lib.gpsg_rasterize_forward_maps_planned_ex
+        aux = _aux_args(depth, alpha)
+        fn = _lib.lib.gpsg_rasterize_forward_maps_planned
         rc = fn(C.byref(settings), *_lib.device_stream(self.dev), S2, pp(valid), pp(xyz),
                 pp(img), pp(rot), pp(scale), pp(opacity), C.c_void_p(color.data_ptr()), *aux,
                 C.c_void_p(self.radii.data_ptr()), C.c_void_p(self.geom.data_ptr()), C.c_void_p(self.binning.data_ptr()),

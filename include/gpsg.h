@@ -63,243 +63,165 @@ typedef void* (*gpsg_alloc_fn)(void* user, size_t bytes);
 GPSG_API const char* gpsg_last_error(void);
 GPSG_API int gpsg_version(void);
 
-/* ---- replaces _C.rasterize_gaussians (SURVEY.md Appendix A.1-A.5) ---------------------------
- * means3D[P,3] opacities[P] ; exactly one of colors_precomp[P,3] / shs[P,sh_M,3] ; either
- * (scales[P,3], rotations[P,4]) or cov3D_precomp[P,6].  Outputs out_color[3,H,W], radii[P].
- * Scratch comes from the three callbacks (geometry / binning / image state, kept for backward).
- * *num_rendered (HOST) receives the number of (tile,Gaussian) pairs.  One host sync, as upstream. */
-GPSG_API int gpsg_rasterize_forward(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
-                           const float* means3D, const float* colors_precomp, const float* shs,
-                           const float* opacities, const float* scales, const float* rotations,
-                           const float* cov3D_precomp, float* out_color, int32_t* radii,
-                           gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn binning_alloc,
-                           void* binning_user, gpsg_alloc_fn image_alloc, void* image_user,
-                           int32_t* num_rendered);
+/* ==== splat rasterizer: replaces _C.rasterize_gaussians / _C.rasterize_gaussians_backward (SURVEY.md Appendix A) ====
+ * Conventions shared by the entry points below.
+ *
+ * Gaussians come in one of two forms.
+ *   AoS: means3D[P,3] opacities[P]; exactly one of colors_precomp[P,3] / shs[P,sh_M,3]; either (scales[P,3],
+ *     rotations[P,4]) or cov3D_precomp[P,6].
+ *   maps (the fused map -> Gaussian ingest behind pts2render, reference lib/GaussianRender.py:5-39): the two source
+ *     views' pixel-aligned maps are read in place instead of boolean-mask gathered (10 `nonzero` host syncs per sample)
+ *     and concatenated.  Per view v in {0,1} (lmain, rmain), with S2 = pixels_per_view: valid[v][S2] (uint8/bool),
+ *     xyz[v][S2,3], img[v][3,S2] in [-1,1] (colour = img*0.5+0.5), rot[v][4,S2], scale[v][3,S2], opacity[v][1,S2].
+ *     Gaussian index = v*S2 + pixel, so P = 2*S2; invalid pixels are culled.  Pointer arguments of this form are HOST
+ *     arrays of two device pointers.  Results (image, and gradients in map layout) equal the gather + render path.
+ *
+ * Outputs: out_color[3,H,W] and radii[P].  out_depth[H,W] and out_alpha[H,W] (fp32) are the aux outputs, both NULL or
+ *   both set:
+ *     alpha = 1 - T_final (accumulated opacity; exactly 1 - the transmittance the backward reads),
+ *     depth = sum_i w_i z_i, w_i = alpha_i T_i the compositing weight and z_i the view-space depth of Gaussian i (the key
+ *             the tile lists are sorted by).  Not normalised by alpha and without background (depth = 0 where nothing is
+ *             drawn): depth is a fourth colour channel whose colour is z and whose background is 0.
+ *   The colour image, radii and the saved buffers are bit-identical with and without the aux outputs, and the buffers
+ *   have the same sizes (z is read from the geometry buffer).
+ *
+ * Forward flags (`flags` of gpsg_rasterize_forward, _maps_begin, _planned and _maps_planned):
+ *   0: the upstream forward.
+ *   GPSG_FWD_ANTIALIAS: opacity-compensated screen-space filter (upstream's `antialiasing` setting, the 2-D filter of
+ *     Mip-Splatting).  The 0.3 px^2 dilation of the screen covariance stays, so the conics, radii, tile lists and sort
+ *     keys are bit-identical to flags = 0; each splat's opacity is scaled by rho = sqrt(max(2.5e-5, det(Sigma2D) /
+ *     det(Sigma2D + 0.3 I))), so its integrated alpha no longer grows with the dilation (sub-pixel splats no longer turn
+ *     into >= 0.55 px blobs at full opacity).  The scaled opacity o * rho is what conic_opacity[P,4].w (gpsg_geom_view)
+ *     holds and what the compositing uses.
+ *   The forward records its flags in its image buffer, on the device and in stream order (no host synchronisation, so
+ *   the planned forwards stay graph-capturable).  The backward reads them from the image buffer it is given, so it always
+ *   differentiates the mode of the forward whose buffers it receives.  A reused planned image buffer carries the mode of
+ *   its last forward.
+ *   Unknown flag bits return GPSG_E_INVALID before any other argument is checked.
+ *
+ * Saved buffers: every forward leaves a geometry, a binning and an image buffer; the backward reads the three of the
+ * forward it differentiates. */
+#define GPSG_FWD_ANTIALIAS 1
 
-/* ---- sync-free ("planned") forward: same computation as gpsg_rasterize_forward, but every buffer is provided by the
- * caller up front and there is NO host synchronisation, so the call is CUDA-graph capturable and the CPU can run
- * ahead.  `capacity_pairs` bounds the number of (tile,Gaussian) pairs the binning buffer can hold.  The kernels
- * read the actual pair count from device memory; if it exceeds the capacity (or a tile list exceeds the in-CTA sort
- * limit) they set the overflow word and skip their work: the caller must inspect status[2] once it next
- * synchronises and, if set, retry with a larger capacity / the exact entry point (out_color is then undefined).
- * status (device pointer into image_buf, see gpsg_raster_status_ptr; optionally mirrored to `status_host`, pinned):
- * [0] pairs N, [1] longest tile list, [2] overflow flag.  For gpsg_rasterize_backward pass num_rendered = capacity. */
+/* ---- exact forward: replaces _C.rasterize_gaussians --------------------------------------------------------------
+ * AoS Gaussians.  Scratch comes from the three callbacks (geometry / binning / image buffer, kept for the backward).
+ * *num_rendered (HOST) receives the number of (tile, Gaussian) pairs.  One host synchronisation, as upstream, and tile
+ * lists of any length (a global radix sort takes those too long for the in-CTA sort). */
+GPSG_API int gpsg_rasterize_forward(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
+                                    const float* means3D, const float* colors_precomp, const float* shs,
+                                    const float* opacities, const float* scales, const float* rotations,
+                                    const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
+                                    int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
+                                    gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
+                                    void* image_user, int32_t* num_rendered, int flags);
+
+/* ---- exact forward of the maps, in two halves ---------------------------------------------------------------------
+ * A BATCH of samples needs ONE host synchronisation (reference lib/GaussianRender.py:8 loops over the samples; upstream
+ * synchronises once per sample to read num_rendered):
+ *   _begin : projection (under `flags`), pairs-per-tile counts, tile ranges; allocates the geometry and image buffers
+ *            through the callbacks (the caller keeps the pointers they returned) and enqueues a copy of 6 status words
+ *            into `totals_host` (pinned host memory).  Does NOT synchronise.
+ *   ... the caller synchronises `stream` once after the _begin calls of all samples ...
+ *   _finish: sizes and allocates the binning buffer from totals_host, bins, sorts, composites into out_color (and the
+ *            aux outputs when set); *num_rendered (HOST) receives the pair count.  The forward's mode is the one _begin
+ *            recorded, so _finish takes no flags.
+ * A batch of one is begin, one synchronisation, finish.  The saved buffers feed gpsg_rasterize_backward_maps. */
+GPSG_API int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* settings, int device, void* stream,
+                                               int pixels_per_view, const uint8_t* const* valid, const float* const* xyz,
+                                               const float* const* img, const float* const* rot,
+                                               const float* const* scale, const float* const* opacity, int32_t* radii,
+                                               gpsg_alloc_fn geom_alloc, void* geom_user, gpsg_alloc_fn image_alloc,
+                                               void* image_user, uint32_t* totals_host /* >= 6 words, pinned */,
+                                               int flags);
+GPSG_API int gpsg_rasterize_forward_maps_finish(const GpsgRasterSettings* settings, int device, void* stream,
+                                                int pixels_per_view, const uint8_t* const* valid,
+                                                const float* const* xyz, const float* const* img,
+                                                const float* const* rot, const float* const* scale,
+                                                const float* const* opacity, float* out_color, float* out_depth,
+                                                float* out_alpha, int32_t* radii, void* geom_buffer, void* image_buffer,
+                                                gpsg_alloc_fn binning_alloc, void* binning_user,
+                                                const uint32_t* totals_host, int32_t* num_rendered);
+
+/* ---- sync-free ("planned") forwards: the serving loop (reference test_view_interp.py:39-47) ------------------------
+ * The same computation as the exact forward, but every buffer is provided by the caller up front and there is NO host
+ * synchronisation, so the call is CUDA-graph capturable and the CPU can run ahead.  Buffer sizes: gpsg_raster_geom_bytes
+ * (P; P = 2*pixels_per_view for the maps), gpsg_raster_image_bytes(W, H) and gpsg_raster_binning_bytes(capacity_pairs),
+ * where capacity_pairs bounds the number of (tile, Gaussian) pairs the binning buffer can hold.
+ * Overflow: the kernels read the actual pair count from device memory; if it exceeds the capacity (or a tile list exceeds
+ * the in-CTA sort limit) they set the overflow word and skip their work.  The caller must inspect the status words once
+ * it next synchronises and, if the overflow word is set, retry with a larger capacity or the exact forward (out_color
+ * and the aux outputs are then undefined).  Status words, [0] pairs N, [1] longest tile list, [2] overflow flag: kept in
+ * the image buffer and copied to `status_host` (pinned host memory, >= 3 words) when it is not NULL.
+ * gpsg_rasterize_forward_planned takes AoS Gaussians with colors_precomp (no SH); gpsg_rasterize_forward_maps_planned
+ * renders many novel cameras from one pair's cached maps without gathering them.  For the backward of a planned forward
+ * pass num_rendered = capacity_pairs. */
 GPSG_API size_t gpsg_raster_geom_bytes(int P);
 GPSG_API size_t gpsg_raster_binning_bytes(int64_t capacity_pairs);
 GPSG_API size_t gpsg_raster_image_bytes(int W, int H);
-GPSG_API const uint32_t* gpsg_raster_status_ptr(const void* image_buffer, int W, int H);
 GPSG_API int gpsg_rasterize_forward_planned(const GpsgRasterSettings* settings, int device, void* stream, int P,
                                             const float* means3D, const float* colors_precomp, const float* opacities,
                                             const float* scales, const float* rotations, const float* cov3D_precomp,
-                                            float* out_color, int32_t* radii, void* geom_buffer, void* binning_buffer,
-                                            int64_t capacity_pairs, void* image_buffer, uint32_t* status_host);
-
-/* ---- replaces _C.rasterize_gaussians_backward (Appendix A.6-A.8) ----------------------------
- * geom/binning/image buffers are the ones the forward allocated.  All dL_* outputs are written
- * (zero for culled Gaussians); dL_dmeans2D is [P,3] (z unused), dL_dcov3D [P,6] and dL_dsh
- * [P,sh_M,3] may be NULL when not needed.  `workspace` must hold gpsg_rasterize_backward_workspace_bytes(P). */
-GPSG_API size_t gpsg_rasterize_backward_workspace_bytes(int P);
-GPSG_API int gpsg_rasterize_backward(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
-                            int32_t num_rendered, const float* means3D, const float* colors_precomp,
-                            const float* shs, const float* opacities, const float* scales, const float* rotations,
-                            const float* cov3D_precomp, const int32_t* radii, const void* geom_buffer,
-                            const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
-                            float* dL_dmeans2D, float* dL_dcolors, float* dL_dopacity, float* dL_dmeans3D,
-                            float* dL_dcov3D, float* dL_dsh, float* dL_dscales, float* dL_drotations,
-                            void* workspace);
-
-/* ---- deterministic backward: the same two backward entry points with a `flags` word -------------------------------
- * flags = 0: exactly gpsg_rasterize_backward / _maps (same workspace size, same results; those two are these with 0).
- * flags = GPSG_BWD_DETERMINISTIC: bit-identical gradients for identical inputs on the same device and build, whatever
- *   the CTA schedule, concurrent work on other streams or the binning path (tile bucket or GPSG_BINNING=radix).  The
- *   compositing backward stores its per-(pair, warp) partial sums instead of adding them with atomics, and one thread
- *   per Gaussian adds them in a fixed order.  The gradients differ from flags = 0 only by fp32 re-association.  It reads
- *   the sorted keys and point list, so it needs the buffers of an EXACT forward (gpsg_rasterize_forward or maps
- *   _begin/_finish); the planned forwards do not write them and are not supported.  No host synchronisation, no
- *   allocation: graph-capturable like flags = 0.  The workspace grows by 289 bytes per pair (1-byte slot mask + 8 x 9
- *   floats), plus alignment, so the workspace-size functions also take num_rendered.
- * Unknown flag bits: the backward returns GPSG_E_INVALID and the size functions return 0 (message in gpsg_last_error). */
-#define GPSG_BWD_DETERMINISTIC 1
-GPSG_API size_t gpsg_rasterize_backward_workspace_bytes_ex(int P, int64_t num_rendered, int flags);
-GPSG_API int gpsg_rasterize_backward_ex(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
-                                        int32_t num_rendered, const float* means3D, const float* colors_precomp,
-                                        const float* shs, const float* opacities, const float* scales,
-                                        const float* rotations, const float* cov3D_precomp, const int32_t* radii,
-                                        const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
-                                        const float* dL_dout_color, float* dL_dmeans2D, float* dL_dcolors,
-                                        float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
-                                        float* dL_dscales, float* dL_drotations, void* workspace, int flags);
-
-/* ---- fused map -> Gaussian ingest: the rasterizer behind lib/GaussianRender.py:5-39 (pts2render) -------------------
- * Instead of boolean-mask gathering (10 `nonzero` host syncs per sample) and concatenating the two source views'
- * pixel-aligned maps into [P,k] tensors, the maps are read in place: per view v in {0,1} (lmain, rmain), with S2 =
- * pixels_per_view:  valid[v][S2] (uint8/bool), xyz[v][S2,3], img[v][3,S2] in [-1,1] (colour = img*0.5+0.5),
- * rot[v][4,S2], scale[v][3,S2], opacity[v][1,S2].  Gaussian index = v*S2 + pixel; invalid pixels are culled.
- * radii has 2*S2 entries.  Results (image, and gradients in map layout) equal the gather+render path.
- * The exact forward comes in two halves, so that a BATCH of samples needs ONE host synchronisation (reference
- * lib/GaussianRender.py:8 loops over the samples; upstream synchronises once per sample to read num_rendered):
- *   _begin : projection, pairs-per-tile counts, tile ranges; allocates the geometry and image buffers through the callbacks
- *            (the caller keeps the pointers they returned) and enqueues a copy of 6 status words into `totals_host`
- *            (pinned host memory).  Does NOT synchronise.
- *   ... the caller synchronises `stream` once after the _begin calls of all samples ...
- *   _finish: sizes and allocates the binning buffer from totals_host, bins, sorts, composites into out_color.
- * A batch of one is begin, one synchronisation, finish.  The saved buffers feed gpsg_rasterize_backward_maps. */
-GPSG_API int gpsg_rasterize_forward_maps_begin(const GpsgRasterSettings* settings, int device, void* stream, int pixels_per_view,
-                                               const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                               const float* const* rot, const float* const* scale,
-                                               const float* const* opacity, int32_t* radii, gpsg_alloc_fn geom_alloc,
-                                               void* geom_user, gpsg_alloc_fn image_alloc, void* image_user,
-                                               uint32_t* totals_host /* >= 6 words, pinned */);
-GPSG_API int gpsg_rasterize_forward_maps_finish(const GpsgRasterSettings* settings, int device, void* stream, int pixels_per_view,
-                                                const uint8_t* const* valid, const float* const* xyz, const float* const* img,
-                                                const float* const* rot, const float* const* scale,
-                                                const float* const* opacity, float* out_color, int32_t* radii,
-                                                void* geom_buffer, void* image_buffer, gpsg_alloc_fn binning_alloc,
-                                                void* binning_user, const uint32_t* totals_host, int32_t* num_rendered);
-
-/* sync-free form of the map-ingest forward (same contract as gpsg_rasterize_forward_planned; geom buffer sized for
- * P = 2*pixels_per_view): the serving loop of test_view_interp.py:39-47 renders many novel cameras from ONE pair's
- * cached maps without gathering them and without a host sync. */
+                                            float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
+                                            void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
+                                            void* image_buffer, uint32_t* status_host, int flags);
 GPSG_API int gpsg_rasterize_forward_maps_planned(const GpsgRasterSettings* settings, int device, void* stream,
-                                                 int pixels_per_view, const uint8_t* const* valid, const float* const* xyz,
-                                                 const float* const* img, const float* const* rot,
-                                                 const float* const* scale, const float* const* opacity, float* out_color,
-                                                 int32_t* radii, void* geom_buffer, void* binning_buffer,
-                                                 int64_t capacity_pairs, void* image_buffer, uint32_t* status_host);
-GPSG_API size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view);
-GPSG_API int gpsg_rasterize_backward_maps(const GpsgRasterSettings* settings, int device, void* stream, int pixels_per_view,
-                                          int32_t num_rendered, const uint8_t* const* valid, const float* const* xyz,
-                                          const float* const* img, const float* const* rot, const float* const* scale,
-                                          const float* const* opacity, const int32_t* radii, const void* geom_buffer,
-                                          const void* binning_buffer, const void* image_buffer, const float* dL_dout_color,
+                                                 int pixels_per_view, const uint8_t* const* valid,
+                                                 const float* const* xyz, const float* const* img,
+                                                 const float* const* rot, const float* const* scale,
+                                                 const float* const* opacity, float* out_color, float* out_depth,
+                                                 float* out_alpha, int32_t* radii, void* geom_buffer,
+                                                 void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
+                                                 uint32_t* status_host, int flags);
+
+/* ---- backward: replaces _C.rasterize_gaussians_backward -------------------------------------------------------------
+ * gpsg_rasterize_backward differentiates gpsg_rasterize_forward or a planned AoS forward; gpsg_rasterize_backward_maps
+ * differentiates the maps forwards and writes the gradients in map layout.  The geom / binning / image buffers, radii and
+ * num_rendered are the forward's.  All dL_* outputs are written (zero for culled Gaussians).  AoS: dL_dmeans2D is [P,3]
+ * (z unused); dL_dsh [P,sh_M,3] is given exactly when shs is; dL_dcolors may be NULL on the SH path and dL_dcov3D [P,6]
+ * when not needed.
+ * Aux gradients: dL_dout_depth[H,W] and dL_dout_alpha[H,W], both NULL or both set (either may hold zeros).  When set, the
+ *   buffers (and num_rendered) must come from a forward of the same inputs that wrote the depth and alpha outputs those
+ *   gradients belong to.  The depth gradient reaches dL_dmeans3D (maps: dL_dxyz) through the view matrix's third row; the
+ *   alpha gradient reaches the opacities and the geometry through the compositing weights.
+ * flags:
+ *   0: per-Gaussian sums with atomics, as upstream.
+ *   GPSG_BWD_DETERMINISTIC: bit-identical gradients for identical inputs on the same device and build, whatever the CTA
+ *     schedule, concurrent work on other streams or the binning path (tile bucket or GPSG_BINNING=radix).  The
+ *     compositing backward stores its per-(pair, warp) partial sums instead of adding them with atomics, and one thread
+ *     per Gaussian adds them in a fixed order.  The gradients differ from flags = 0 only by fp32 re-association.  It
+ *     reads the sorted keys and point list, so it needs the buffers of an EXACT forward (gpsg_rasterize_forward or maps
+ *     _begin / _finish); the planned forwards do not write them and are not supported.
+ *   Unknown flag bits return GPSG_E_INVALID before any other argument is checked.
+ * No host synchronisation and no allocation in either mode: graph-capturable.
+ * `workspace` must hold gpsg_rasterize_backward_workspace_bytes(P, num_rendered, flags, aux) bytes (maps:
+ * gpsg_rasterize_backward_maps_workspace_bytes(pixels_per_view, ...)), aux = 1 when the aux gradients are set, else 0.
+ * Without GPSG_BWD_DETERMINISTIC the size depends on neither num_rendered nor aux.  With it the partial sums add per pair
+ * a 1-byte slot mask and 8 slots of 9 floats (aux = 0: 289 B) or 10 floats (aux = 1: 321 B), plus alignment.  The size
+ * queries return 0 (message in gpsg_last_error) for unknown flag bits, an aux other than 0 or 1, or, with
+ * GPSG_BWD_DETERMINISTIC, a num_rendered outside [0, 2^31). */
+#define GPSG_BWD_DETERMINISTIC 1
+GPSG_API size_t gpsg_rasterize_backward_workspace_bytes(int P, int64_t num_rendered, int flags, int aux);
+GPSG_API int gpsg_rasterize_backward(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
+                                     int32_t num_rendered, const float* means3D, const float* colors_precomp,
+                                     const float* shs, const float* opacities, const float* scales,
+                                     const float* rotations, const float* cov3D_precomp, const int32_t* radii,
+                                     const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
+                                     const float* dL_dout_color, const float* dL_dout_depth,
+                                     const float* dL_dout_alpha, float* dL_dmeans2D, float* dL_dcolors,
+                                     float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
+                                     float* dL_dscales, float* dL_drotations, void* workspace, int flags);
+GPSG_API size_t gpsg_rasterize_backward_maps_workspace_bytes(int pixels_per_view, int64_t num_rendered, int flags,
+                                                             int aux);
+GPSG_API int gpsg_rasterize_backward_maps(const GpsgRasterSettings* settings, int device, void* stream,
+                                          int pixels_per_view, int32_t num_rendered, const uint8_t* const* valid,
+                                          const float* const* xyz, const float* const* img, const float* const* rot,
+                                          const float* const* scale, const float* const* opacity,
+                                          const int32_t* radii, const void* geom_buffer, const void* binning_buffer,
+                                          const void* image_buffer, const float* dL_dout_color,
+                                          const float* dL_dout_depth, const float* dL_dout_alpha,
                                           float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
-                                          float* const* dL_dscale, float* const* dL_dopacity, void* workspace);
-/* the map-ingest backward with a flags word (see gpsg_rasterize_backward_ex) */
-GPSG_API size_t gpsg_rasterize_backward_maps_workspace_bytes_ex(int pixels_per_view, int64_t num_rendered, int flags);
-GPSG_API int gpsg_rasterize_backward_maps_ex(const GpsgRasterSettings* settings, int device, void* stream,
-                                             int pixels_per_view, int32_t num_rendered, const uint8_t* const* valid,
-                                             const float* const* xyz, const float* const* img, const float* const* rot,
-                                             const float* const* scale, const float* const* opacity,
-                                             const int32_t* radii, const void* geom_buffer, const void* binning_buffer,
-                                             const void* image_buffer, const float* dL_dout_color,
-                                             float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
-                                             float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
-                                             int flags);
-
-/* ---- aux mode: expected depth and alpha beside the colour image ---------------------------------------------------
- * Each forward above has an _aux form with two more outputs after out_color, out_depth[H,W] and out_alpha[H,W] (fp32,
- * both NULL -- then it is exactly the forward without _aux, which is that form with NULL -- or both set):
- *   alpha = 1 - T_final (accumulated opacity; exactly 1 - the transmittance the backward reads),
- *   depth = sum_i w_i z_i,  w_i = alpha_i T_i the compositing weight and z_i the view-space depth of Gaussian i (the
- *           key the tile lists are sorted by).  Not normalised by alpha and without background (depth = 0 where nothing
- *           is drawn), i.e. depth is a fourth colour channel whose colour is z and whose background is 0.
- * The colour image, radii and the saved buffers are bit-identical to the forward without _aux on the same inputs.  The
- * buffers have the same sizes (z is read from the geometry buffer, so the planned forwards take the same
- * gpsg_raster_binning_bytes capacity), and the sync-free / overflow contract of the planned forms is unchanged.
- * maps: gpsg_rasterize_forward_maps_begin is shared; only _finish has an _aux form. */
-GPSG_API int gpsg_rasterize_forward_aux(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
-                                        const float* means3D, const float* colors_precomp, const float* shs,
-                                        const float* opacities, const float* scales, const float* rotations,
-                                        const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
-                                        int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
-                                        gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
-                                        void* image_user, int32_t* num_rendered);
-GPSG_API int gpsg_rasterize_forward_maps_finish_aux(const GpsgRasterSettings* settings, int device, void* stream,
-                                                    int pixels_per_view, const uint8_t* const* valid,
-                                                    const float* const* xyz, const float* const* img,
-                                                    const float* const* rot, const float* const* scale,
-                                                    const float* const* opacity, float* out_color, float* out_depth,
-                                                    float* out_alpha, int32_t* radii, void* geom_buffer,
-                                                    void* image_buffer, gpsg_alloc_fn binning_alloc, void* binning_user,
-                                                    const uint32_t* totals_host, int32_t* num_rendered);
-GPSG_API int gpsg_rasterize_forward_planned_aux(const GpsgRasterSettings* settings, int device, void* stream, int P,
-                                                const float* means3D, const float* colors_precomp, const float* opacities,
-                                                const float* scales, const float* rotations, const float* cov3D_precomp,
-                                                float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
-                                                void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
-                                                void* image_buffer, uint32_t* status_host);
-GPSG_API int gpsg_rasterize_forward_maps_planned_aux(const GpsgRasterSettings* settings, int device, void* stream,
-                                                     int pixels_per_view, const uint8_t* const* valid,
-                                                     const float* const* xyz, const float* const* img,
-                                                     const float* const* rot, const float* const* scale,
-                                                     const float* const* opacity, float* out_color, float* out_depth,
-                                                     float* out_alpha, int32_t* radii, void* geom_buffer,
-                                                     void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
-                                                     uint32_t* status_host);
-/* Backward of the aux forwards: the _ex backwards with dL_dout_depth[H,W] and dL_dout_alpha[H,W] after dL_dout_color
- * (both NULL -- then it is exactly the _ex backward, which is this with NULL -- or both set; either may hold zeros).
- * Precondition: with the aux gradients set, the buffers (and num_rendered) must come from an _aux forward of the same
- * inputs whose depth and alpha outputs those gradients belong to.  The depth gradient reaches dL_dmeans3D (maps:
- * dL_dxyz) through the view matrix's third row; the alpha gradient reaches the opacities and the geometry through the
- * compositing weights.  flags as for the _ex backwards (GPSG_BWD_DETERMINISTIC or 0).  The workspace must hold the
- * _aux_workspace_bytes size: with GPSG_BWD_DETERMINISTIC the partial sums are 8 x 10 floats per pair (321 B per pair
- * plus alignment); without it the size equals the _ex size. */
-GPSG_API size_t gpsg_rasterize_backward_aux_workspace_bytes(int P, int64_t num_rendered, int flags);
-GPSG_API int gpsg_rasterize_backward_aux(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
-                                         int32_t num_rendered, const float* means3D, const float* colors_precomp,
-                                         const float* shs, const float* opacities, const float* scales,
-                                         const float* rotations, const float* cov3D_precomp, const int32_t* radii,
-                                         const void* geom_buffer, const void* binning_buffer, const void* image_buffer,
-                                         const float* dL_dout_color, const float* dL_dout_depth,
-                                         const float* dL_dout_alpha, float* dL_dmeans2D, float* dL_dcolors,
-                                         float* dL_dopacity, float* dL_dmeans3D, float* dL_dcov3D, float* dL_dsh,
-                                         float* dL_dscales, float* dL_drotations, void* workspace, int flags);
-GPSG_API size_t gpsg_rasterize_backward_maps_aux_workspace_bytes(int pixels_per_view, int64_t num_rendered, int flags);
-GPSG_API int gpsg_rasterize_backward_maps_aux(const GpsgRasterSettings* settings, int device, void* stream,
-                                              int pixels_per_view, int32_t num_rendered, const uint8_t* const* valid,
-                                              const float* const* xyz, const float* const* img, const float* const* rot,
-                                              const float* const* scale, const float* const* opacity,
-                                              const int32_t* radii, const void* geom_buffer, const void* binning_buffer,
-                                              const void* image_buffer, const float* dL_dout_color,
-                                              const float* dL_dout_depth, const float* dL_dout_alpha,
-                                              float* const* dL_dxyz, float* const* dL_dimg, float* const* dL_drot,
-                                              float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
-                                              int flags);
-
-/* ---- forward flags: the forwards above with a trailing `flags` word -----------------------------------------------
- * Each _ex forward covers its aux form too (out_depth / out_alpha both NULL or both set, as for the _aux forwards).
- * flags = 0 is exactly the entry point without _ex (those are these with 0).
- * flags = GPSG_FWD_ANTIALIAS: opacity-compensated screen-space filter (upstream's `antialiasing` setting, the 2-D filter of
- *   Mip-Splatting).  The 0.3 px^2 dilation of the screen covariance stays, so the conics, radii, tile lists and sort
- *   keys are bit-identical to flags = 0; each splat's opacity is scaled by rho = sqrt(max(2.5e-5, det(Sigma2D) /
- *   det(Sigma2D + 0.3 I))), so its integrated alpha no longer grows with the dilation (sub-pixel splats no longer turn
- *   into >= 0.55 px blobs at full opacity).  The scaled opacity o * rho is what conic_opacity[P,4].w (gpsg_geom_view)
- *   holds and what the compositing uses.
- * The forward records its flags in its image buffer, on the device and in stream order (no host synchronisation, so the
- * planned forms stay graph-capturable); every backward reads them from the image buffer it is given, so a backward
- * always differentiates the mode of the forward whose buffers it receives, and the backward entry points, workspace
- * sizes and GPSG_BWD_* flags are unchanged.  A reused planned image buffer carries the mode of its last forward.
- * maps: only _begin takes flags (the projection runs there); _finish / _finish_aux are unchanged.
- * Unknown flag bits return GPSG_E_INVALID before any other argument is checked. */
-#define GPSG_FWD_ANTIALIAS 1
-GPSG_API int gpsg_rasterize_forward_ex(const GpsgRasterSettings* settings, int device, void* stream, int P, int sh_M,
-                                       const float* means3D, const float* colors_precomp, const float* shs,
-                                       const float* opacities, const float* scales, const float* rotations,
-                                       const float* cov3D_precomp, float* out_color, float* out_depth, float* out_alpha,
-                                       int32_t* radii, gpsg_alloc_fn geom_alloc, void* geom_user,
-                                       gpsg_alloc_fn binning_alloc, void* binning_user, gpsg_alloc_fn image_alloc,
-                                       void* image_user, int32_t* num_rendered, int flags);
-GPSG_API int gpsg_rasterize_forward_maps_begin_ex(const GpsgRasterSettings* settings, int device, void* stream,
-                                                  int pixels_per_view, const uint8_t* const* valid,
-                                                  const float* const* xyz, const float* const* img,
-                                                  const float* const* rot, const float* const* scale,
-                                                  const float* const* opacity, int32_t* radii, gpsg_alloc_fn geom_alloc,
-                                                  void* geom_user, gpsg_alloc_fn image_alloc, void* image_user,
-                                                  uint32_t* totals_host, int flags);
-GPSG_API int gpsg_rasterize_forward_planned_ex(const GpsgRasterSettings* settings, int device, void* stream, int P,
-                                               const float* means3D, const float* colors_precomp, const float* opacities,
-                                               const float* scales, const float* rotations, const float* cov3D_precomp,
-                                               float* out_color, float* out_depth, float* out_alpha, int32_t* radii,
-                                               void* geom_buffer, void* binning_buffer, int64_t capacity_pairs,
-                                               void* image_buffer, uint32_t* status_host, int flags);
-GPSG_API int gpsg_rasterize_forward_maps_planned_ex(const GpsgRasterSettings* settings, int device, void* stream,
-                                                    int pixels_per_view, const uint8_t* const* valid,
-                                                    const float* const* xyz, const float* const* img,
-                                                    const float* const* rot, const float* const* scale,
-                                                    const float* const* opacity, float* out_color, float* out_depth,
-                                                    float* out_alpha, int32_t* radii, void* geom_buffer,
-                                                    void* binning_buffer, int64_t capacity_pairs, void* image_buffer,
-                                                    uint32_t* status_host, int flags);
+                                          float* const* dL_dscale, float* const* dL_dopacity, void* workspace,
+                                          int flags);
 
 /* ---- replaces _C.mark_visible : present[P] (uint8) = view-space z > 0.2 ---------------------- */
 GPSG_API int gpsg_mark_visible(int device, void* stream, int P, const float* means3D, const float* viewmatrix_host16,

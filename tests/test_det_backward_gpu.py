@@ -158,7 +158,7 @@ def test_det_c2_and_2048_full_size_parity():
     rc = _run(sc)
     from gps_gaussian_b200 import _lib
     record("2048:det_workspace", P=rc.P, N=rc.num_rendered,
-           bytes=int(_lib.lib.gpsg_rasterize_backward_workspace_bytes_ex(rc.P, rc.num_rendered, 1)))
+           bytes=int(_lib.lib.gpsg_rasterize_backward_workspace_bytes(rc.P, rc.num_rendered, 1, 0)))
     _det_parity(sc, 9, "2048", rc=rc)
 
 
@@ -185,9 +185,9 @@ def test_det_c2_reproducible_across_runs_and_concurrent_load():
     print(f"default backward: {differ} of 4 reruns differed from the first")
     for k in first:
         assert rel_err(_np(first[k]), _np(dflt[0][k])) <= 1e-5, k
-    ws = int(_lib.lib.gpsg_rasterize_backward_workspace_bytes_ex(rc.P, rc.num_rendered, 1))
+    ws = int(_lib.lib.gpsg_rasterize_backward_workspace_bytes(rc.P, rc.num_rendered, 1, 0))
     record("C2:det_workspace", P=rc.P, N=rc.num_rendered, bytes=ws)
-    assert ws <= int(_lib.lib.gpsg_rasterize_backward_workspace_bytes(rc.P)) + 320 * rc.num_rendered + 512
+    assert ws <= int(_lib.lib.gpsg_rasterize_backward_workspace_bytes(rc.P, 0, 0, 0)) + 320 * rc.num_rendered + 512
 
 
 # ---- 4. permutation invariance ----------------------------------------------------------------------------------------

@@ -10,6 +10,27 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
+def _c_kind(param):
+    """Kind of one parameter of a gpsg.h prototype: ptr (pointers and callbacks), i32, i64, size_t, f32, f64 or the name
+    of a struct passed by value."""
+    if "*" in param or param.split()[0] == "gpsg_alloc_fn":
+        return "ptr"
+    t = " ".join(w for w in param.split()[:-1] if w != "const")
+    return {"int": "i32", "int32_t": "i32", "int64_t": "i64", "size_t": "size_t", "float": "f32", "double": "f64"}.get(t, t)
+
+
+def _ctypes_kind(t):
+    """Kind of one ctypes argtype, in the terms of _c_kind."""
+    if t is C.c_void_p or t is C.c_char_p or issubclass(t, (C._Pointer, C._CFuncPtr)):
+        return "ptr"
+    kinds = [(C.c_int32, "i32"), (C.c_int64, "i64"), (C.c_size_t, "size_t"), (C.c_float, "f32"), (C.c_double, "f64")]
+    for ct, kind in kinds:
+        if t is ct:
+            return kind
+    assert issubclass(t, C.Structure), t
+    return "Gpsg" + t.__name__                     # the by-value structs: Mesh -> GpsgMesh, SeqLossArgs -> GpsgSeqLossArgs
+
+
 def test_library_exports_every_declared_symbol(built_lib):
     hdr = open(os.path.join(ROOT, "include", "gpsg.h")).read()
     declared = set(re.findall(r"GPSG_API\s+[\w\s\*]+?\b(gpsg_\w+)\s*\(", hdr))
@@ -20,6 +41,15 @@ def test_library_exports_every_declared_symbol(built_lib):
     from gps_gaussian_b200 import _lib
     assert set(_lib.EXPORTED) == declared
     assert _lib.lib.gpsg_version() == 90
+    # every prototype's parameter list against the argtypes the bindings set (a ctypes call with a wrong list passes
+    # garbage to the device instead of failing); jpeg declares its own functions on the same library
+    from gps_gaussian_b200 import jpeg  # noqa: F401
+    protos = re.findall(r"GPSG_API\s+[\w\s\*]+?\b(gpsg_\w+)\s*\(([^)]*)\)\s*;", re.sub(r"/\*.*?\*/", "", hdr, flags=re.S))
+    assert {name for name, _ in protos} == declared
+    for name, params in protos:
+        want = [] if params.strip() in ("", "void") else [_c_kind(p) for p in params.split(",")]
+        got = [_ctypes_kind(t) for t in getattr(_lib.lib, name).argtypes or []]
+        assert got == want, (name, want, got)
 
 
 def test_settings_struct_layout_matches_header(built_lib):
@@ -35,14 +65,14 @@ def test_argument_validation_without_gpu(built_lib):
     s = _lib.RasterSettings()
     s.image_height, s.image_width = 0, 16
     n = C.c_int32(0)
-    rc = _lib.lib.gpsg_rasterize_forward(C.byref(s), 0, None, 0, 0, None, None, None, None, None, None, None, None, None,
-                                         _lib.ALLOC_CB, None, _lib.ALLOC_CB, None, _lib.ALLOC_CB, None, C.byref(n))
+    rc = _lib.lib.gpsg_rasterize_forward(C.byref(s), 0, None, 0, 0, *([None] * 11), _lib.ALLOC_CB, None, _lib.ALLOC_CB,
+                                         None, _lib.ALLOC_CB, None, C.byref(n), 0)
     assert rc == -1 and b"image size" in _lib.lib.gpsg_last_error()
     with pytest.raises(_lib.GpsgError):
         _lib.check(rc, "x")
     assert _lib.lib.gpsg_corr_sampler_forward(0, None, 7, 1, 1, 1, 1, None, 0, 0, 0, None, 0, 4, None) == -1
     assert _lib.lib.gpsg_corr_sampler_forward(0, None, 0, 0, 4, 4, 4, None, 0, 0, 0, None, 0, 4, None) == 0   # empty batch: no-op
-    assert _lib.lib.gpsg_rasterize_backward_workspace_bytes(1000) >= 16000
+    assert _lib.lib.gpsg_rasterize_backward_workspace_bytes(1000, 0, 0, 0) >= 16000
     # the newer rows: shape / pointer validation happens before any CUDA call
     assert _lib.lib.gpsg_l1_ssim_forward(0, None, 0, 8, 8, None, None, 0.8, 0.2, None, None, None) == -1
     assert b"empty image" in _lib.lib.gpsg_last_error()
@@ -52,8 +82,8 @@ def test_argument_validation_without_gpu(built_lib):
     assert _lib.lib.gpsg_unproject_forward(0, None, 0, 16, None, None, 0, None, None, 3, None, None, None, None, None) == 0
     s.image_height = 16
     pp = (C.c_void_p * 2)()
-    rc = _lib.lib.gpsg_rasterize_forward_maps_planned(C.byref(s), 0, None, 0, pp, pp, pp, pp, pp, pp, None, None, None, None,
-                                                      1, None, None)
+    rc = _lib.lib.gpsg_rasterize_forward_maps_planned(C.byref(s), 0, None, 0, pp, pp, pp, pp, pp, pp, *([None] * 6), 1, None,
+                                                      None, 0)
     assert rc == -1 and b"pixels per view" in _lib.lib.gpsg_last_error()
 
 

@@ -1,5 +1,5 @@
-"""GPU: aux mode of the novel-view cache -- depth and alpha sweeps beside the image sweep, through the planned aux
-forwards (gpsg_rasterize_forward_planned_aux / _maps_planned_aux), including the overflow re-render and the exact
+"""GPU: aux mode of the novel-view cache -- depth and alpha sweeps beside the image sweep, through the planned forwards'
+out_depth / out_alpha (gpsg_rasterize_forward_planned / _maps_planned), including the overflow re-render and the exact
 fallback for over-long tile lists."""
 import pytest
 import torch

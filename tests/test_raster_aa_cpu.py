@@ -17,8 +17,8 @@ from helpers import oracle_forward, record
 import aa_reference as aar
 
 AA = 1
-FWD_EX = ("gpsg_rasterize_forward_ex", "gpsg_rasterize_forward_maps_begin_ex", "gpsg_rasterize_forward_planned_ex",
-          "gpsg_rasterize_forward_maps_planned_ex")
+FWD_FLAGS = ("gpsg_rasterize_forward", "gpsg_rasterize_forward_maps_begin", "gpsg_rasterize_forward_planned",
+             "gpsg_rasterize_forward_maps_planned")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -26,7 +26,7 @@ def test_aa_symbols_exported(built_lib):
     from gps_gaussian_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "gpsg.h")).read()
     assert "#define GPSG_FWD_ANTIALIAS 1" in hdr and _lib.FWD_ANTIALIAS == 1
-    for name in FWD_EX:
+    for name in FWD_FLAGS:
         assert name in _lib.EXPORTED and hasattr(_lib.lib, name)
         assert re.search(r"GPSG_API int %s\(" % name, hdr)
     assert _lib.lib.gpsg_version() == 90
@@ -36,14 +36,14 @@ def test_aa_symbols_exported(built_lib):
 def _calls(L, s, p, pp, flags):
     alloc = _lib_alloc()
     return {
-        "gpsg_rasterize_forward_ex": lambda: L.gpsg_rasterize_forward_ex(s, 0, None, 4, 0, p, p, None, p, p, p, None, p, None,
-                                                                         None, p, alloc, None, alloc, None, alloc, None,
-                                                                         None, flags),
-        "gpsg_rasterize_forward_maps_begin_ex": lambda: L.gpsg_rasterize_forward_maps_begin_ex(
+        "gpsg_rasterize_forward": lambda: L.gpsg_rasterize_forward(s, 0, None, 4, 0, p, p, None, p, p, p, None, p, None,
+                                                                   None, p, alloc, None, alloc, None, alloc, None, None,
+                                                                   flags),
+        "gpsg_rasterize_forward_maps_begin": lambda: L.gpsg_rasterize_forward_maps_begin(
             s, 0, None, 4, *([pp] * 6), p, alloc, None, alloc, None, p, flags),
-        "gpsg_rasterize_forward_planned_ex": lambda: L.gpsg_rasterize_forward_planned_ex(
+        "gpsg_rasterize_forward_planned": lambda: L.gpsg_rasterize_forward_planned(
             s, 0, None, 4, p, p, p, p, p, None, p, None, None, p, p, p, 16, p, None, flags),
-        "gpsg_rasterize_forward_maps_planned_ex": lambda: L.gpsg_rasterize_forward_maps_planned_ex(
+        "gpsg_rasterize_forward_maps_planned": lambda: L.gpsg_rasterize_forward_maps_planned(
             s, 0, None, 4, *([pp] * 6), p, None, None, p, p, p, 16, p, None, flags),
     }
 
@@ -54,7 +54,7 @@ def _lib_alloc():
 
 
 def test_aa_unknown_forward_flags_refused_first(built_lib):
-    """Every _ex forward refuses unknown bits before checking anything else (NULL settings included)."""
+    """Every forward that takes flags refuses unknown bits before checking anything else (NULL settings included)."""
     from gps_gaussian_b200 import _lib
     L = _lib.lib
     buf = (C.c_float * 1024)()
@@ -67,7 +67,7 @@ def test_aa_unknown_forward_flags_refused_first(built_lib):
 
 
 def test_aa_null_and_empty_as_plain(built_lib):
-    """With GPSG_FWD_ANTIALIAS the argument checks are those of the plain forwards (same codes, same messages)."""
+    """With GPSG_FWD_ANTIALIAS the argument checks are those of flags = 0 (same codes, same messages)."""
     from gps_gaussian_b200 import _lib
     L = _lib.lib
     buf = (C.c_float * 1024)()
@@ -81,20 +81,20 @@ def test_aa_null_and_empty_as_plain(built_lib):
     alloc = _lib.ALLOC_CB
     for flags in (0, AA):
         # planned forwards need P > 0; the maps forwards need pixels_per_view > 0; aux outputs both or neither
-        assert L.gpsg_rasterize_forward_planned_ex(C.byref(s), 0, None, 0, p, p, p, p, p, None, p, None, None, p, p, p, 16,
-                                                   p, None, flags) == -1
+        assert L.gpsg_rasterize_forward_planned(C.byref(s), 0, None, 0, p, p, p, p, p, None, p, None, None, p, p, p, 16,
+                                                p, None, flags) == -1
         assert b"P > 0" in L.gpsg_last_error()
-        assert L.gpsg_rasterize_forward_maps_planned_ex(C.byref(s), 0, None, 0, *([pp] * 6), p, None, None, p, p, p, 16, p,
-                                                        None, flags) == -1
+        assert L.gpsg_rasterize_forward_maps_planned(C.byref(s), 0, None, 0, *([pp] * 6), p, None, None, p, p, p, 16, p,
+                                                     None, flags) == -1
         assert b"pixels per view" in L.gpsg_last_error()
-        assert L.gpsg_rasterize_forward_maps_begin_ex(C.byref(s), 0, None, 0, *([pp] * 6), p, alloc, None, alloc, None, p,
-                                                      flags) == -1
+        assert L.gpsg_rasterize_forward_maps_begin(C.byref(s), 0, None, 0, *([pp] * 6), p, alloc, None, alloc, None, p,
+                                                   flags) == -1
         assert b"pixels per view" in L.gpsg_last_error()
-        assert L.gpsg_rasterize_forward_ex(C.byref(s), 0, None, 4, 0, p, p, None, p, p, p, None, p, p, None, p, alloc, None,
-                                           alloc, None, alloc, None, None, flags) == -1
+        assert L.gpsg_rasterize_forward(C.byref(s), 0, None, 4, 0, p, p, None, p, p, p, None, p, p, None, p, alloc, None,
+                                        alloc, None, alloc, None, None, flags) == -1
         assert b"out_depth and out_alpha" in L.gpsg_last_error()
-        assert L.gpsg_rasterize_forward_ex(C.byref(s), 0, None, -1, 0, *([None] * 7), p, None, None, None, alloc, None,
-                                           alloc, None, alloc, None, None, flags) == -1
+        assert L.gpsg_rasterize_forward(C.byref(s), 0, None, -1, 0, *([None] * 7), p, None, None, None, alloc, None,
+                                        alloc, None, alloc, None, None, flags) == -1
         assert b"P < 0" in L.gpsg_last_error()
 
 

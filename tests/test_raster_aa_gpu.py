@@ -1,8 +1,6 @@
 """GPU: anti-aliasing (GPSG_FWD_ANTIALIAS) -- the device against the fp32 / fp64 oracles fed with o * rho
 (tests/aa_reference.py), the discrete state against the forward without it, the mode carried by the saved state, and
 every entry point and Python layer against each other."""
-import ctypes as C
-
 import numpy as np
 import pytest
 import torch
@@ -154,34 +152,6 @@ def test_aa_mode_follows_state():
     assert float((g_aa["dL_dopacity"] - g_off["dL_dopacity"]).abs().max()) > 1e-3 * float(g_off["dL_dopacity"].abs().max())
 
 
-def test_aa_flags_zero_equals_old_entry_points():
-    """flags = 0 through the _ex forward is the old gpsg_rasterize_forward: images, radii, and DET gradients bit for bit."""
-    sc = SCENES["C1"]()
-    new = RasterCall(sc)
-    new.forward()
-    old = RasterCall(sc, dev_inputs=new.inp)
-    i = old._inputs()
-    idx, stream = _lib.device_stream(old.device)
-    n = C.c_int32(0)
-    _lib.begin_alloc(old.device)
-    try:
-        rc = _lib.lib.gpsg_rasterize_forward(C.byref(old.settings), idx, stream, old.P, 0, _lib._ptr(i["means3D"]),
-                                             _lib._ptr(i["colors_precomp"]), None, _lib._ptr(i["opacities"]),
-                                             _lib._ptr(i["scales"]), _lib._ptr(i["rotations"]), None, _lib._ptr(old.color),
-                                             _lib._ptr(old.radii), _lib.ALLOC_CB, C.c_void_p(1), _lib.ALLOC_CB,
-                                             C.c_void_p(2), _lib.ALLOC_CB, C.c_void_p(3), C.byref(n))
-    finally:
-        bufs = _lib.end_alloc()
-    _lib.check(rc, "gpsg_rasterize_forward")
-    old.num_rendered, old.bufs = int(n.value), (bufs.get(1), bufs.get(2), bufs.get(3))
-    assert torch.equal(old.color, new.color) and torch.equal(old.radii, new.radii)
-    g = torch.from_numpy(np.random.default_rng(7).standard_normal((3, old.H, old.W)).astype(np.float32)).cuda()
-    a = {k: v.clone() for k, v in old.backward(g, deterministic=True).items() if v is not None}
-    b = new.backward(g, deterministic=True)
-    for k in a:
-        assert torch.equal(a[k], b[k]), k
-
-
 def test_aa_paths_bit_identical():
     """With AA: exact, planned, graph replay and the drop-in GaussianRasterizer give the same image bit for bit."""
     import diff_gaussian_rasterization as dgr
@@ -265,7 +235,7 @@ def test_aa_pts2render_and_novel_views():
 
 
 def test_aa_empty_scene_as_plain():
-    """P = 0 through gpsg_rasterize_forward_ex with GPSG_FWD_ANTIALIAS: the background, exactly as the plain forward."""
+    """P = 0 through gpsg_rasterize_forward with GPSG_FWD_ANTIALIAS: the background, exactly as with flags = 0."""
     sc = synth.random_cube_scene(10, 64, seed=1, bg=(0.2, 0.4, 0.6))
     sc = dict(sc, **{k: sc[k][:0] for k in ("means3D", "colors", "opacity", "scales", "rots")})
     off, aa = _pair(sc)

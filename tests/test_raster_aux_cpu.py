@@ -16,10 +16,9 @@ from oracle import raster_torch64 as rt
 from helpers import oracle_forward
 
 DET = 1
-AUX_SYMBOLS = ("gpsg_rasterize_forward_aux", "gpsg_rasterize_forward_maps_finish_aux", "gpsg_rasterize_forward_planned_aux",
-               "gpsg_rasterize_forward_maps_planned_aux", "gpsg_rasterize_backward_aux_workspace_bytes",
-               "gpsg_rasterize_backward_aux", "gpsg_rasterize_backward_maps_aux_workspace_bytes",
-               "gpsg_rasterize_backward_maps_aux")
+AUX_SYMBOLS = ("gpsg_rasterize_forward", "gpsg_rasterize_forward_maps_finish", "gpsg_rasterize_forward_planned",
+               "gpsg_rasterize_forward_maps_planned", "gpsg_rasterize_backward_workspace_bytes", "gpsg_rasterize_backward",
+               "gpsg_rasterize_backward_maps_workspace_bytes", "gpsg_rasterize_backward_maps")
 SIZES = [(0, 0), (1, 0), (1, 1), (7, 3), (1000, 5000), (499_400, 1_307_000), (2_000_000, 30_000_000)]
 
 
@@ -35,19 +34,14 @@ def test_aux_workspace_sizes(built_lib):
     it the partial sums are 8 x 10 floats per pair: 321 B per pair plus alignment."""
     from gps_gaussian_b200 import _lib
     L = _lib.lib
-    for P, N in SIZES:
-        assert L.gpsg_rasterize_backward_aux_workspace_bytes(P, N, 0) == L.gpsg_rasterize_backward_workspace_bytes_ex(P, N, 0)
-        assert L.gpsg_rasterize_backward_maps_aux_workspace_bytes(P, N, 0) == \
-            L.gpsg_rasterize_backward_maps_workspace_bytes_ex(P, N, 0)
-        for aux_fn, base_fn in ((L.gpsg_rasterize_backward_aux_workspace_bytes, L.gpsg_rasterize_backward_workspace_bytes),
-                                (L.gpsg_rasterize_backward_maps_aux_workspace_bytes,
-                                 L.gpsg_rasterize_backward_maps_workspace_bytes)):
-            extra = aux_fn(P, N, DET) - base_fn(P)
-            assert 321 * N <= extra <= 352 * N + 512, (P, N, extra)
-    for flags in (2, 4, -1):
-        assert L.gpsg_rasterize_backward_aux_workspace_bytes(10, 5, flags) == 0
-        assert L.gpsg_rasterize_backward_maps_aux_workspace_bytes(10, 5, flags) == 0
-    assert L.gpsg_rasterize_backward_aux_workspace_bytes(10, -1, DET) == 0
+    for ws in (L.gpsg_rasterize_backward_workspace_bytes, L.gpsg_rasterize_backward_maps_workspace_bytes):
+        for P, N in SIZES:
+            assert ws(P, N, 0, 1) == ws(P, N, 0, 0) == ws(P, 0, 0, 0), (ws.__name__, P, N)
+            extra = ws(P, N, DET, 1) - ws(P, 0, 0, 0)
+            assert 321 * N <= extra <= 352 * N + 512, (ws.__name__, P, N, extra)
+        for flags in (2, 4, -1):
+            assert ws(10, 5, flags, 1) == 0
+        assert ws(10, -1, DET, 1) == 0
 
 
 def test_aux_argument_validation_without_gpu(built_lib):
@@ -60,35 +54,35 @@ def test_aux_argument_validation_without_gpu(built_lib):
     alloc = _lib.ALLOC_CB
     # forward: out_depth / out_alpha both NULL or both set
     for d, a in ((p, None), (None, p)):
-        assert L.gpsg_rasterize_forward_aux(C.byref(s), 0, None, 0, 0, *([None] * 7), p, d, a, None, alloc, None, alloc,
-                                            None, alloc, None, None) == -1
+        assert L.gpsg_rasterize_forward(C.byref(s), 0, None, 0, 0, *([None] * 7), p, d, a, None, alloc, None, alloc,
+                                        None, alloc, None, None, 0) == -1
         assert b"out_depth and out_alpha" in L.gpsg_last_error()
-        assert L.gpsg_rasterize_forward_planned_aux(C.byref(s), 0, None, 4, p, p, p, p, p, None, p, d, a, p, p, p, 16,
-                                                    p, None) == -1
+        assert L.gpsg_rasterize_forward_planned(C.byref(s), 0, None, 4, p, p, p, p, p, None, p, d, a, p, p, p, 16,
+                                                p, None, 0) == -1
         assert b"out_depth and out_alpha" in L.gpsg_last_error()
         pp = (C.c_void_p * 2)(p, p)
-        assert L.gpsg_rasterize_forward_maps_finish_aux(C.byref(s), 0, None, 4, *([pp] * 6), p, d, a, p, p, p, alloc, None,
-                                                        p, None) == -1
+        assert L.gpsg_rasterize_forward_maps_finish(C.byref(s), 0, None, 4, *([pp] * 6), p, d, a, p, p, p, alloc, None,
+                                                    p, None) == -1
         assert b"out_depth and out_alpha" in L.gpsg_last_error()
-        assert L.gpsg_rasterize_forward_maps_planned_aux(C.byref(s), 0, None, 4, *([pp] * 6), p, d, a, p, p, p, 16, p,
-                                                         None) == -1
+        assert L.gpsg_rasterize_forward_maps_planned(C.byref(s), 0, None, 4, *([pp] * 6), p, d, a, p, p, p, 16, p,
+                                                     None, 0) == -1
         assert b"out_depth and out_alpha" in L.gpsg_last_error()
     # backward: dL_dout_depth / dL_dout_alpha both NULL or both set; unknown flags refused first
     for d, a in ((p, None), (None, p)):
         for flags in (0, DET):
-            assert L.gpsg_rasterize_backward_aux(C.byref(s), 0, None, 10, 0, 5, *([None] * 12), d, a, *([None] * 9),
-                                                 flags) == -1
+            assert L.gpsg_rasterize_backward(C.byref(s), 0, None, 10, 0, 5, *([None] * 12), d, a, *([None] * 9),
+                                             flags) == -1
             assert b"dL_dout_depth and dL_dout_alpha" in L.gpsg_last_error()
-            assert L.gpsg_rasterize_backward_maps_aux(C.byref(s), 0, None, 8, 5, *([None] * 6), *([None] * 5), d, a,
-                                                      *([None] * 5), None, flags) == -1
+            assert L.gpsg_rasterize_backward_maps(C.byref(s), 0, None, 8, 5, *([None] * 6), *([None] * 5), d, a,
+                                                  *([None] * 5), None, flags) == -1
             assert b"dL_dout_depth and dL_dout_alpha" in L.gpsg_last_error()
     for flags in (2, 4, 1 | 8):
-        assert L.gpsg_rasterize_backward_aux(C.byref(s), 0, None, 10, 0, 5, *([None] * 12), p, p, *([None] * 9), flags) == -1
+        assert L.gpsg_rasterize_backward(C.byref(s), 0, None, 10, 0, 5, *([None] * 12), p, p, *([None] * 9), flags) == -1
         assert b"flag" in L.gpsg_last_error()
     # P = 0: nothing to do, in both modes; missing inputs otherwise
     for flags in (0, DET):
-        assert L.gpsg_rasterize_backward_aux(C.byref(s), 0, None, 0, 0, 0, *([None] * 12), p, p, *([None] * 9), flags) == 0
-        assert L.gpsg_rasterize_backward_aux(C.byref(s), 0, None, 10, 0, 5, *([None] * 12), p, p, *([None] * 9), flags) == -1
+        assert L.gpsg_rasterize_backward(C.byref(s), 0, None, 0, 0, 0, *([None] * 12), p, p, *([None] * 9), flags) == 0
+        assert L.gpsg_rasterize_backward(C.byref(s), 0, None, 10, 0, 5, *([None] * 12), p, p, *([None] * 9), flags) == -1
         assert b"NULL" in L.gpsg_last_error()
 
 

@@ -1,5 +1,5 @@
-"""GPU: aux mode of the rasterizer -- expected depth and alpha beside the colour image (gpsg_rasterize_forward_aux /
-gpsg_rasterize_backward_aux and the Python layers above them).
+"""GPU: aux mode of the rasterizer -- expected depth and alpha beside the colour image (the out_depth / out_alpha outputs
+of gpsg_rasterize_forward, the aux gradients of gpsg_rasterize_backward and the Python layers above them).
 
 Depth is a fourth colour channel (colour z, background 0) and alpha = 1 - T_final is 1 + the colour image of a scene with
 black Gaussians on the background (-1, 0, 0).  The oracles therefore check aux mode with their existing entry points:

@@ -74,8 +74,8 @@ def run(aux, aa=False):
     out["total_us_per_view"] = round(e0.elapsed_time(e1) * 1e3 / (a.reps * len(calls)), 1)
     out["N_dup_mean"] = sum(c.num_rendered for c in calls) / len(calls)
     flags = _lib.BWD_DETERMINISTIC if a.deterministic else 0
-    size = _lib.lib.gpsg_rasterize_backward_aux_workspace_bytes if aux else _lib.lib.gpsg_rasterize_backward_workspace_bytes_ex
-    out["bwd_workspace_bytes_mean"] = sum(size(c.P, c.num_rendered, flags) for c in calls) / len(calls)
+    size = _lib.lib.gpsg_rasterize_backward_workspace_bytes
+    out["bwd_workspace_bytes_mean"] = sum(size(c.P, c.num_rendered, flags, int(aux)) for c in calls) / len(calls)
     out["aux"] = aux
     out["antialias"] = aa
     out["gpu"] = torch.cuda.get_device_name(0)
