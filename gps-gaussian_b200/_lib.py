@@ -171,6 +171,9 @@ class SeqLossArgs(C.Structure):
 
 
 SEQ_LOSS_MAX_PRED = 32    # GPSG_SEQ_LOSS_MAX_PRED (include/gpsg.h)
+# GpsgGsHeadWeights field order (include/gpsg.h)
+GS_HEAD_PARAMS = ("out_w", "out_b", "rot_w1", "rot_b1", "rot_w2", "rot_b2", "scale_w1", "scale_b1", "scale_w2",
+                  "scale_b2", "opacity_w1", "opacity_b1", "opacity_w2", "opacity_b2")
 lib.gpsg_convex_upsample_forward.restype = _i
 lib.gpsg_convex_upsample_forward.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]
 lib.gpsg_convex_upsample_backward_workspace_bytes.restype = _sz
@@ -183,6 +186,17 @@ lib.gpsg_sequence_loss_forward.restype = _i
 lib.gpsg_sequence_loss_forward.argtypes = [_i, _vp, SeqLossArgs, _vp, _vp]
 lib.gpsg_sequence_loss_backward.restype = _i
 lib.gpsg_sequence_loss_backward.argtypes = [_i, _vp, SeqLossArgs, _vp, _vp]
+
+
+class GsHeadWeights(C.Structure):
+    """GpsgGsHeadWeights (include/gpsg.h), passed by value: the 14 device pointers of the regressor tail's weights."""
+    _fields_ = [(n, C.c_void_p) for n in GS_HEAD_PARAMS]
+
+
+lib.gpsg_gs_head_workspace_bytes.restype = _sz
+lib.gpsg_gs_head_workspace_bytes.argtypes = [_i, _i, _i]
+lib.gpsg_gs_head_forward.restype = _i
+lib.gpsg_gs_head_forward.argtypes = [_i, _vp, _i, _i, _i] + [_vp] * 6 + [GsHeadWeights, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -205,7 +219,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_convex_upsample_backward", "gpsg_sequence_loss_workspace_bytes", "gpsg_sequence_loss_forward",
             "gpsg_sequence_loss_backward", "gpsg_mesh_render_workspace_bytes", "gpsg_mesh_render", "gpsg_jpeg_parse",
             "gpsg_jpeg_decode_workspace_bytes", "gpsg_jpeg_decode", "gpsg_jpeg_encode_max_bytes",
-            "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode"]
+            "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode", "gpsg_gs_head_workspace_bytes",
+            "gpsg_gs_head_forward"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

@@ -35,6 +35,7 @@ SOURCES = {
     "point_splat.cu": [],
     "rectify.cu": ["-fmad=false"],
     "flow_head.cu": [],
+    "gs_head.cu": [],
     "mesh_render.cu": ["-fmad=false"],
     "jpeg_decode.cu": [],
     "jpeg_encode.cu": [],

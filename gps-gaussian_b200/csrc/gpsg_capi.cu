@@ -910,6 +910,25 @@ int gpsg_sequence_loss_backward(int device, void* stream_, GpsgSeqLossArgs args,
     return launch_sequence_loss_bwd(args, grad_loss, stats, (cudaStream_t)stream_);
 }
 
+size_t gpsg_gs_head_workspace_bytes(int B, int H, int W) {
+    return (B > 0 && H > 0 && W > 0) ? gs_head_workspace_bytes(B, H, W) : 0;
+}
+
+int gpsg_gs_head_forward(int device, void* stream_, int B, int H, int W, const float* src, const float* img,
+                         const float* depth, float* rot, float* scale, float* opacity, GpsgGsHeadWeights weights,
+                         void* workspace) {
+    GPSG_REQUIRE(B >= 0 && H >= 0 && W >= 0 && H % 2 == 0 && W % 2 == 0, "gs_head: H and W must be even, sizes >= 0");
+    GPSG_REQUIRE(H <= 65536 && W <= 65536 && (int64_t)B * H * W * 32 < (int64_t(1) << 40), "gs_head: too large");
+    if ((int64_t)B * H * W == 0) return GPSG_OK;
+    GPSG_REQUIRE(src && img && depth && rot && scale && opacity && workspace, "NULL pointer");
+    const float* const* w = &weights.out_w;
+    for (int i = 0; i < 14; ++i) GPSG_REQUIRE(w[i], "gs_head: NULL weight pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 16 == 0, "gs_head: workspace must be 16-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_gs_head_fwd(device, B, H, W, src, img, depth, weights, rot, scale, opacity, workspace,
+                              (cudaStream_t)stream_);
+}
+
 int gpsg_set_corr_build(int mode) {
     set_corr_build_mode(mode);
     return GPSG_OK;

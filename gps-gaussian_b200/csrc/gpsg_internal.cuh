@@ -262,6 +262,10 @@ int launch_convex_upsample_bwd(int dtype, int f, int N, int D, int H, int W, con
                                const float* grad_out, void* grad_mask, float* grad_flow, void* workspace,
                                cudaStream_t stream);
 size_t sequence_loss_workspace_bytes();
+size_t gs_head_workspace_bytes(int B, int H, int W);
+int launch_gs_head_fwd(int device, int B, int H, int W, const float* src, const float* img, const float* depth,
+                       const GpsgGsHeadWeights& wt, float* rot, float* scale, float* opacity, void* workspace,
+                       cudaStream_t stream);
 int launch_sequence_loss_fwd(const GpsgSeqLossArgs& a, float* stats, void* workspace, cudaStream_t stream);
 int launch_sequence_loss_bwd(const GpsgSeqLossArgs& a, const float* grad_loss, const float* stats, cudaStream_t stream);
 // corr.cu

@@ -1,0 +1,150 @@
+"""The full-resolution tail of the Gaussian-parameter regressor on sm_90a (csrc/gs_head.cu), forward only.
+
+`GSRegresser.forward` (reference lib/gs_parm_network.py) runs at 1/8 to 1/2 resolution up to `decoder1`; its last step
+upsamples the 48-channel decoder output x2, concatenates the image and the depth, and runs `out_conv` and the rot /
+scale / opacity heads at full resolution, in fp32.  `gs_head` does that step in two TF32 warpgroup-MMA (wgmma)
+kernels in place of the upsample / cat / seven convolutions / ReLU / activation chain, reading the half-resolution
+decoder output, the image and the depth and writing the three maps.
+
+`make_regresser_forward(orig)` is `GSRegresser.forward` that hands the decoder1 output to `gs_head` when autograd is off
+(the inference scripts and the stage-2 evaluation run under `torch.no_grad()`) and `supported(...)` holds; with grad
+enabled (the training step), under autocast, or for inputs the kernels do not cover, it calls `orig`, the reference's
+own method, unchanged.  The maps differ from cuDNN's TF32 convolutions by TF32 re-association; see include/gpsg.h for
+the exact semantics.
+"""
+import ctypes as C
+
+import torch
+from torch import nn
+
+from . import _lib
+
+SRC_C, RGB_C, DEPTH_C, HEAD_C = 48, 3, 1, 32
+
+
+def _p(t):
+    return C.c_void_p(t.data_ptr())
+
+
+def params_of(regresser):
+    """The 14 weight / bias tensors of the tail, in GpsgGsHeadWeights order (`_lib.GS_HEAD_PARAMS`)."""
+    r = regresser
+    return (r.out_conv.weight, r.out_conv.bias,
+            r.rot_head[0].weight, r.rot_head[0].bias, r.rot_head[2].weight, r.rot_head[2].bias,
+            r.scale_head[0].weight, r.scale_head[0].bias, r.scale_head[2].weight, r.scale_head[2].bias,
+            r.opacity_head[0].weight, r.opacity_head[0].bias, r.opacity_head[2].weight, r.opacity_head[2].bias)
+
+
+PARAM_SHAPES = ((HEAD_C, SRC_C + RGB_C + DEPTH_C, 3, 3), (HEAD_C,),
+                (HEAD_C, HEAD_C, 3, 3), (HEAD_C,), (4, HEAD_C, 1, 1), (4,),
+                (HEAD_C, HEAD_C, 3, 3), (HEAD_C,), (3, HEAD_C, 1, 1), (3,),
+                (HEAD_C, HEAD_C, 3, 3), (HEAD_C,), (1, HEAD_C, 1, 1), (1,))
+
+
+def _conv(m, cin, cout, k):
+    return (type(m) is nn.Conv2d and m.in_channels == cin and m.out_channels == cout and m.kernel_size == (k, k)
+            and m.stride == (1, 1) and m.padding == ((k - 1) // 2,) * 2 and m.dilation == (1, 1) and m.groups == 1
+            and m.padding_mode == "zeros" and m.bias is not None)
+
+
+def _module_supported(r):
+    try:
+        heads = (r.rot_head, r.scale_head, r.opacity_head)
+        if list(getattr(r, "decoder_dims", ()))[:1] != [SRC_C] or getattr(r, "head_dim", None) != HEAD_C:
+            return False
+        up = r.up
+        if not (type(up) is nn.Upsample and up.scale_factor in (2, 2.0, (2.0, 2.0)) and up.mode == "bilinear"
+                and not up.align_corners and up.size is None):
+            return False
+        if not (_conv(r.out_conv, SRC_C + RGB_C + DEPTH_C, HEAD_C, 3) and type(r.out_relu) is nn.ReLU):
+            return False
+        tails = ((4, ()), (3, (nn.Softplus,)), (1, (nn.Sigmoid,)))
+        for head, (n, act) in zip(heads, tails):
+            if type(head) is not nn.Sequential or len(head) != 3 + len(act):
+                return False
+            if not (_conv(head[0], HEAD_C, HEAD_C, 3) and type(head[1]) is nn.ReLU and _conv(head[2], HEAD_C, n, 1)):
+                return False
+            if act and type(head[3]) is not act[0]:
+                return False
+        sp = r.scale_head[3]
+        return sp.beta == 100 and sp.threshold == 20
+    except (AttributeError, IndexError, TypeError):
+        return False
+
+
+def _tensors_supported(dev, *ts):
+    return all(torch.is_tensor(t) and t.is_cuda and t.device == dev and t.dtype == torch.float32 for t in ts)
+
+
+def supported(regresser, img, depth, up_src):
+    """Whether `gs_head` runs these inputs: CUDA fp32 tensors on one device, img [B,3,H,W] and depth [B,1,H,W] with H and W
+    even, up_src [B,48,H/2,W/2] (None skips its check), fp32 weights there too, and a module whose tail has the expected
+    layers (decoder_dims[0] == 48, head_dim == 32, 3x3 / 1x1 Conv2d with bias and zero padding, bilinear x2 Upsample
+    without align_corners, Softplus(beta=100, threshold=20), Sigmoid)."""
+    if not (torch.is_tensor(img) and img.is_cuda and _module_supported(regresser)):
+        return False
+    dev = img.device
+    if not _tensors_supported(dev, img, depth, *params_of(regresser)):
+        return False
+    if img.dim() != 4 or depth.dim() != 4:
+        return False
+    B, c, H, W = img.shape
+    if c != RGB_C or tuple(depth.shape) != (B, DEPTH_C, H, W) or H % 2 or W % 2:
+        return False
+    if up_src is not None:
+        return _tensors_supported(dev, up_src) and tuple(up_src.shape) == (B, SRC_C, H // 2, W // 2)
+    return True
+
+
+def run(up_src, img, depth, params):
+    """The kernels on raw tensors: up_src [B,48,H/2,W/2], img [B,3,H,W], depth [B,1,H,W] and the 14 parameters in
+    `params_of` order, all CUDA fp32 on one device -> (rot [B,4,H,W], scale [B,3,H,W], opacity [B,1,H,W])."""
+    B, _, H, W = (int(s) for s in img.shape)
+    dev = img.device
+    if not (_tensors_supported(dev, up_src, img, depth, *params) and tuple(up_src.shape) == (B, SRC_C, H // 2, W // 2)
+            and tuple(depth.shape) == (B, DEPTH_C, H, W) and img.shape[1] == RGB_C and H % 2 == 0 and W % 2 == 0
+            and all(tuple(p.shape) == s for p, s in zip(params, PARAM_SHAPES)) and len(params) == len(PARAM_SHAPES)):
+        raise RuntimeError(
+            f"gs_head (gpsg): needs CUDA fp32 up_src [B,48,H/2,W/2], img [B,3,H,W], depth [B,1,H,W] with even H, W and "
+            f"the 14 tail parameters on one device; got up_src {tuple(up_src.shape)} {up_src.dtype} {up_src.device}, "
+            f"img {tuple(img.shape)} {img.dtype} {img.device}, depth {tuple(depth.shape)} {depth.dtype}")
+    with torch.no_grad():
+        src, im, dp = (t.detach().contiguous() for t in (up_src, img, depth))
+        ps = [p.detach().contiguous() for p in params]
+        rot = torch.empty((B, 4, H, W), dtype=torch.float32, device=dev)
+        scale = torch.empty((B, 3, H, W), dtype=torch.float32, device=dev)
+        opacity = torch.empty((B, 1, H, W), dtype=torch.float32, device=dev)
+        ws = torch.empty(max(int(_lib.lib.gpsg_gs_head_workspace_bytes(B, H, W)) // 4, 1), dtype=torch.float32,
+                         device=dev)
+        wt = _lib.GsHeadWeights(*[p.data_ptr() for p in ps])
+        with torch.cuda.device(dev):
+            rc = _lib.lib.gpsg_gs_head_forward(*_lib.device_stream(dev), B, H, W, _p(src), _p(im), _p(dp), _p(rot),
+                                               _p(scale), _p(opacity), wt, _p(ws))
+        _lib.check(rc, "gpsg_gs_head_forward")
+    return rot, scale, opacity
+
+
+def gs_head(up_src, img, depth, regresser):
+    """(rot [B,4,H,W], scale [B,3,H,W], opacity [B,1,H,W]) of `regresser`'s tail from its decoder1 output up_src
+    [B,48,H/2,W/2], the image [B,3,H,W] and the depth [B,1,H,W]: forward only, no autograd."""
+    if not supported(regresser, img, depth, up_src):
+        raise RuntimeError("gs_head (gpsg): inputs or module not supported; see gs_head.supported")
+    return run(up_src, img, depth, params_of(regresser))
+
+
+def make_regresser_forward(orig):
+    """`GSRegresser.forward` with the full-resolution tail on the kernels when grad is disabled and the inputs are
+    supported; otherwise `orig`, the reference's own method."""
+    def forward(self, img, depth, img_feat):
+        if torch.is_grad_enabled() or torch.is_autocast_enabled() or not supported(self, img, depth, None):
+            return orig(self, img, depth, img_feat)
+        img_feat1, img_feat2, img_feat3 = img_feat
+        depth_feat1, depth_feat2, depth_feat3 = self.depth_encoder(depth)
+        x = self.decoder3(torch.cat([img_feat3, depth_feat3], dim=1))
+        x = self.decoder2(torch.cat([self.up(x), img_feat2, depth_feat2], dim=1))
+        x = self.decoder1(torch.cat([self.up(x), img_feat1, depth_feat1], dim=1))
+        if not supported(self, img, depth, x):        # e.g. fp16 image features: the decoders ran in fp16
+            return orig(self, img, depth, img_feat)
+        return run(x, img, depth, params_of(self))
+    forward.__doc__ = orig.__doc__
+    return forward

@@ -49,6 +49,16 @@ Inputs the kernels do not cover (CPU tensors, other dtypes or factors) reach the
 differ from the op chain's by fp32 re-association and by where fp16 rounding falls in the backward, which is why the
 switch is opt-in.  Unset or any other value hooks neither.
 
+`GPSG_GS_HEAD=1`, read once by `install()`, also hooks `lib.gs_parm_network` and rebinds
+
+    GSRegresser.forward -> gs_head.make_regresser_forward (a class method, kept in _ORIG_METHODS)
+
+so that with autograd off (test_view_interp.py, test_real_data.py, train_stage2.py's run_eval) the regressor's
+full-resolution tail, from the decoder1 output to the rot / scale / opacity maps, runs on the TF32 tensor-core kernels
+(gps_gaussian_b200.gs_head, csrc/gs_head.cu).  With grad enabled (the training step), under autocast or for inputs the
+kernels do not cover, the reference's own forward runs unchanged.  The maps differ from cuDNN's by TF32 re-association,
+which is why the switch is opt-in.  Unset or any other value leaves `lib.gs_parm_network` alone.
+
 `taichi_three` and its submodules always resolve to the stand-in in dropin/taichi_three (the dataset renderer on
 csrc/mesh_render.cu).  `python prepare_data/render_data.py` puts prepare_data/ first on sys.path, where the reference's
 own package, which cannot import without Taichi, would shadow anything on PYTHONPATH.
@@ -66,6 +76,7 @@ _RECTIFY = False      # GPSG_RECTIFY=1 at install()
 _FLOW_HEAD = False    # GPSG_FLOW_HEAD=1 at install()
 _DECODE = False       # GPSG_DECODE=1 at install()
 _ENCODE = False       # GPSG_ENCODE=1 at install()
+_GS_HEAD = False      # GPSG_GS_HEAD=1 at install()
 
 
 def _set(mod, attr, new):
@@ -170,6 +181,15 @@ def _patch_loss(mod):
     user = sys.modules.get("lib.network")                     # `from lib.loss import sequence_loss` copies the binding
     if user is not None and hasattr(user, "sequence_loss"):
         _set(user, "sequence_loss", flow_head.sequence_loss)
+
+
+def _patch_regresser(mod):
+    from gps_gaussian_b200 import gs_head
+    cls = mod.GSRegresser
+    key = (cls, "forward")
+    if key not in _ORIG_METHODS:
+        _ORIG_METHODS[key] = cls.__dict__["forward"]
+    cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key])
 
 
 _JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
@@ -279,11 +299,12 @@ _TARGETS = {"core.corr": _patch_corr, "lib.GaussianRender": _patch_render}
 _RECTIFY_TARGETS = {"lib.human_loader": _patch_loader}
 _FLOW_HEAD_TARGETS = {"core.raft_stereo_human": _patch_upsample, "lib.loss": _patch_loss}
 _ENCODE_TARGETS = {"cv2": _patch_cv2}
+_GS_HEAD_TARGETS = {"lib.gs_parm_network": _patch_regresser}
 
 
 def _targets():
     return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {}),
-            **(_ENCODE_TARGETS if _ENCODE else {})}
+            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD else {})}
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -333,13 +354,14 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD, GPSG_DECODE and GPSG_ENCODE here, once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE
+    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE and GPSG_GS_HEAD here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
     _DECODE = os.environ.get("GPSG_DECODE", "") == "1"
     _ENCODE = os.environ.get("GPSG_ENCODE", "") == "1"
+    _GS_HEAD = os.environ.get("GPSG_GS_HEAD", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -395,3 +417,9 @@ def encode():
 def flow_head():
     """Whether the installed patch runs the disparity head on the fused kernels (GPSG_FLOW_HEAD=1 at install())."""
     return _FLOW_HEAD
+
+
+def gs_head():
+    """Whether the installed patch runs the regressor's full-resolution tail on the fused kernels (GPSG_GS_HEAD=1 at
+    install())."""
+    return _GS_HEAD

@@ -522,6 +522,32 @@ GPSG_API int gpsg_sequence_loss_forward(int device, void* stream, GpsgSeqLossArg
 GPSG_API int gpsg_sequence_loss_backward(int device, void* stream, GpsgSeqLossArgs args, const float* grad_loss,
                                          const float* stats);
 
+/* ---- full-resolution tail of the Gaussian-parameter regressor (reference lib/gs_parm_network.py, GSRegresser) -------
+ * gpsg_gs_head_forward: from the decoder1 output to the three parameter maps, forward only:
+ *   up   = bilinear x2 upsampling of src [B,48,H/2,W/2] (align_corners=False: source (dst + 0.5) / 2 - 0.5, clamped at
+ *          0 below, upper neighbour clamped to the last row / column);
+ *   mid  = relu(conv3x3(cat[up, img [B,3,H,W], depth [B,1,H,W]], out_w, out_b)), zero padding of the concatenation;
+ *   rot  [B,4,H,W] = normalize(conv1x1(relu(conv3x3(mid, rot_w1, rot_b1)), rot_w2, rot_b2)), x / max(||x||, 1e-12);
+ *   scale [B,3,H,W] = min(softplus_100(conv1x1(relu(conv3x3(mid, scale_w1, ...)), ...)), 0.01), softplus_100(x) = x
+ *          where 100 x > 20, else log1p(exp(100 x)) / 100;
+ *   opacity [B,1,H,W] = sigmoid(conv1x1(relu(conv3x3(mid, opacity_w1, ...)), ...)).
+ *   Weights in torch's layouts: out_w [32,52,3,3], *_w1 [32,32,3,3], rot_w2 [4,32,1,1], scale_w2 [3,32,1,1],
+ *   opacity_w2 [1,32,1,1], biases [Cout]; every tensor fp32 and contiguous.  Every convolution operand (weights and
+ *   activations) is rounded to TF32 (round to nearest, ties away), products and sums are fp32 in an unspecified order:
+ *   the precision class of cuDNN with allow_tf32.  ReLU and the clamp keep NaN.  H and W even, B >= 0.
+ *   workspace: gpsg_gs_head_workspace_bytes(B, H, W) bytes, 16-byte aligned (the 32-channel intermediate).
+ *   Enqueues on `stream` and does not synchronise. */
+typedef struct GpsgGsHeadWeights {
+    const float* out_w; const float* out_b;
+    const float* rot_w1; const float* rot_b1; const float* rot_w2; const float* rot_b2;
+    const float* scale_w1; const float* scale_b1; const float* scale_w2; const float* scale_b2;
+    const float* opacity_w1; const float* opacity_b1; const float* opacity_w2; const float* opacity_b2;
+} GpsgGsHeadWeights;
+GPSG_API size_t gpsg_gs_head_workspace_bytes(int B, int H, int W);
+GPSG_API int gpsg_gs_head_forward(int device, void* stream, int B, int H, int W, const float* src, const float* img,
+                                  const float* depth, float* rot, float* scale, float* opacity, GpsgGsHeadWeights weights,
+                                  void* workspace);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.
