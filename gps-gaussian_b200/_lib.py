@@ -197,6 +197,17 @@ lib.gpsg_gs_head_workspace_bytes.restype = _sz
 lib.gpsg_gs_head_workspace_bytes.argtypes = [_i, _i, _i]
 lib.gpsg_gs_head_forward.restype = _i
 lib.gpsg_gs_head_forward.argtypes = [_i, _vp, _i, _i, _i] + [_vp] * 6 + [GsHeadWeights, _vp]
+
+
+class GsHeadGrads(C.Structure):
+    """GpsgGsHeadGrads (include/gpsg.h), passed by value: the 14 device pointers of the tail's weight gradients."""
+    _fields_ = [(n, C.c_void_p) for n in GS_HEAD_PARAMS]
+
+
+lib.gpsg_gs_head_backward_workspace_bytes.restype = _sz
+lib.gpsg_gs_head_backward_workspace_bytes.argtypes = [_i, _i, _i]
+lib.gpsg_gs_head_backward.restype = _i
+lib.gpsg_gs_head_backward.argtypes = [_i, _vp, _i, _i, _i] + [_vp] * 9 + [GsHeadWeights, GsHeadGrads, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -220,7 +231,7 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_sequence_loss_backward", "gpsg_mesh_render_workspace_bytes", "gpsg_mesh_render", "gpsg_jpeg_parse",
             "gpsg_jpeg_decode_workspace_bytes", "gpsg_jpeg_decode", "gpsg_jpeg_encode_max_bytes",
             "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode", "gpsg_gs_head_workspace_bytes",
-            "gpsg_gs_head_forward"]
+            "gpsg_gs_head_forward", "gpsg_gs_head_backward_workspace_bytes", "gpsg_gs_head_backward"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

@@ -929,6 +929,29 @@ int gpsg_gs_head_forward(int device, void* stream_, int B, int H, int W, const f
                               (cudaStream_t)stream_);
 }
 
+size_t gpsg_gs_head_backward_workspace_bytes(int B, int H, int W) {
+    return (B > 0 && H > 0 && W > 0) ? gs_head_backward_workspace_bytes(B, H, W) : 0;
+}
+
+int gpsg_gs_head_backward(int device, void* stream_, int B, int H, int W, const float* src, const float* img,
+                          const float* depth, const float* mid, const float* g_rot, const float* g_scale,
+                          const float* g_opacity, float* d_src, float* d_depth, GpsgGsHeadWeights weights,
+                          GpsgGsHeadGrads grads, void* workspace) {
+    GPSG_REQUIRE(B >= 0 && H >= 0 && W >= 0 && H % 2 == 0 && W % 2 == 0, "gs_head: H and W must be even, sizes >= 0");
+    GPSG_REQUIRE(H <= 65536 && W <= 65536 && (int64_t)B * H * W * 128 < (int64_t(1) << 40), "gs_head: too large");
+    if ((int64_t)B * H * W == 0) return GPSG_OK;
+    GPSG_REQUIRE(src && img && depth && mid && g_rot && g_scale && g_opacity && workspace, "NULL pointer");
+    const float* const* w = &weights.out_w;
+    for (int i = 0; i < 14; ++i) GPSG_REQUIRE(w[i], "gs_head: NULL weight pointer");
+    float* const* gw = &grads.out_w;
+    for (int i = 0; i < 14; ++i) GPSG_REQUIRE(gw[i], "gs_head: NULL gradient pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 16 == 0 && (uintptr_t)mid % 16 == 0,
+                 "gs_head: workspace and mid must be 16-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_gs_head_bwd(device, B, H, W, src, img, depth, mid, g_rot, g_scale, g_opacity, weights, d_src, d_depth,
+                              grads, workspace, (cudaStream_t)stream_);
+}
+
 int gpsg_set_corr_build(int mode) {
     set_corr_build_mode(mode);
     return GPSG_OK;

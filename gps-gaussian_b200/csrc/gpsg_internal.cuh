@@ -266,6 +266,11 @@ size_t gs_head_workspace_bytes(int B, int H, int W);
 int launch_gs_head_fwd(int device, int B, int H, int W, const float* src, const float* img, const float* depth,
                        const GpsgGsHeadWeights& wt, float* rot, float* scale, float* opacity, void* workspace,
                        cudaStream_t stream);
+size_t gs_head_backward_workspace_bytes(int B, int H, int W);
+int launch_gs_head_bwd(int device, int B, int H, int W, const float* src, const float* img, const float* depth,
+                       const float* mid, const float* g_rot, const float* g_scale, const float* g_opacity,
+                       const GpsgGsHeadWeights& wt, float* d_src, float* d_depth, const GpsgGsHeadGrads& grads,
+                       void* workspace, cudaStream_t stream);
 int launch_sequence_loss_fwd(const GpsgSeqLossArgs& a, float* stats, void* workspace, cudaStream_t stream);
 int launch_sequence_loss_bwd(const GpsgSeqLossArgs& a, const float* grad_loss, const float* stats, cudaStream_t stream);
 // corr.cu

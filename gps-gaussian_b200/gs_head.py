@@ -1,21 +1,25 @@
-"""The full-resolution tail of the Gaussian-parameter regressor on sm_90a (csrc/gs_head.cu), forward only.
+"""The full-resolution tail of the Gaussian-parameter regressor on sm_90a (csrc/gs_head.cu), forward and backward.
 
 `GSRegresser.forward` (reference lib/gs_parm_network.py) runs at 1/8 to 1/2 resolution up to `decoder1`; its last step
 upsamples the 48-channel decoder output x2, concatenates the image and the depth, and runs `out_conv` and the rot /
 scale / opacity heads at full resolution, in fp32.  `gs_head` does that step in two TF32 warpgroup-MMA (wgmma)
 kernels in place of the upsample / cat / seven convolutions / ReLU / activation chain, reading the half-resolution
-decoder output, the image and the depth and writing the three maps.
+decoder output, the image and the depth and writing the three maps.  `gs_head_train` is the same with autograd: its
+backward (`gpsg_gs_head_backward`) recomputes the heads from the forward's saved 32-channel intermediate and returns
+the gradients of the decoder output, the depth and the 14 weights (not the image's).
 
 `make_regresser_forward(orig)` is `GSRegresser.forward` that hands the decoder1 output to `gs_head` when autograd is off
 (the inference scripts and the stage-2 evaluation run under `torch.no_grad()`) and `supported(...)` holds; with grad
 enabled (the training step), under autocast, or for inputs the kernels do not cover, it calls `orig`, the reference's
-own method, unchanged.  The maps differ from cuDNN's TF32 convolutions by TF32 re-association; see include/gpsg.h for
-the exact semantics.
+own method, unchanged.  `make_regresser_forward(orig, train=True)` also sends a grad-enabled call to `gs_head_train`
+when the image does not require grad.  The maps and gradients differ from cuDNN's TF32 convolutions by TF32
+re-association; see include/gpsg.h for the exact semantics.
 """
 import ctypes as C
 
 import torch
 from torch import nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -96,9 +100,7 @@ def supported(regresser, img, depth, up_src):
     return True
 
 
-def run(up_src, img, depth, params):
-    """The kernels on raw tensors: up_src [B,48,H/2,W/2], img [B,3,H,W], depth [B,1,H,W] and the 14 parameters in
-    `params_of` order, all CUDA fp32 on one device -> (rot [B,4,H,W], scale [B,3,H,W], opacity [B,1,H,W])."""
+def _check_args(up_src, img, depth, params):
     B, _, H, W = (int(s) for s in img.shape)
     dev = img.device
     if not (_tensors_supported(dev, up_src, img, depth, *params) and tuple(up_src.shape) == (B, SRC_C, H // 2, W // 2)
@@ -108,6 +110,13 @@ def run(up_src, img, depth, params):
             f"gs_head (gpsg): needs CUDA fp32 up_src [B,48,H/2,W/2], img [B,3,H,W], depth [B,1,H,W] with even H, W and "
             f"the 14 tail parameters on one device; got up_src {tuple(up_src.shape)} {up_src.dtype} {up_src.device}, "
             f"img {tuple(img.shape)} {img.dtype} {img.device}, depth {tuple(depth.shape)} {depth.dtype}")
+    return B, H, W, dev
+
+
+def forward_with_mid(up_src, img, depth, params):
+    """`run`, and the forward's workspace: (rot, scale, opacity, mid) with mid the 32-channel intermediate, a flat fp32
+    tensor holding NHWC [B,H,W,32] (TF32 values), as the backward takes it."""
+    B, H, W, dev = _check_args(up_src, img, depth, params)
     with torch.no_grad():
         src, im, dp = (t.detach().contiguous() for t in (up_src, img, depth))
         ps = [p.detach().contiguous() for p in params]
@@ -121,7 +130,84 @@ def run(up_src, img, depth, params):
             rc = _lib.lib.gpsg_gs_head_forward(*_lib.device_stream(dev), B, H, W, _p(src), _p(im), _p(dp), _p(rot),
                                                _p(scale), _p(opacity), wt, _p(ws))
         _lib.check(rc, "gpsg_gs_head_forward")
-    return rot, scale, opacity
+    return rot, scale, opacity, ws
+
+
+def run(up_src, img, depth, params):
+    """The kernels on raw tensors: up_src [B,48,H/2,W/2], img [B,3,H,W], depth [B,1,H,W] and the 14 parameters in
+    `params_of` order, all CUDA fp32 on one device -> (rot [B,4,H,W], scale [B,3,H,W], opacity [B,1,H,W])."""
+    return forward_with_mid(up_src, img, depth, params)[:3]
+
+
+_COUNTS = {"backward": 0}
+
+
+def counts():
+    """{'backward': n}: calls of the backward kernels in this process."""
+    return dict(_COUNTS)
+
+
+def reset_counts():
+    _COUNTS["backward"] = 0
+
+
+def backward(up_src, img, depth, params, mid, g_rot, g_scale, g_opacity, need_src=True, need_depth=True,
+             workspace=None):
+    """The backward kernels: (d_src or None, d_depth or None, [14 parameter gradients]) from the forward's inputs, its
+    workspace `mid` (`forward_with_mid`) and the upstream gradients of rot, scale and opacity.  `workspace`: an fp32
+    CUDA tensor of at least gpsg_gs_head_backward_workspace_bytes to use as scratch (allocated here when None); after
+    the call its first B*H*W*48 floats hold dcat[:, :48] NHWC when d_src or d_depth was computed."""
+    B, H, W, dev = _check_args(up_src, img, depth, params)
+    gs = [g.detach().to(torch.float32).contiguous() for g in (g_rot, g_scale, g_opacity)]
+    if not (_tensors_supported(dev, mid, *gs) and mid.numel() * 4 >= _lib.lib.gpsg_gs_head_workspace_bytes(B, H, W)
+            and [tuple(g.shape) for g in gs] == [(B, 4, H, W), (B, 3, H, W), (B, 1, H, W)]):
+        raise RuntimeError("gs_head backward (gpsg): needs the forward's workspace and fp32 gradients of the three maps")
+    with torch.no_grad():
+        src, im, dp = (t.detach().contiguous() for t in (up_src, img, depth))
+        ps = [p.detach().contiguous() for p in params]
+        d_src = torch.empty((B, SRC_C, H // 2, W // 2), dtype=torch.float32, device=dev) if need_src else None
+        d_depth = torch.empty((B, DEPTH_C, H, W), dtype=torch.float32, device=dev) if need_depth else None
+        grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in PARAM_SHAPES]
+        nbytes = int(_lib.lib.gpsg_gs_head_backward_workspace_bytes(B, H, W))
+        ws = workspace
+        if ws is None:
+            ws = torch.empty(max(nbytes // 4, 1), dtype=torch.float32, device=dev)
+        elif not (_tensors_supported(dev, ws) and ws.is_contiguous() and ws.numel() * 4 >= nbytes):
+            raise RuntimeError("gs_head backward (gpsg): workspace must be a contiguous fp32 tensor on the device of "
+                               f"at least {nbytes} bytes")
+        wt = _lib.GsHeadWeights(*[p.data_ptr() for p in ps])
+        gr = _lib.GsHeadGrads(*[g.data_ptr() for g in grads])
+        opt = lambda t: _p(t) if t is not None else None
+        with torch.cuda.device(dev):
+            rc = _lib.lib.gpsg_gs_head_backward(*_lib.device_stream(dev), B, H, W, _p(src), _p(im), _p(dp), _p(mid),
+                                                *[_p(g) for g in gs], opt(d_src), opt(d_depth), wt, gr, _p(ws))
+        _lib.check(rc, "gpsg_gs_head_backward")
+    _COUNTS["backward"] += 1
+    return d_src, d_depth, grads
+
+
+class _Tail(torch.autograd.Function):
+    """The tail with autograd over (up_src, img, depth, *params); the image's gradient is not computed."""
+
+    @staticmethod
+    def forward(ctx, up_src, img, depth, *params):
+        rot, scale, opacity, mid = forward_with_mid(up_src, img, depth, params)
+        ctx.save_for_backward(up_src, img, depth, mid, *params)
+        return rot, scale, opacity
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_rot, g_scale, g_opacity):
+        up_src, img, depth, mid, *params = ctx.saved_tensors
+        if ctx.needs_input_grad[1]:
+            raise RuntimeError("gs_head_train (gpsg): the image's gradient is not computed")
+        outs = []
+        for g, c in zip((g_rot, g_scale, g_opacity), (4, 3, 1)):
+            B, _, H, W = img.shape
+            outs.append(g if g is not None else torch.zeros((B, c, H, W), dtype=torch.float32, device=img.device))
+        need = ctx.needs_input_grad
+        d_src, d_depth, grads = backward(up_src, img, depth, params, mid, *outs, need_src=need[0], need_depth=need[2])
+        return (d_src, None, d_depth) + tuple(g if n else None for g, n in zip(grads, need[3:]))
 
 
 def gs_head(up_src, img, depth, regresser):
@@ -132,11 +218,24 @@ def gs_head(up_src, img, depth, regresser):
     return run(up_src, img, depth, params_of(regresser))
 
 
-def make_regresser_forward(orig):
+def gs_head_train(up_src, img, depth, regresser):
+    """`gs_head` with autograd: gradients reach up_src, depth and the tail's 14 parameters through the backward kernels.
+    The image must not require grad (its gradient is not computed)."""
+    if not supported(regresser, img, depth, up_src):
+        raise RuntimeError("gs_head (gpsg): inputs or module not supported; see gs_head.supported")
+    if img.requires_grad and torch.is_grad_enabled():
+        raise RuntimeError("gs_head_train (gpsg): the image's gradient is not computed; img must not require grad")
+    return _Tail.apply(up_src, img, depth, *params_of(regresser))
+
+
+def make_regresser_forward(orig, train=False):
     """`GSRegresser.forward` with the full-resolution tail on the kernels when grad is disabled and the inputs are
-    supported; otherwise `orig`, the reference's own method."""
+    supported; with `train`, also when grad is enabled and the image does not require grad (`gs_head_train`);
+    otherwise `orig`, the reference's own method."""
     def forward(self, img, depth, img_feat):
-        if torch.is_grad_enabled() or torch.is_autocast_enabled() or not supported(self, img, depth, None):
+        grad = torch.is_grad_enabled()
+        if ((grad and not (train and torch.is_tensor(img) and not img.requires_grad)) or torch.is_autocast_enabled()
+                or not supported(self, img, depth, None)):
             return orig(self, img, depth, img_feat)
         img_feat1, img_feat2, img_feat3 = img_feat
         depth_feat1, depth_feat2, depth_feat3 = self.depth_encoder(depth)
@@ -145,6 +244,8 @@ def make_regresser_forward(orig):
         x = self.decoder1(torch.cat([self.up(x), img_feat1, depth_feat1], dim=1))
         if not supported(self, img, depth, x):        # e.g. fp16 image features: the decoders ran in fp16
             return orig(self, img, depth, img_feat)
+        if grad:
+            return _Tail.apply(x, img, depth, *params_of(self))
         return run(x, img, depth, params_of(self))
     forward.__doc__ = orig.__doc__
     return forward

@@ -59,6 +59,12 @@ full-resolution tail, from the decoder1 output to the rot / scale / opacity maps
 kernels do not cover, the reference's own forward runs unchanged.  The maps differ from cuDNN's by TF32 re-association,
 which is why the switch is opt-in.  Unset or any other value leaves `lib.gs_parm_network` alone.
 
+`GPSG_GS_HEAD_TRAIN=1`, read once by `install()`, rebinds the same method with `make_regresser_forward(orig,
+train=True)`: the autograd-off route above, and with grad enabled (train_stage2.py's training step) the tail runs on
+the kernels forward and backward (gs_head.gs_head_train) when the image does not require grad.  Under autocast or for
+inputs the kernels do not cover, the reference's own forward runs.  The gradients differ from cuDNN's by TF32
+re-association, which is why this switch is opt-in too; `GPSG_GS_HEAD=1` alone keeps the training step on cuDNN.
+
 `taichi_three` and its submodules always resolve to the stand-in in dropin/taichi_three (the dataset renderer on
 csrc/mesh_render.cu).  `python prepare_data/render_data.py` puts prepare_data/ first on sys.path, where the reference's
 own package, which cannot import without Taichi, would shadow anything on PYTHONPATH.
@@ -77,6 +83,7 @@ _FLOW_HEAD = False    # GPSG_FLOW_HEAD=1 at install()
 _DECODE = False       # GPSG_DECODE=1 at install()
 _ENCODE = False       # GPSG_ENCODE=1 at install()
 _GS_HEAD = False      # GPSG_GS_HEAD=1 at install()
+_GS_HEAD_TRAIN = False  # GPSG_GS_HEAD_TRAIN=1 at install()
 
 
 def _set(mod, attr, new):
@@ -189,7 +196,7 @@ def _patch_regresser(mod):
     key = (cls, "forward")
     if key not in _ORIG_METHODS:
         _ORIG_METHODS[key] = cls.__dict__["forward"]
-    cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key])
+    cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key], train=_GS_HEAD_TRAIN)
 
 
 _JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
@@ -304,7 +311,7 @@ _GS_HEAD_TARGETS = {"lib.gs_parm_network": _patch_regresser}
 
 def _targets():
     return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {}),
-            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD else {})}
+            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD or _GS_HEAD_TRAIN else {})}
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -354,14 +361,15 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE and GPSG_GS_HEAD here, once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD
+    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD and GPSG_GS_HEAD_TRAIN here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
     _DECODE = os.environ.get("GPSG_DECODE", "") == "1"
     _ENCODE = os.environ.get("GPSG_ENCODE", "") == "1"
     _GS_HEAD = os.environ.get("GPSG_GS_HEAD", "") == "1"
+    _GS_HEAD_TRAIN = os.environ.get("GPSG_GS_HEAD_TRAIN", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -423,3 +431,9 @@ def gs_head():
     """Whether the installed patch runs the regressor's full-resolution tail on the fused kernels (GPSG_GS_HEAD=1 at
     install())."""
     return _GS_HEAD
+
+
+def gs_head_train():
+    """Whether the installed patch also trains the regressor's full-resolution tail on the fused kernels, forward and
+    backward (GPSG_GS_HEAD_TRAIN=1 at install())."""
+    return _GS_HEAD_TRAIN

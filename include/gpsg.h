@@ -548,6 +548,35 @@ GPSG_API int gpsg_gs_head_forward(int device, void* stream, int B, int H, int W,
                                   const float* depth, float* rot, float* scale, float* opacity, GpsgGsHeadWeights weights,
                                   void* workspace);
 
+/* gpsg_gs_head_backward: the gradients of gpsg_gs_head_forward's maps with respect to src, depth and the 14 weights, from
+ * the upstream gradients g_rot [B,4,H,W], g_scale [B,3,H,W], g_opacity [B,1,H,W] (fp32, contiguous):
+ *   d_src [B,48,H/2,W/2] (NULL: not computed), d_depth [B,1,H,W] (NULL: not computed), and `grads`, 14 device
+ *   pointers in GpsgGsHeadWeights order and torch's layouts, all required.  The image's gradient is not computed.
+ *   mid: the forward's workspace after gpsg_gs_head_forward on the same inputs and weights (the 32-channel intermediate),
+ *   16-byte aligned; the pre-activations of the heads are recomputed from it.
+ *   Masks and branches are those of torch's autograd on the forward's maths: ReLU passes the gradient where its result
+ *   is not <= 0 (NaN passes), clamp_max(0.01) where the softplus is <= 0.01, softplus(beta 100, threshold 20) takes
+ *   g where 100 x > 20 and g e / (e + 1), e = exp(100 x), elsewhere, normalize differentiates x / clamp_min(||x||,
+ *   1e-12) with the norm's branch masked below 1e-12, sigmoid uses g (1 - y) y; the upsample's adjoint multiplies
+ *   every interpolation weight in, zero weights included.  Non-finite upstream gradients reach the outputs as they do
+ *   through torch's autograd.
+ *   Precision as the forward: every convolution operand, forward recomputation and backward GEMMs (dh and dmid, the
+ *   intermediates they read, the weights) is rounded to TF32 (round to nearest, ties away), products and sums are fp32.
+ *   Bit-reproducible: no floating-point atomics; every sum has a fixed order given the shape and the device's SM count.
+ *   workspace: gpsg_gs_head_backward_workspace_bytes(B, H, W) bytes, 16-byte aligned (128 channels per pixel of NHWC
+ *   scratch and the per-CTA partial sums).  H and W even, B >= 0.  Enqueues on `stream` and does not synchronise. */
+typedef struct GpsgGsHeadGrads {
+    float* out_w; float* out_b;
+    float* rot_w1; float* rot_b1; float* rot_w2; float* rot_b2;
+    float* scale_w1; float* scale_b1; float* scale_w2; float* scale_b2;
+    float* opacity_w1; float* opacity_b1; float* opacity_w2; float* opacity_b2;
+} GpsgGsHeadGrads;
+GPSG_API size_t gpsg_gs_head_backward_workspace_bytes(int B, int H, int W);
+GPSG_API int gpsg_gs_head_backward(int device, void* stream, int B, int H, int W, const float* src, const float* img,
+                                   const float* depth, const float* mid, const float* g_rot, const float* g_scale,
+                                   const float* g_opacity, float* d_src, float* d_depth, GpsgGsHeadWeights weights,
+                                   GpsgGsHeadGrads grads, void* workspace);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.

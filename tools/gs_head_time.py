@@ -1,7 +1,7 @@
 """Time the regressor's full-resolution tail: the reference module's torch chain (oracle/_ref, cuDNN defaults) against the
 fused kernels (gps_gaussian_b200.gs_head), and a whole RtStereoHumanModel eval forward with GPSG_GS_HEAD off and on.
 
-    python tools/gs_head_time.py [--seconds 2] [--rounds 3] [--no-model] [--trace] [--out DIR]
+    python tools/gs_head_time.py [--seconds 2] [--rounds 3] [--no-model] [--trace] [--train] [--out DIR]
 
 On cuda:0, in one process:
   * the tail alone at B = 2 (one inference frame: two source views) and B = 4 (a stage-2 eval batch), 1024^2: from the
@@ -11,6 +11,10 @@ On cuda:0, in one process:
   * the eval forward of the reference's RtStereoHumanModel on a synthetic 1024^2 pair (batch 1), switch off / on.
   * --trace: instead, one torch.profiler trace of the switched-on eval forward (DIR/gs_head_eval.pt.trace.json) and the
     table of CUDA kernels that ran in it.
+  * --train: instead, forward + backward of the tail at B = 4, 1024^2 (a stage-2 training batch: two samples x two
+    source views), the reference module's chain under autograd (cuDNN defaults) against gs_head_train, alternated rounds
+    as above; each backward kernel timed by the profiler with its share of the TF32 or HBM bound; and one whole
+    harness.c3_step at src_res 1024, batch 2, with GPSG_GS_HEAD_TRAIN off and on: step time and peak allocated memory.
 Prints one JSON object with the GPU name and power limit (also written to DIR/gs_head_time.json with --out)."""
 import argparse
 import json
@@ -37,6 +41,117 @@ def work(B, H=1024, W=1024):
     src, io = B * 48 * (H // 2) * (W // 2) * 4, px * 4 * 4          # decoder output; img + depth
     mid = px * 32 * 4
     return {"stage1": dict(flop=f1, bytes=src + io + mid), "stage2": dict(flop=f2, bytes=mid + px * 8 * 4)}
+
+
+def train_work(B, H=1024, W=1024):
+    """Algorithmic FLOPs and HBM bytes of the forward + backward kernels from the shapes (K unpadded)."""
+    px = B * H * W
+    w = work(B, H, W)
+    src = B * 48 * (H // 2) * (W // 2) * 4
+    w.update({
+        "bwd_heads": dict(flop=2 * px * (96 * 32 * 9 + 2 * 32 * 8), bytes=px * (32 + 8 + 96) * 4),
+        "bwd_mid": dict(flop=2 * px * 32 * 96 * 9, bytes=px * (96 + 32 + 32) * 4),
+        "wgrad_heads": dict(flop=2 * px * 96 * 32 * 9, bytes=px * (96 + 32) * 4),
+        "bwd_cat": dict(flop=2 * px * 52 * 32 * 9, bytes=px * (32 + 48 + 1) * 4),
+        "bwd_src": dict(flop=2 * px * 48 * 4, bytes=px * 48 * 4 + src),
+        "wgrad_out": dict(flop=2 * px * 32 * 52 * 9, bytes=px * (32 + 4) * 4 + src),
+    })
+    return w
+
+
+_KERNEL_NAMES = (("gs_head_stage1", "stage1"), ("gs_head_stage2", "stage2"), ("gs_head_bwd_heads", "bwd_heads"),
+                 ("gs_head_bwd_mid", "bwd_mid"), ("gs_head_wgrad<96", "wgrad_heads"), ("gs_head_bwd_cat", "bwd_cat"),
+                 ("gs_head_bwd_src", "bwd_src"), ("gs_head_wgrad<32", "wgrad_out"), ("gs_head_bwd_reduce", "bwd_reduce"))
+
+
+def _per_kernel(prof, w):
+    per = {}
+    for e in prof.key_averages():
+        for pat, name in _KERNEL_NAMES:
+            if pat in e.key:
+                ms = e.device_time_total / max(e.count, 1) / 1e3
+                row = dict(ms=round(ms, 4))
+                if name in w:
+                    t = ms * 1e-3
+                    f, b = w[name]["flop"], w[name]["bytes"]
+                    row.update(flop=f, bytes=b, TFLOPs=round(f / t / 1e12, 1), TBps=round(b / t / 1e12, 3),
+                               bound="compute" if f / DATASHEET_TF32 > b / DATASHEET_BW else "memory",
+                               share_of_bound=round(max(f / DATASHEET_TF32, b / DATASHEET_BW) / t, 3))
+                per[name] = row
+    return per
+
+
+def _train_tail(seconds, rounds, B=4):
+    m = _module().train()
+    H = W = 1024
+    x = torch.randn(B, 48, H // 2, W // 2, device="cuda", requires_grad=True)
+    img = torch.rand(B, 3, H, W, device="cuda") * 2 - 1
+    depth = torch.rand(B, 1, H, W, device="cuda", requires_grad=True)
+    grads = [torch.randn(B, c, H, W, device="cuda") for c in (4, 3, 1)]
+
+    def step(fwd):
+        m.zero_grad(set_to_none=True)
+        x.grad = depth.grad = None
+        torch.autograd.backward(fwd(), grads)
+
+    arms = {"torch": lambda: step(lambda: _torch_tail(m, x, img, depth)),
+            "fused": lambda: step(lambda: gs_head.gs_head_train(x, img, depth, m))}
+    row = {k: [] for k in arms}
+    for _ in range(rounds):
+        for name, fn in arms.items():
+            row[name].append(round(_window(fn, seconds), 4))
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(10):
+            arms["fused"]()
+        torch.cuda.synchronize()
+    for name in arms:
+        r = row[name]
+        row[name] = dict(ms=r, best=min(r), spread=round((max(r) - min(r)) / min(r), 4))
+    row["speedup"] = round(row["torch"]["best"] / row["fused"]["best"], 2)
+    row["kernels"] = _per_kernel(prof, train_work(B))
+    peak = {}
+    for name, fn in arms.items():
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        fn()
+        torch.cuda.synchronize()
+        peak[name] = round((torch.cuda.max_memory_allocated() - base) / 2 ** 30, 3)
+    row["peak_extra_GiB"] = peak
+    return {f"B{B}_1024": row}
+
+
+def _train_step(rounds, steps=5):
+    from gps_gaussian_b200 import synth_dataset
+    res = {}
+    with tempfile.TemporaryDirectory() as root:
+        synth_dataset.write_dataset(root, n_train=2, n_val=1, res=1024, hr=True)
+        for on in (False, True):
+            patch.uninstall()
+            os.environ["GPSG_GS_HEAD_TRAIN"] = "1" if on else "0"
+            harness.add_reference_to_path()
+            patch.install()
+            cfg = harness.load_cfg(root, src_res=1024, num_steps=100, batch_size=2)
+            st = harness.C3State(cfg)
+            harness.c3_step(st, st.batch(0))                              # warm-up (allocator, cuDNN plans)
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            times = []
+            for _ in range(rounds):
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                for _ in range(steps):
+                    harness.c3_step(st, st.batch(0))
+                b.record()
+                b.synchronize()
+                times.append(round(a.elapsed_time(b) / steps, 2))
+            res["on" if on else "off"] = dict(step_ms=times, best=min(times),
+                                              max_memory_allocated_GiB=round(torch.cuda.max_memory_allocated() / 2 ** 30, 3))
+            del st
+            torch.cuda.empty_cache()
+        patch.uninstall()
+        os.environ.pop("GPSG_GS_HEAD_TRAIN", None)
+    return res
 
 
 def _gpu_info():
@@ -191,6 +306,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--no-model", action="store_true")
     ap.add_argument("--trace", action="store_true")
+    ap.add_argument("--train", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -203,6 +319,9 @@ def main():
         if not a.out:
             raise SystemExit("--trace needs --out")
         out["trace"] = _trace(a.out)
+    elif a.train:
+        out["train_tail"] = _train_tail(a.seconds, a.rounds)
+        out["c3_step_1024_batch2"] = _train_step(a.rounds)
     else:
         out["tail"] = _tail(a.seconds, a.rounds)
         if not a.no_model:
@@ -211,7 +330,8 @@ def main():
     print(s)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "gs_head_trace.json" if a.trace else "gs_head_time.json"), "w") as f:
+        name = "gs_head_trace.json" if a.trace else ("gs_head_train_time.json" if a.train else "gs_head_time.json")
+        with open(os.path.join(a.out, name), "w") as f:
             f.write(s + "\n")
 
 
