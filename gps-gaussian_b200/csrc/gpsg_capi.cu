@@ -4,6 +4,9 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
+#include <map>
+#include <mutex>
+#include <utility>
 #include "gpsg_internal.cuh"
 
 namespace gpsg {
@@ -15,6 +18,24 @@ void set_error(const char* fmt, ...) {
     va_start(ap, fmt);
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
+}
+
+// CTAs of `kernel` (at `threads` threads, no dynamic shared memory) resident on the whole current device at once.  Cached per
+// (device, kernel): the query runs on the host, outside any stream, once, so later forwards stay capturable into graphs.
+int resident_grid(const void* kernel, int threads) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, int> cache;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return -1;
+    std::lock_guard<std::mutex> lk(mu);
+    const auto key = std::make_pair(dev, kernel);
+    const auto it = cache.find(key);
+    if (it != cache.end()) return it->second;
+    int per_sm = 0, sms = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0) != cudaSuccess ||
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || per_sm < 1 || sms < 1)
+        return -1;
+    return cache[key] = per_sm * sms;
 }
 
 Camera make_camera(const GpsgRasterSettings& s) {
@@ -151,7 +172,6 @@ static uint32_t* pinned_slot() {
 
 
 // ---- profiling -------------------------------------------------------------------------------
-#include <mutex>
 #include <vector>
 namespace gpsg {
 struct ProfSlot { cudaEvent_t a, b; Stage stage; bool used; };

@@ -41,6 +41,8 @@ struct Camera {
     float campos[3];
 };
 Camera make_camera(const GpsgRasterSettings& s);
+// size of a persistent grid: CTAs of `kernel` at `threads` threads resident on the current device at once (-1: query failed)
+int resident_grid(const void* kernel, int threads);
 
 
 // ---- where the per-Gaussian inputs / gradients live -------------------------------------------------------------
@@ -154,7 +156,8 @@ struct ImageState {
     uint32_t* tile_count; // [tiles]  pairs per tile (counted by preprocess)
     uint32_t* tile_cursor;// [tiles]  scatter cursors
     uint32_t* totals;     // [64]     N, max count, overflow flag, #big tiles, preprocess CTA ticket (see tile_scan.cuh),
-                          //          [kFwdFlagsWord] the GPSG_FWD_* flags of the forward that wrote this state
+                          //          [kFwdFlagsWord] the GPSG_FWD_* flags of the forward that wrote this state,
+                          //          [kSortTicketWord] the tile sort's work ticket
     uint32_t* big_tiles;  // [tiles]  ids of tiles with more than kBigTile pairs
     uint32_t* tile_order; // [tiles]  all tile ids, longest list first (tile_scan.cuh): work order of the compositing kernels
     uint32_t* blk_count;  // [8*tiles] survivors per warp block (BinningState::blk_list); only read for non-empty tiles
@@ -165,6 +168,9 @@ struct ImageState {
 // totals at the start of every forward), read by the projection backward -- a backward always follows the mode of the
 // forward whose buffers it is given, without a host read or an extra ABI argument.
 constexpr int kFwdFlagsWord = 6;
+// totals word of the ticket the persistent tile sort takes its tiles with (zeroed with the rest of totals at the start of
+// every forward, so graph replays start from 0 too)
+constexpr int kSortTicketWord = 7;
 size_t scan_temp_bytes(int P);
 size_t sort_temp_bytes(size_t N, int end_bit);
 

@@ -174,83 +174,49 @@ __device__ __forceinline__ void slab_entry(uint32_t id, const GaussianSrc& src, 
 }
 
 constexpr int kSortThreads = 512;
-constexpr int kSortWarps = kSortThreads / 32;
 constexpr int kSortCTAsPerSM = 3;
 
 // ---- per-block survivor lists of the compositing forward (raster_render.cu) ------------------------------------------
 // For each of the 8 warp blocks of a tile (fwd_block_origin), the tile-local list positions of the entries whose cull box
-// (slabA: centre +- half-extents) meets the block, in list order.  The test is the expression the compositing kernel used
-// to evaluate per entry and block, on the same floats, so the forward composites exactly the entries it did before.
-// Built by a whole CTA of kSortThreads threads over chunks of kSortThreads consecutive positions: ballot ranks inside a
-// warp plus a CTA-wide prefix of the 8 per-warp counts.  Positions are 32-bit: tile lists exceed 65535 entries on the
-// radix path.
-struct BlockLists {
-    uint32_t cnt[kSortWarps][8];   // survivors of the chunk per (warp, block)
-    uint32_t off[kSortWarps][8];   // where each warp's survivors go in each block's list
-    uint32_t base[8];              // survivors of the earlier chunks per block
-};
+// (slabA: centre +- half-extents) meets the block, in list order.  Positions are 32-bit: tile lists exceed 65535 entries on
+// the radix path.  Both binning paths build them from the two functions below, so they define the lists identically.
 
-// Every thread of the CTA calls this, after the tile's slabA entries [0, n) are written (tileA = slabA + tile start; on the
-// sort path each thread reads back only entries it wrote itself).  list = blk_list + 8 * (tile start),
-// count = blk_count + 8 * tile.  The entries are read back (from L2) rather than taken from the gather loop's registers:
-// fused into that loop, the build pushes the sort kernel past its 40 registers into spills, and measured slower.
-__device__ __forceinline__ void build_block_lists(BlockLists& s, const float4* __restrict__ tileA, uint32_t n, int tile_x,
-                                                  int tile_y, uint32_t* __restrict__ list, uint32_t* __restrict__ count) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+// Bit k: the cull box of slab entry `a` meets block k of tile (tile_x, tile_y).  The test is the expression the compositing
+// kernel used to evaluate per entry and block, on the same floats, so the forward composites exactly the entries it did
+// before it had lists.  The x half depends on the block's column only and the y half on its row only.
+__device__ __forceinline__ uint32_t block_hit_mask(const float4& a, int tile_x, int tile_y) {
+    bool hx[2], hy[4];
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+        const float wx0 = (float)(tile_x * GPSG_TILE_X + 8 * c), wx1 = (float)(tile_x * GPSG_TILE_X + 8 * c + 7);
+        hx[c] = (a.x >= wx0 - a.z) && (a.x <= wx1 + a.z);
+    }
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+        const float wy0 = (float)(tile_y * GPSG_TILE_Y + 4 * w), wy1 = (float)(tile_y * GPSG_TILE_Y + 4 * w + 3);
+        hy[w] = (a.y >= wy0 - a.w) && (a.y <= wy1 + a.w);
+    }
+    uint32_t hits = 0u;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) hits |= (uint32_t)(hx[fwd_block_col(k)] && hy[fwd_block_row(k)]) << k;
+    return hits;
+}
+
+// Called by one whole warp: appends the positions r0 + i, i in [0, m), whose hit mask hits[i] has bit k to block k's list
+// (list = blk_list + 8 * (tile start) + k * n), in order; `base` counts the list's entries before position r0.  One ballot
+// per 32 positions and no CTA barrier: the warp owns this part of block k's list.
+__device__ __forceinline__ void append_block_list(const uint8_t* hits, uint32_t r0, uint32_t m, int k,
+                                                  uint32_t* __restrict__ list, uint32_t& base) {
+    const int lane = threadIdx.x & 31;
     const unsigned lt = (1u << lane) - 1u;
-    // block k keeps an entry iff (a.x >= wx0 - a.z) && (a.x <= wx1 + a.z) && (a.y >= wy0 - a.w) && (a.y <= wy1 + a.w) for
-    // its window; the x half depends on the block's column only and the y half on its row only
-    float wx0[2], wx1[2], wy0[4], wy1[4];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        int bx0, by0;
-        fwd_block_origin(tile_x, tile_y, k, bx0, by0);
-        wx0[fwd_block_col(k)] = (float)bx0; wx1[fwd_block_col(k)] = (float)(bx0 + 7);
-        wy0[fwd_block_row(k)] = (float)by0; wy1[fwd_block_row(k)] = (float)(by0 + 3);
+#pragma unroll 4
+    for (uint32_t c = 0; c < m; c += 32) {
+        const uint32_t i = c + lane;
+        const bool hit = i < m && ((hits[i] >> k) & 1u);
+        const unsigned mask = __ballot_sync(0xffffffffu, hit);
+        if (hit) list[base + __popc(mask & lt)] = r0 + i;
+        base += __popc(mask);
     }
-    if (threadIdx.x < 8) s.base[threadIdx.x] = 0u;
-#pragma unroll 1
-    for (uint32_t c0 = 0; c0 < n; c0 += kSortThreads) {
-        const uint32_t r = c0 + threadIdx.x;
-        const bool valid = r < n;
-        const float4 a = valid ? tileA[r] : make_float4(0.f, 0.f, 0.f, 0.f);
-        bool hx[2], hy[4];
-#pragma unroll
-        for (int c = 0; c < 2; ++c) hx[c] = (a.x >= wx0[c] - a.z) && (a.x <= wx1[c] + a.z);
-#pragma unroll
-        for (int w = 0; w < 4; ++w) hy[w] = (a.y >= wy0[w] - a.w) && (a.y <= wy1[w] + a.w);
-        uint32_t hits = 0u;   // bit k: the entry survives block k's cull
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const bool hit = valid && hx[fwd_block_col(k)] && hy[fwd_block_row(k)];
-            hits |= (uint32_t)hit << k;
-            const unsigned m = __ballot_sync(0xffffffffu, hit);
-            if (lane == k) s.cnt[warp][k] = __popc(m);
-        }
-        __syncthreads();
-        if (threadIdx.x < kSortWarps * 8) {   // one 16-lane segment per block: exclusive scan over the warps
-            static_assert(kSortWarps == 16, "one 16-lane segment per block");
-            const int k = threadIdx.x >> 4, w = threadIdx.x & 15;
-            const uint32_t cw = s.cnt[w][k];
-            uint32_t incl = cw;
-#pragma unroll
-            for (int o = 1; o < 16; o <<= 1) {
-                const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o, 16);
-                if (w >= o) incl += u;
-            }
-            const uint32_t b = s.base[k];
-            s.off[w][k] = b + incl - cw;
-            __syncwarp();
-            if (w == 15) s.base[k] = b + incl;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const unsigned m = __ballot_sync(0xffffffffu, (hits >> k) & 1u);
-            if ((hits >> k) & 1u) list[(size_t)k * n + s.off[warp][k] + __popc(m & lt)] = r;
-        }
-    }
-    if (threadIdx.x < 8) count[threadIdx.x] = s.base[threadIdx.x];   // base was last written before the final barrier
 }
 
 // one CTA per tile: radix sort of the tile's bucket inside the CTA (cub::BlockRadixSort, keys in registers), then the
@@ -278,7 +244,7 @@ struct TileSort {
     //    to the full (id, then depth) LSD radix sort, so degenerate inputs (thousands of identical depths) stay correct
     //    and bounded.
     static constexpr int kMaxRun = 16;
-    __device__ static void run(Smem& sm, uint32_t* flags, BlockLists& bl, const uint2* __restrict__ src, int n, int id_bits,
+    __device__ static void run(Smem& sm, uint32_t* flags, uint8_t* hits, const uint2* __restrict__ src, int n, int id_bits,
                                uint32_t tile, int grid_x, size_t out0, const GaussianSrc& src_in, const GeomState& g,
                                const BinningState& b, uint32_t* __restrict__ blk_count) {
         uint32_t keys[ITEMS], ids[ITEMS];
@@ -365,8 +331,11 @@ struct TileSort {
                 sm.keys[k * kSortThreads + (int)threadIdx.x] = ((unsigned long long)(keys[k] + dlo) << 32) | ids[k];
             __syncthreads();
         }
-        // ---- gather: each thread takes ranks tid, tid + kSortThreads, ... so every store below is coalesced ----
+        // ---- gather: each thread takes ranks tid, tid + kSortThreads, ... so every store below is coalesced; the block
+        // hit mask of each rank goes to shared memory for the list build (cheaper than reading slab A back from L2 and
+        // prefixing per-warp counts across the CTA per 512 positions: DESIGN.md, footnote 10) ----
         const unsigned long long tile_hi = (unsigned long long)tile << 32;
+        const int tile_y = (int)tile / grid_x, tile_x = (int)tile - tile_y * grid_x;
 #pragma unroll 1
         for (int k = 0; k < ITEMS; ++k) {
             const int r = k * kSortThreads + (int)threadIdx.x;
@@ -383,34 +352,53 @@ struct TileSort {
                 b.slabA[o] = A;
                 b.slabB[o] = B;
                 b.slabC[o] = C;
+                hits[r] = (uint8_t)block_hit_mask(A, tile_x, tile_y);
             }
         }
-        const int tile_y = (int)tile / grid_x;
-        build_block_lists(bl, b.slabA + out0, (uint32_t)n, (int)tile - tile_y * grid_x, tile_y, b.blk_list + 8 * out0,
-                          blk_count + 8 * (size_t)tile);
+        __syncthreads();
+        // ---- per-block survivor lists: warp k writes block k's for positions [0, split), warp k + 8 for [split, n), from
+        // the masks of the whole tile.  Warp k + 8 starts at the number of block k's survivors in [0, split), which it
+        // counts from the masks itself (4 positions per lane and load); split is a multiple of 128 positions for that ----
+        const int warp = (int)threadIdx.x >> 5, blk = warp & 7;
+        const uint32_t split = ((uint32_t)n / 2u) & ~127u;
+        uint32_t* __restrict__ list = b.blk_list + 8 * out0 + (size_t)blk * n;
+        uint32_t cnt = 0u;
+        if (warp < 8) {
+            append_block_list(hits, 0u, split, blk, list, cnt);
+        } else {
+            const uint32_t* __restrict__ words = reinterpret_cast<const uint32_t*>(hits);
+#pragma unroll 1
+            for (uint32_t i = threadIdx.x & 31; i < split / 4u; i += 32) cnt += __popc(words[i] & (0x01010101u << blk));
+            cnt = __reduce_add_sync(0xffffffffu, cnt);
+            append_block_list(hits + split, split, (uint32_t)n - split, blk, list, cnt);
+            if ((threadIdx.x & 31) == 0) blk_count[8 * (size_t)tile + blk] = cnt;
+        }
     }
 };
 
-// BIG = false: one CTA per tile, tiles with n <= 2048 (1/2/3/4 keys per thread; real scenes put most busy tiles
-// between 1025 and 1536 entries).  BIG = true: a small persistent grid that walks the list of big tiles
-// (2048 < n <= 4096) built by the tile scan -- it costs ~nothing when the list is empty, so the planned (sync-free)
-// path can always launch it.  Two kernels so that the common case is not held at the register / shared-memory
-// footprint of the rare one.
+// BIG = false: tiles with n <= 2048 (1/2/3/4 keys per thread; real scenes put most busy tiles between 1025 and 1536
+// entries), on a persistent grid of as many CTAs as fit on the GPU at once.  A CTA takes the next tile of `tile_order` with
+// an atomic ticket (totals[kSortTicketWord]) and stops at the first empty one: tile_order is longest first and ends with
+// exactly the empty tiles (order_bucket), so no CTA is spent on them.  BIG = true: a small persistent grid that walks the
+// list of big tiles (2048 < n <= 4096) built by the tile scan -- it costs ~nothing when the list is empty, so the planned
+// (sync-free) path can always launch it.  Two kernels so that the common case is not held at the register /
+// shared-memory footprint of the rare one.
 template <bool BIG>
 __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_sort_gather_kernel(const GaussianSrc colors, GeomState g,
                                                                             BinningState b, ImageState im, int id_bits,
-                                                                            int grid_x) {
-    __shared__ uint32_t flags[4];
-    __shared__ BlockLists bl;
+                                                                            int grid_x, uint32_t tiles) {
+    // tiles = length of tile_order, which bounds the ticket walk of BIG = false; BIG = true walks big_tiles instead
+    __shared__ uint32_t flags[4];   // [0..2] TileSort::run, [3] the CTA's current ticket
     if (im.totals[2]) return;                   // planned mode overflow
     if constexpr (BIG) {
         __shared__ typename TileSort<kBigItems>::Smem t16;
+        __shared__ __align__(16) uint8_t hits[kSortThreads * kBigItems];
         const uint32_t nbig = im.totals[3];
         for (uint32_t k = blockIdx.x; k < nbig; k += gridDim.x) {
             const uint32_t tile = im.big_tiles[k];
             const uint2 range = im.ranges[tile];
             const int n = (int)(range.y - range.x);
-            TileSort<kBigItems>::run(t16, flags, bl, b.bucket + range.x, n, id_bits, tile, grid_x, range.x, colors, g, b,
+            TileSort<kBigItems>::run(t16, flags, hits, b.bucket + range.x, n, id_bits, tile, grid_x, range.x, colors, g, b,
                                      im.blk_count);
             __syncthreads();
         }
@@ -421,15 +409,24 @@ __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_s
             typename TileSort<3>::Smem t3;
             typename TileSort<4>::Smem t4;
         } temp;
-        const uint32_t tile = im.tile_order[blockIdx.x];       // longest lists first: the last wave holds the short ones
-        const uint2 range = im.ranges[tile];
-        const int n = (int)(range.y - range.x);
-        if (n == 0 || n > (int)kBigTile) return;
-        const uint2* __restrict__ src = b.bucket + range.x;
-        if (n <= 512) TileSort<1>::run(temp.t1, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
-        else if (n <= 1024) TileSort<2>::run(temp.t2, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
-        else if (n <= 1536) TileSort<3>::run(temp.t3, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
-        else TileSort<4>::run(temp.t4, flags, bl, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+        __shared__ __align__(16) uint8_t hits[kSortThreads * 4];
+#pragma unroll 1
+        for (;;) {
+            if (threadIdx.x == 0) flags[3] = atomicAdd(&im.totals[kSortTicketWord], 1u);
+            __syncthreads();
+            const uint32_t i = flags[3];
+            if (i >= tiles) break;
+            const uint32_t tile = im.tile_order[i];
+            const uint2 range = im.ranges[tile];
+            const int n = (int)(range.y - range.x);
+            if (n == 0) break;                                  // this and every later tile of tile_order is empty
+            const uint2* __restrict__ src = b.bucket + range.x;
+            if (n <= 512) TileSort<1>::run(temp.t1, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+            else if (n <= 1024) TileSort<2>::run(temp.t2, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+            else if (n <= 1536) TileSort<3>::run(temp.t3, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+            else if (n <= (int)kBigTile) TileSort<4>::run(temp.t4, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
+            __syncthreads();                                    // shared memory and flags[3] are reused for the next tile
+        }
     }
 }
 
@@ -440,11 +437,14 @@ int launch_tile_sort_gather(const Camera& cam, int P, uint32_t max_count, const 
     int id_bits = 1;
     while (id_bits < 32 && (1ll << id_bits) < (long long)P) ++id_bits;
     const int tiles = cam.grid_x * cam.grid_y;
-    tile_sort_gather_kernel<false><<<tiles, kSortThreads, 0, stream>>>(colors, g, b, im, id_bits, cam.grid_x);
+    const int ctas = resident_grid((const void*)tile_sort_gather_kernel<false>, kSortThreads);
+    GPSG_REQUIRE(ctas > 0, "tile sort: could not query the occupancy of tile_sort_gather_kernel on the current device");
+    tile_sort_gather_kernel<false><<<min(tiles, ctas), kSortThreads, 0, stream>>>(colors, g, b, im, id_bits, cam.grid_x,
+                                                                                   (uint32_t)tiles);
     GPSG_LAUNCH_CHECK();
     if (max_count > kBigTile) {   // exact mode passes the real maximum; planned mode passes kMaxTileSort (always launch)
         tile_sort_gather_kernel<true><<<min(tiles, kBigTileCTAs), kSortThreads, 0, stream>>>(colors, g, b, im, id_bits,
-                                                                                             cam.grid_x);
+                                                                                             cam.grid_x, (uint32_t)tiles);
         GPSG_LAUNCH_CHECK();
     }
     return GPSG_OK;
@@ -475,16 +475,29 @@ __global__ void __launch_bounds__(256) gather_ranges_kernel(size_t N, const Gaus
     b.slabC[i] = C;
 }
 
-// One CTA per tile, after gather_ranges: the per-block survivor lists from the tile's slabs (any tile length).
+// One CTA per tile, after gather_ranges: the per-block survivor lists from the tile's slabs (any tile length), in chunks of
+// kListChunk positions: the CTA writes the chunk's hit masks to shared memory, then warp k appends block k's survivors.
+constexpr uint32_t kListChunk = 8 * kSortThreads;
 __global__ void __launch_bounds__(kSortThreads) block_lists_kernel(int grid_x, BinningState b, ImageState im) {
-    __shared__ BlockLists bl;
+    __shared__ uint8_t hits[kListChunk];
     const uint32_t tile = blockIdx.x;
     const uint2 range = im.ranges[tile];
     const uint32_t n = range.y - range.x;
     if (n == 0) return;
-    const int tile_y = (int)tile / grid_x;
-    build_block_lists(bl, b.slabA + range.x, n, (int)tile - tile_y * grid_x, tile_y, b.blk_list + 8 * (size_t)range.x,
-                      im.blk_count + 8 * (size_t)tile);
+    const int tile_y = (int)tile / grid_x, tile_x = (int)tile - tile_y * grid_x;
+    const float4* __restrict__ tileA = b.slabA + range.x;
+    const int warp = (int)threadIdx.x >> 5;
+    uint32_t* __restrict__ list = b.blk_list + 8 * (size_t)range.x + (size_t)min(warp, 7) * n;
+    uint32_t cnt = 0u;
+#pragma unroll 1
+    for (uint32_t r0 = 0; r0 < n; r0 += kListChunk) {
+        const uint32_t m = min(kListChunk, n - r0);
+        for (uint32_t i = threadIdx.x; i < m; i += kSortThreads) hits[i] = (uint8_t)block_hit_mask(tileA[r0 + i], tile_x, tile_y);
+        __syncthreads();
+        if (warp < 8) append_block_list(hits, r0, m, warp, list, cnt);
+        __syncthreads();
+    }
+    if (warp < 8 && (threadIdx.x & 31) == 0) im.blk_count[8 * (size_t)tile + warp] = cnt;
 }
 
 int launch_gather_ranges(const Camera& cam, size_t N, const GaussianSrc& colors, GeomState g, BinningState b, ImageState im,

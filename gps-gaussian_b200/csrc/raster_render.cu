@@ -3,7 +3,7 @@
 //
 // Design (not upstream's):
 //  * a warp renders one 8x4 pixel block (fwd_block_origin) and walks that block's own survivor list, built where the
-//    tile list is sorted (raster_binning.cu: build_block_lists).  The list holds exactly the entries whose conservative
+//    tile list is sorted (raster_binning.cu: block_hit_mask).  The list holds exactly the entries whose conservative
 //    alpha >= 1/255 bounding box meets the block, in list order; every other entry is one that all 32 pixels would
 //    `continue` on, so the result is that of walking the whole tile list (n_contrib counts list positions);
 //  * the survivors' slab entries (A, B, C) are copied from the tile's slab range (L2-resident after the sort) with 16-byte
