@@ -208,6 +208,22 @@ lib.gpsg_gs_head_backward_workspace_bytes.restype = _sz
 lib.gpsg_gs_head_backward_workspace_bytes.argtypes = [_i, _i, _i]
 lib.gpsg_gs_head_backward.restype = _i
 lib.gpsg_gs_head_backward.argtypes = [_i, _vp, _i, _i, _i] + [_vp] * 9 + [GsHeadWeights, GsHeadGrads, _vp]
+# GpsgEncoderStemWeights field order (include/gpsg.h)
+ENCODER_STEM_PARAMS = ("in_conv_w", "in_conv_b", "in_norm_w", "in_norm_b") + tuple(
+    f"b{k}_{n}" for k in (1, 2) for n in ("conv1_w", "conv1_b", "norm1_w", "norm1_b", "conv2_w", "conv2_b", "norm2_w",
+                                          "norm2_b"))
+ENCODER_STEM_TF32, ENCODER_STEM_FP16 = 0, 1     # GPSG_ENCODER_STEM_TF32 / _FP16 (include/gpsg.h)
+
+
+class EncoderStemWeights(C.Structure):
+    """GpsgEncoderStemWeights (include/gpsg.h), passed by value: the 20 device pointers of the stem's parameters."""
+    _fields_ = [(n, C.c_void_p) for n in ENCODER_STEM_PARAMS]
+
+
+lib.gpsg_encoder_stem_workspace_bytes.restype = _sz
+lib.gpsg_encoder_stem_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
+lib.gpsg_encoder_stem_forward.restype = _i
+lib.gpsg_encoder_stem_forward.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _vp, EncoderStemWeights, _vp, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -231,7 +247,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_sequence_loss_backward", "gpsg_mesh_render_workspace_bytes", "gpsg_mesh_render", "gpsg_jpeg_parse",
             "gpsg_jpeg_decode_workspace_bytes", "gpsg_jpeg_decode", "gpsg_jpeg_encode_max_bytes",
             "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode", "gpsg_gs_head_workspace_bytes",
-            "gpsg_gs_head_forward", "gpsg_gs_head_backward_workspace_bytes", "gpsg_gs_head_backward"]
+            "gpsg_gs_head_forward", "gpsg_gs_head_backward_workspace_bytes", "gpsg_gs_head_backward",
+            "gpsg_encoder_stem_workspace_bytes", "gpsg_encoder_stem_forward"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

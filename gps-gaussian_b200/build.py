@@ -36,6 +36,7 @@ SOURCES = {
     "rectify.cu": ["-fmad=false"],
     "flow_head.cu": [],
     "gs_head.cu": [],
+    "encoder_stem.cu": [],
     "mesh_render.cu": ["-fmad=false"],
     "jpeg_decode.cu": [],
     "jpeg_encode.cu": [],

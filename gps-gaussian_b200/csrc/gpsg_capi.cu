@@ -972,6 +972,31 @@ int gpsg_gs_head_backward(int device, void* stream_, int B, int H, int W, const 
                               grads, workspace, (cudaStream_t)stream_);
 }
 
+static bool encoder_stem_shape_ok(int B, int Cin, int H, int W, int precision) {
+    return B >= 0 && H >= 1 && W >= 1 && H <= 65536 && W <= 65536 && (Cin == 1 || Cin == 3) &&
+           (precision == GPSG_ENCODER_STEM_TF32 || precision == GPSG_ENCODER_STEM_FP16) &&
+           (int64_t)B * ((H + 1) / 2) * ((W + 1) / 2) * 32 < (int64_t(1) << 40);
+}
+
+size_t gpsg_encoder_stem_workspace_bytes(int B, int Cin, int H, int W, int precision) {
+    return (B > 0 && encoder_stem_shape_ok(B, Cin, H, W, precision))
+               ? encoder_stem_workspace_bytes(B, Cin, H, W, precision) : 0;
+}
+
+int gpsg_encoder_stem_forward(int device, void* stream_, int B, int Cin, int H, int W, int precision,
+                              const float* input, GpsgEncoderStemWeights weights, float* x1_out, void* workspace) {
+    GPSG_REQUIRE(encoder_stem_shape_ok(B, Cin, H, W, precision),
+                 "encoder_stem: needs Cin 1 or 3, H, W >= 1, B >= 0 and a known precision");
+    if (B == 0) return GPSG_OK;
+    GPSG_REQUIRE(input && x1_out && workspace, "NULL pointer");
+    const float* const* w = &weights.in_conv_w;
+    for (int i = 0; i < 20; ++i) GPSG_REQUIRE(w[i], "encoder_stem: NULL weight pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 256 == 0, "encoder_stem: workspace must be 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_encoder_stem(device, B, Cin, H, W, precision, input, weights, x1_out, workspace,
+                               (cudaStream_t)stream_);
+}
+
 int gpsg_set_corr_build(int mode) {
     set_corr_build_mode(mode);
     return GPSG_OK;

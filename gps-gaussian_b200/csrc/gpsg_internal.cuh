@@ -277,6 +277,10 @@ int launch_gs_head_bwd(int device, int B, int H, int W, const float* src, const 
                        const float* mid, const float* g_rot, const float* g_scale, const float* g_opacity,
                        const GpsgGsHeadWeights& wt, float* d_src, float* d_depth, const GpsgGsHeadGrads& grads,
                        void* workspace, cudaStream_t stream);
+// encoder_stem.cu
+size_t encoder_stem_workspace_bytes(int B, int Cin, int H, int W, int precision);
+int launch_encoder_stem(int device, int B, int Cin, int H, int W, int precision, const float* x,
+                        const GpsgEncoderStemWeights& wt, float* x1, void* workspace, cudaStream_t stream);
 int launch_sequence_loss_fwd(const GpsgSeqLossArgs& a, float* stats, void* workspace, cudaStream_t stream);
 int launch_sequence_loss_bwd(const GpsgSeqLossArgs& a, const float* grad_loss, const float* stats, cudaStream_t stream);
 // corr.cu

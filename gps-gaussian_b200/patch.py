@@ -65,6 +65,18 @@ the kernels forward and backward (gs_head.gs_head_train) when the image does not
 inputs the kernels do not cover, the reference's own forward runs.  The gradients differ from cuDNN's by TF32
 re-association, which is why this switch is opt-in too; `GPSG_GS_HEAD=1` alone keeps the training step on cuDNN.
 
+`GPSG_ENCODER=1`, read once by `install()`, also hooks `core.extractor` and rebinds
+
+    UnetExtractor.forward -> encoder.make_extractor_forward (a class method, kept in _ORIG_METHODS)
+
+which covers the image encoder (lib/network.py) and the regressor's depth encoder (lib/gs_parm_network.py): with
+autograd off, the half-resolution stem (in_ds + res1) runs on the kernels of csrc/encoder_stem.cu
+(gps_gaussian_b200.encoder) in TF32 when autocast is off and cudnn.allow_tf32 is on, in fp16 under CUDA autocast in
+fp16; res2 and res3 stay the module's own.  With grad enabled, bf16 autocast, allow_tf32 off or inputs and modules
+the kernels do not cover, the reference's own forward runs unchanged.  x1 differs from cuDNN's by TF32 or fp16
+re-association, which is why the switch is opt-in.  It composes with GPSG_GS_HEAD / GPSG_GS_HEAD_TRAIN, whose rebound
+regressor calls its depth encoder as a module.  Unset or any other value leaves `core.extractor` alone.
+
 `taichi_three` and its submodules always resolve to the stand-in in dropin/taichi_three (the dataset renderer on
 csrc/mesh_render.cu).  `python prepare_data/render_data.py` puts prepare_data/ first on sys.path, where the reference's
 own package, which cannot import without Taichi, would shadow anything on PYTHONPATH.
@@ -84,6 +96,7 @@ _DECODE = False       # GPSG_DECODE=1 at install()
 _ENCODE = False       # GPSG_ENCODE=1 at install()
 _GS_HEAD = False      # GPSG_GS_HEAD=1 at install()
 _GS_HEAD_TRAIN = False  # GPSG_GS_HEAD_TRAIN=1 at install()
+_ENCODER = False      # GPSG_ENCODER=1 at install()
 
 
 def _set(mod, attr, new):
@@ -199,6 +212,15 @@ def _patch_regresser(mod):
     cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key], train=_GS_HEAD_TRAIN)
 
 
+def _patch_extractor(mod):
+    from gps_gaussian_b200 import encoder
+    cls = mod.UnetExtractor
+    key = (cls, "forward")
+    if key not in _ORIG_METHODS:
+        _ORIG_METHODS[key] = cls.__dict__["forward"]
+    cls.forward = encoder.make_extractor_forward(_ORIG_METHODS[key])
+
+
 _JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
 _JPEG_SAMPLING = {0x111111: "444", 0x211111: "422", 0x221111: "420"}   # cv2.IMWRITE_JPEG_SAMPLING_FACTOR_444/422/420
 _IMWRITE_JPEG_QUALITY, _IMWRITE_JPEG_SAMPLING_FACTOR = 1, 7
@@ -307,11 +329,13 @@ _RECTIFY_TARGETS = {"lib.human_loader": _patch_loader}
 _FLOW_HEAD_TARGETS = {"core.raft_stereo_human": _patch_upsample, "lib.loss": _patch_loss}
 _ENCODE_TARGETS = {"cv2": _patch_cv2}
 _GS_HEAD_TARGETS = {"lib.gs_parm_network": _patch_regresser}
+_ENCODER_TARGETS = {"core.extractor": _patch_extractor}
 
 
 def _targets():
     return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {}),
-            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD or _GS_HEAD_TRAIN else {})}
+            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD or _GS_HEAD_TRAIN else {}),
+            **(_ENCODER_TARGETS if _ENCODER else {})}
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -361,8 +385,8 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD and GPSG_GS_HEAD_TRAIN here, once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN
+    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN and GPSG_ENCODER here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
@@ -370,6 +394,7 @@ def install():
     _ENCODE = os.environ.get("GPSG_ENCODE", "") == "1"
     _GS_HEAD = os.environ.get("GPSG_GS_HEAD", "") == "1"
     _GS_HEAD_TRAIN = os.environ.get("GPSG_GS_HEAD_TRAIN", "") == "1"
+    _ENCODER = os.environ.get("GPSG_ENCODER", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -437,3 +462,9 @@ def gs_head_train():
     """Whether the installed patch also trains the regressor's full-resolution tail on the fused kernels, forward and
     backward (GPSG_GS_HEAD_TRAIN=1 at install())."""
     return _GS_HEAD_TRAIN
+
+
+def encoder():
+    """Whether the installed patch runs the UnetExtractor's half-resolution stem on the fused kernels (GPSG_ENCODER=1 at
+    install())."""
+    return _ENCODER

@@ -577,6 +577,44 @@ GPSG_API int gpsg_gs_head_backward(int device, void* stream, int B, int H, int W
                                    const float* g_opacity, float* d_src, float* d_depth, GpsgGsHeadWeights weights,
                                    GpsgGsHeadGrads grads, void* workspace);
 
+/* ---- half-resolution stem of the UnetExtractor (reference core/extractor.py: in_ds + res1), inference ------------------
+ * gpsg_encoder_stem_forward: x1 [B,32,Ho,Wo] (NCHW fp32, Ho = ceil(H/2), Wo = ceil(W/2)), the output of res1, from the
+ * input [B,Cin,H,W] (NCHW fp32, Cin 1 or 3, H, W >= 1):
+ *   x0 = relu(GN8(conv5x5(input, in_conv_w, in_conv_b; stride 2, zero padding 2)))
+ *   per residual block k = 1, 2 (input x, no downsample branch):
+ *     h = relu(GN4(conv3x3(x, bk_conv1_w, bk_conv1_b)));  g = relu(GN4(conv3x3(h, bk_conv2_w, bk_conv2_b)));
+ *     out = relu(x + g)
+ *   GNg(y): GroupNorm with g groups over 32 channels per sample, biased variance, (y - mean) / sqrt(var + 1e-5) times
+ *   the channel's weight plus its bias (evaluated as fmaf(y, A, C) with A = w rstd and C = b - mean A in fp32, the
+ *   statistics in fp64).  A non-finite value in a (sample, group) makes that group NaN; ReLU keeps NaN.
+ *   Weights in torch's layouts, every tensor fp32 and contiguous: in_conv_w [32,Cin,5,5], the 3x3 weights [32,32,3,3],
+ *   biases and the GroupNorm weights / biases [32].
+ *   precision GPSG_ENCODER_STEM_TF32 (cuDNN with allow_tf32): every convolution operand, weights and activations, rounded
+ *     to TF32 (round to nearest, ties away); products and sums fp32 in an unspecified order; the bias added in fp32.
+ *   precision GPSG_ENCODER_STEM_FP16 (CUDA autocast in fp16): the convolution operands (the input, each convolution's
+ *     normalized input, the weights) and the biases rounded to fp16 (round to nearest even); products and sums fp32;
+ *     each convolution's output, bias included, rounded to fp16 before GroupNorm reads it; GroupNorm, ReLU and the
+ *     residual add in fp32.
+ *   Bit-reproducible: no floating-point atomics; every sum has a fixed order given the shape and the device's SM count.
+ *   workspace: gpsg_encoder_stem_workspace_bytes(B, Cin, H, W, precision) bytes, 256-byte aligned.  After the call it
+ *   starts with the five raw convolution outputs y0 .. y4 (bias included, NHWC [B,Ho,Wo,32], fp32 in TF32 mode, fp16 in
+ *   FP16 mode), y_i at byte i * S with S = B Ho Wo 32 sizeof(element) rounded up to a multiple of 256; then the
+ *   per-channel A, C and the per-tile GroupNorm partials.  B >= 0.
+ *   Enqueues on `stream` and does not synchronise. */
+#define GPSG_ENCODER_STEM_TF32 0
+#define GPSG_ENCODER_STEM_FP16 1
+typedef struct GpsgEncoderStemWeights {
+    const float* in_conv_w; const float* in_conv_b; const float* in_norm_w; const float* in_norm_b;
+    const float* b1_conv1_w; const float* b1_conv1_b; const float* b1_norm1_w; const float* b1_norm1_b;
+    const float* b1_conv2_w; const float* b1_conv2_b; const float* b1_norm2_w; const float* b1_norm2_b;
+    const float* b2_conv1_w; const float* b2_conv1_b; const float* b2_norm1_w; const float* b2_norm1_b;
+    const float* b2_conv2_w; const float* b2_conv2_b; const float* b2_norm2_w; const float* b2_norm2_b;
+} GpsgEncoderStemWeights;
+GPSG_API size_t gpsg_encoder_stem_workspace_bytes(int B, int Cin, int H, int W, int precision);
+GPSG_API int gpsg_encoder_stem_forward(int device, void* stream, int B, int Cin, int H, int W, int precision,
+                                       const float* input, GpsgEncoderStemWeights weights, float* x1_out,
+                                       void* workspace);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.
