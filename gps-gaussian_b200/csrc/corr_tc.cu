@@ -18,7 +18,7 @@
 // 96 KB of shared memory per CTA at D = 192, N = 128: two CTAs per SM, so one CTA's loads overlap the other's MMA +
 // epilogue.  HBM-bound by design: 2*D*W*2 B in, 1.875*W1*W2*2 B out per (b, h).
 #include "gpsg_internal.cuh"
-#include "tma_bulk.cuh"
+#include "sm90_ptx.cuh"
 
 #include <cuda_fp16.h>
 
@@ -26,38 +26,10 @@ namespace gpsg {
 
 namespace {
 
+using namespace sm90;
+
 constexpr int kTcThreads = 256;
 constexpr int kTcM = 128;              // volume rows per CTA: warpgroup g owns rows 64g .. 64g+63
-
-// shared-memory matrix descriptor (sm_90 GMMA), no swizzle (layout type 0); address and offsets in 16-byte units
-__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    return d;
-}
-
-// D[64 x 16] (+)= A[64 x 16] B[16 x 16], fp16 in, fp32 accumulate; TA / TB = 1: the operand is MN-major in shared memory
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, int accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB)
-        : "memory");
-}
-
-// keeps the compiler from moving accesses of the accumulators across the asynchronous MMAs that own them
-template <int NC>
-__device__ __forceinline__ void fence_acc(float (&acc)[NC][8]) {
-#pragma unroll
-    for (int c = 0; c < NC; ++c)
-#pragma unroll
-        for (int i = 0; i < 8; ++i) asm volatile("" : "+f"(acc[c][i])::"memory");
-}
 
 // acc[c] = A x B[:, 16c .. 16c+15] for c < nch over ksteps K-steps of 16.  a0 / b0: shared addresses of this warpgroup's
 // A rows and of the B panel; A's K-adjacent core groups are 2048 B apart, B's lbo_b; MN-adjacent cores 128 B apart.
@@ -69,22 +41,18 @@ __device__ __forceinline__ void warpgroup_mma(float (&acc)[NC][8], uint32_t a0, 
 #pragma unroll
         for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
     fence_acc(acc);
-    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    wgmma_fence();
     for (int s = 0; s < ksteps; ++s) {
         const uint64_t da = gmma_desc(a0 + (uint32_t)s * 2u * 2048u, 2048u, 128u);
 #pragma unroll
         for (int c = 0; c < NC; ++c)
             if (c < nch)
-                wgmma_m64n16k16<TA, TB>(acc[c], da, gmma_desc(b0 + (uint32_t)s * 2u * lbo_b + (uint32_t)c * 256u, lbo_b, 128u),
-                                        s > 0);
+                wgmma_m64n16k16_f16<TA, TB>(acc[c], da,
+                                            gmma_desc(b0 + (uint32_t)s * 2u * lbo_b + (uint32_t)c * 256u, lbo_b, 128u), s > 0);
     }
-    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    wgmma_commit();
+    wgmma_wait();
     fence_acc(acc);
-}
-
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, uint32_t src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(src_bytes) : "memory");
 }
 
 // correctly rounded a / d from r = RN(1/d) with one Newton correction (Markstein): q0 = a r; q = q0 + (a - q0 d) r.
@@ -141,21 +109,21 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_tc_kernel(int D, int H,
     for (int it = warp; it < KC * 4; it += kTcThreads / 32) {
         const int kc = it >> 2, c = (it & 3) * 4 + cl;
         const bool in = x_base + c * 8 < W1;                      // ragged last M tile: zero-fill (src-size 0)
-        cp_async16(sA + (size_t)kc * 2048 + c * 128 + dl * 16, in ? g1 + (size_t)(kc * 8 + dl) * plane1 + c * 8 : g1, in ? 16u : 0u);
+        cp_async16_zfill(sA + (size_t)kc * 2048 + c * 128 + dl * 16, in ? g1 + (size_t)(kc * 8 + dl) * plane1 + c * 8 : g1, in ? 16u : 0u);
     }
     const int NBg = (NB + 3) >> 2;
     for (int it = warp; it < KC * NBg; it += kTcThreads / 32) {
         const int kc = it / NBg, c = (it % NBg) * 4 + cl;
-        if (c < NB) cp_async16(sB + ((size_t)kc * NB + c) * 128 + dl * 16, g2 + (size_t)(kc * 8 + dl) * plane2 + c * 8, 16u);
+        if (c < NB) cp_async16_zfill(sB + ((size_t)kc * NB + c) * 128 + dl * 16, g2 + (size_t)(kc * 8 + dl) * plane2 + c * 8, 16u);
     }
-    asm volatile("cp.async.wait_all;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+    cp_async_wait_all();
+    fence_async();                                               // generic-proxy writes -> visible to the tensor core
     __syncthreads();
 
     // ---- MMA: warpgroup wg computes volume rows 64 wg .. 64 wg + 63, all N columns --------------------------------------
     const int wg = warp >> 2, wwg = warp & 3;
     float acc[8][8];
-    warpgroup_mma<1, 1>(acc, smem_u32(sA) + (uint32_t)wg * 1024u, smem_u32(sB), (uint32_t)NB * 128u, D >> 4, W2 >> 4);
+    warpgroup_mma<1, 1>(acc, smem_addr(sA) + (uint32_t)wg * 1024u, smem_addr(sB), (uint32_t)NB * 128u, D >> 4, W2 >> 4);
     __syncthreads();                                             // both warpgroups are done reading the panels
 
     // ---- epilogue 1: scale + round to fp16 into a [128][W2 + 8] tile over the panels (row pad: conflict-free stores) ----
@@ -243,7 +211,7 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_bwd_tc_kernel(int D, in
             const int kc = it >> 2, c = (it & 3) * 4 + cl;
             const int x = kc * 8 + dl;
             const bool in = x < W1 && c * 8 < W2;
-            cp_async16(sA + (size_t)kc * 2048 + c * 128 + dl * 16, in ? gbh + (size_t)x * W2 + c * 8 : gbh, in ? 16u : 0u);
+            cp_async16_zfill(sA + (size_t)kc * 2048 + c * 128 + dl * 16, in ? gbh + (size_t)x * W2 + c * 8 : gbh, in ? 16u : 0u);
         }
     } else {         // g[x][y]: m = x (row), K cores = chunks of 8 y
         for (int it = warp; it < 16 * KCg; it += kTcThreads / 32) {
@@ -251,7 +219,7 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_bwd_tc_kernel(int D, in
             const int x = m_base + m8 * 8 + dl;
             if (kc < KC) {
                 const bool in = x < W1 && kc * 8 < W2;
-                cp_async16(sA + (size_t)kc * 2048 + m8 * 128 + dl * 16, in ? gbh + (size_t)x * W2 + kc * 8 : gbh, in ? 16u : 0u);
+                cp_async16_zfill(sA + (size_t)kc * 2048 + m8 * 128 + dl * 16, in ? gbh + (size_t)x * W2 + kc * 8 : gbh, in ? 16u : 0u);
             }
         }
     }
@@ -261,17 +229,17 @@ __global__ void __launch_bounds__(kTcThreads) corr_build_bwd_tc_kernel(int D, in
         const int d8 = it / KCg, kc = (it % KCg) * 4 + cl;
         if (kc < KC) {
             const bool in = kc * 8 < Kdim;
-            cp_async16(sB + ((size_t)kc * NB + d8) * 128 + dl * 16, in ? fb + (size_t)(d8 * 8 + dl) * plane + kc * 8 : fb,
-                       in ? 16u : 0u);
+            cp_async16_zfill(sB + ((size_t)kc * NB + d8) * 128 + dl * 16, in ? fb + (size_t)(d8 * 8 + dl) * plane + kc * 8 : fb,
+                             in ? 16u : 0u);
         }
     }
-    asm volatile("cp.async.wait_all;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    cp_async_wait_all();
+    fence_async();
     __syncthreads();
 
     const int wg = warp >> 2, wwg = warp & 3;
     float acc[16][8];
-    warpgroup_mma<A_MN ? 1 : 0, 0>(acc, smem_u32(sA) + (uint32_t)wg * 1024u, smem_u32(sB), (uint32_t)NB * 128u, KC >> 1, D >> 4);
+    warpgroup_mma<A_MN ? 1 : 0, 0>(acc, smem_addr(sA) + (uint32_t)wg * 1024u, smem_addr(sB), (uint32_t)NB * 128u, KC >> 1, D >> 4);
     __syncthreads();                                             // both warpgroups are done reading the panels
 
     const float rdiv = __frcp_rn(div);

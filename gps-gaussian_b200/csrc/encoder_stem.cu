@@ -51,7 +51,7 @@
 #include <stdint.h>
 
 #include "gpsg_internal.cuh"
-#include "wgmma_sm90.cuh"
+#include "sm90_ptx.cuh"
 
 namespace gpsg {
 namespace {
@@ -343,9 +343,7 @@ stem_conv(int B, int Ho, int Wo, const typename Prec<H>::T* __restrict__ ya, con
         fence_acc(acc[1]);
         // the descriptors are the same for every tile: made opaque here so that they are not hoisted out of the tile loop
         // and kept live in registers
-        uint32_t aB, wB;
-        asm volatile("mov.u32 %0, %1;" : "=r"(aB) : "r"(aBase));
-        asm volatile("mov.u32 %0, %1;" : "=r"(wB) : "r"(wBase));
+        const uint32_t aB = opaque(aBase), wB = opaque(wBase);
         wgmma_fence();
         const uint64_t aD = gmma_desc(aB, kHY * kHX * 16, 128), wD = gmma_desc(wB, kC * 16, 128);
 #pragma unroll 1

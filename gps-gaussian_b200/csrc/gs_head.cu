@@ -59,7 +59,7 @@
 #include <stdint.h>
 
 #include "gpsg_internal.cuh"
-#include "wgmma_sm90.cuh"
+#include "sm90_ptx.cuh"
 
 namespace gpsg {
 namespace {
@@ -88,23 +88,6 @@ constexpr size_t kSmem2 = (size_t)(2 * kA2Floats + kW2Floats + 8 * kMidC) * size
 static_assert(kSmem1 <= 227 * 1024 && kSmem2 <= 227 * 1024, "shared memory");
 
 __device__ __forceinline__ float relu(float x) { return x < 0.f ? 0.f : x; }
-
-// D[64 x 96] += A[64 x 8] B[8 x 96]: TF32 operands from K-major shared memory, fp32 accumulators
-__device__ __forceinline__ void wgmma_m64n96k8(float (&d)[48], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-        : "l"(a_desc), "l"(b_desc), "n"(1)
-        : "memory");
-}
-
-__device__ __forceinline__ void cp_async16_zfill(void* smem, const void* gmem, bool valid) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr(smem)), "l"(gmem), "r"(valid ? 16 : 0)
-                 : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // torch's upsample_bilinear2d source index for scale 2, align_corners=False: (dst + 0.5) * 0.5 - 0.5, clamped at 0;
 // the upper neighbour is clamped to the last row / column.
@@ -261,7 +244,7 @@ __device__ __forceinline__ void halo_issue(float* sA, const float* t, int H, int
         const int y = y0 + hy - 1, x = x0 + hx - 1;
         const bool in = y >= 0 && y < H && x >= 0 && x < W;
         const float* p = in ? t + (((size_t)b * H + y) * W + x) * (4 * G) + grp * 4 : t;
-        cp_async16_zfill(sA + ((grp * HY + hy) * kHX + hx) * 4, p, in);
+        cp_async16_zfill(sA + ((grp * HY + hy) * kHX + hx) * 4, p, in ? 16u : 0u);
     }
 }
 
@@ -424,26 +407,6 @@ constexpr int kPart1 = kRedW2;
 constexpr int kPartW1 = kHeadN * kMidC * 9 + kHeadN;          // dW1 [96][32][9] + db1 [96]
 constexpr int kPartWo = kMidC * kInC * 9 + kMidC;             // dW_out [32][52][9] + db_out [32]
 static_assert(kSmemB1 <= 227 * 1024 && kSmemB2 <= 227 * 1024 && kSmemB3 <= 227 * 1024, "shared memory");
-
-// D[64 x 56] += A[64 x 8] B[8 x 56]: TF32 operands from K-major shared memory, fp32 accumulators
-__device__ __forceinline__ void wgmma_m64n56k8(float (&d)[28], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %30, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n56k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27}, %28, %29, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
-        : "l"(a_desc), "l"(b_desc), "n"(1)
-        : "memory");
-}
-
-// D[16 x 8] += A[16 x 8] B[8 x 8], TF32 operands in registers (already TF32 values), fp32 accumulators
-__device__ __forceinline__ void mma_m16n8k8(float (&d)[4], const float (&a)[4], float b0, float b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-                 "{%0, %1, %2, %3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])),
-                   "r"(__float_as_uint(a[3])), "r"(__float_as_uint(b0)), "r"(__float_as_uint(b1)));
-}
 
 // Heads backward.  Recomputes pre = conv1x1(h) + b2 from mid exactly as stage 2 does (same MMAs, same FFMA order), then
 // per pixel: dpre through normalize / softplus + clamp / sigmoid as torch's autograd computes them, dh = [h > 0]

@@ -2,10 +2,13 @@
 // backward.cu::renderCUDA / computeCov2DCUDA / preprocessCUDA, reached from
 // _RasterizeGaussians.backward behind reference gaussian_renderer/__init__.py:54-62).
 #include "gpsg_internal.cuh"
+#include "sm90_ptx.cuh"
 #include "slab_ring.cuh"
 
 
 namespace gpsg {
+
+using namespace sm90;
 
 constexpr int kBwdChunk = 64;   // Gaussians per ring stage
 #ifndef GPSG_BWD_STAGES
@@ -238,8 +241,7 @@ __global__ void __launch_bounds__((kBwdWarps + 1) * 32, MIN_BLOCKS) render_backw
     auto chain = [&](const float4& xq, const float4& q, const float4& c, float G, bool active) {
         const float Ge = active ? G : 0.0f;
         const float alpha_e = fminf(0.99f, q.w * Ge);
-        float inv1ma;                                 // 1 - alpha >= 0.01: MUFU.RCP (1 ulp) without the slow path
-        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv1ma) : "f"(1.0f - alpha_e));
+        const float inv1ma = rcp_approx(1.0f - alpha_e);   // 1 - alpha >= 0.01: MUFU.RCP (1 ulp) without the slow path
         T *= inv1ma;
         accum0 = fmaf(last_alpha, lastc0 - accum0, accum0);
         accum1 = fmaf(last_alpha, lastc1 - accum1, accum1);

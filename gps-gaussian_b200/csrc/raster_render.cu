@@ -15,9 +15,11 @@
 //  * tiles are taken longest list first (tile_order from the tile scan), so the longest lists do not start last;
 //  * the conic arrives pre-scaled into the log2 domain, so alpha = o * ex2(p) with p a 5-op polynomial.
 #include "gpsg_internal.cuh"
-#include "slab_ring.cuh"   // ex2_approx
+#include "sm90_ptx.cuh"
 
 namespace gpsg {
+
+using namespace sm90;
 
 // ---- two survivors of the same pixel evaluated side by side: their conic polynomials are independent (only the
 // transmittance blend is sequential), so both are computed as a pair of values with explicitly rounded IEEE operations in
@@ -82,18 +84,6 @@ __device__ __forceinline__ void fwd_eval_pair(const float4& a0, const float4& a1
         px.last = upd ? (u ? pos.y : pos.x) : px.last;
     }
 }
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem)
-                 : "memory");
-}
-__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem)
-                 : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // AUX (aux mode): also composites the view-space depth z of every Gaussian as a fourth colour channel with background 0,
 // D = sum_i alpha_i T_i z_i, and writes alpha = 1 - T beside final_T.  z is gathered per survivor from the geometry

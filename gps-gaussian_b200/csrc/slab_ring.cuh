@@ -1,4 +1,5 @@
-// slab_ring.cuh -- warp-specialised slab pipeline shared by the compositing forward and backward kernels.
+// slab_ring.cuh -- warp-specialised slab pipeline of the compositing backward kernel (raster_backward.cu).  The forward
+// walks per-warp survivor lists instead (raster_render.cu).
 //
 // One producer lane streams a tile's sorted Gaussian slabs (three float4 arrays, see raster_binning.cu) into a
 // ring of shared-memory stages with 1-D TMA bulk copies; each stage has a `full` transaction barrier (armed by
@@ -11,18 +12,6 @@
 
 namespace gpsg {
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
-constexpr float kLog2e = 1.4426950408889634f;
-constexpr float kLn2 = 0.6931471805599453f;
-
 template <int CHUNK, int STAGES>
 struct __align__(128) SlabRing {
     float4 A[STAGES][CHUNK];  // x, y, cull half-extent x, y
@@ -30,7 +19,7 @@ struct __align__(128) SlabRing {
     float4 C[STAGES][CHUNK];  // r, g, b, Gaussian id bits
     uint64_t full[STAGES];
     uint64_t empty[STAGES];
-    int done_warps;           // consumer warps that have nothing left to do (forward early-out)
+    int done_warps;           // consumer warps that have nothing left to do (the backward reports none)
     int hi;                   // backward: deepest list position any pixel of the CTA contributes to
 };
 

@@ -1,0 +1,151 @@
+// sm90_ptx.cuh -- every inline-PTX wrapper but the TMA bulk copies and mbarriers (tma_bulk.cuh): shared-memory
+// addresses, TF32 rounding, the warpgroup MMAs (wgmma), their descriptors and fences, the TF32 mma.sync, the cp.async
+// family and single SFU / move instructions.  Instruction forms whose PTX differs are separate wrappers.  sm_90a only.
+#pragma once
+#include <stdint.h>
+
+namespace gpsg {
+namespace sm90 {
+
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// round to TF32 (10 explicit mantissa bits): to nearest, ties away from zero, as cuDNN / cuBLAS round in TF32 mode
+__device__ __forceinline__ float tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+
+// 2^x on the SFU (MUFU.EX2), denormals flushed
+__device__ __forceinline__ float ex2_approx(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+
+// 1/x on the SFU (MUFU.RCP, 1 ulp), without the slow path of the IEEE reciprocal; denormals flushed
+__device__ __forceinline__ float rcp_approx(float x) {
+    float y;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+
+// x, through a move the compiler cannot see through: keeps a loop-invariant value from being hoisted out of a loop
+__device__ __forceinline__ uint32_t opaque(uint32_t x) {
+    uint32_t y;
+    asm volatile("mov.u32 %0, %1;" : "=r"(y) : "r"(x));
+    return y;
+}
+
+// shared-memory matrix descriptor (sm_90), no swizzle; start address and offsets in 16-byte units
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    uint64_t d = 0;
+    d |= (uint64_t)((addr & 0x3FFFFu) >> 4);
+    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
+    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
+    return d;
+}
+
+// D[64 x 32] += A[64 x 8] B[8 x 32]: TF32 operands from K-major shared memory, fp32 accumulators
+__device__ __forceinline__ void wgmma_m64n32k8(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "n"(1)
+        : "memory");
+}
+
+// D[64 x 56] += A[64 x 8] B[8 x 56]: TF32 operands from K-major shared memory, fp32 accumulators
+__device__ __forceinline__ void wgmma_m64n56k8(float (&d)[28], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %30, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n56k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27}, %28, %29, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
+        : "l"(a_desc), "l"(b_desc), "n"(1)
+        : "memory");
+}
+
+// D[64 x 96] += A[64 x 8] B[8 x 96]: TF32 operands from K-major shared memory, fp32 accumulators
+__device__ __forceinline__ void wgmma_m64n96k8(float (&d)[48], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(a_desc), "l"(b_desc), "n"(1)
+        : "memory");
+}
+
+// D[64 x 16] (+)= A[64 x 16] B[16 x 16], f16 operands from shared memory, fp32 accumulators.  TA / TB = 1: the operand is
+// MN-major in shared memory (0: K-major); accumulate = 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16k16_f16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB)
+        : "memory");
+}
+
+// D[64 x 32] += A[64 x 16] B[16 x 32]: f16 operands from K-major shared memory, fp32 accumulators
+__device__ __forceinline__ void wgmma_m64n32k16_f16(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "n"(1)
+        : "memory");
+}
+
+// keeps the compiler from moving accesses of the accumulators across the asynchronous MMAs that own them
+template <int N>
+__device__ __forceinline__ void fence_acc(float (&acc)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+}
+template <int NC>
+__device__ __forceinline__ void fence_acc(float (&acc)[NC][8]) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c) fence_acc(acc[c]);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// generic-proxy shared-memory writes (st.shared, cp.async) -> visible to the tensor core's async proxy
+__device__ __forceinline__ void fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// D[16 x 8] += A[16 x 8] B[8 x 8], TF32 operands in registers (already TF32 values), fp32 accumulators
+__device__ __forceinline__ void mma_m16n8k8(float (&d)[4], const float (&a)[4], float b0, float b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])),
+                   "r"(__float_as_uint(a[3])), "r"(__float_as_uint(b0)), "r"(__float_as_uint(b1)));
+}
+
+// cp.async (LDGSTS) global -> shared copies: 16 bytes cached in L2 only, 16 bytes of which the first src_bytes are read
+// and the rest zero-filled (src_bytes = 0: gmem is not read), 4 bytes cached in L1 and L2
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async16_zfill(void* smem, const void* gmem, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr(smem)), "l"(gmem), "r"(src_bytes)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_addr(smem)), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// every committed group but the most recent one is complete
+__device__ __forceinline__ void cp_async_wait1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+}  // namespace sm90
+}  // namespace gpsg

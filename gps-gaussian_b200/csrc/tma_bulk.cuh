@@ -1,22 +1,28 @@
 // tma_bulk.cuh -- minimal inline-PTX wrappers for 1-D TMA bulk copies (cp.async.bulk, SASS: UBLKCP) and the
-// mbarrier transaction barrier they complete on (sm_90+).  No CUTLASS dependency.
+// mbarrier transaction barrier they complete on (sm_90+).  No CUTLASS dependency.  Every other PTX wrapper is in
+// sm90_ptx.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "sm90_ptx.cuh"
 
 namespace gpsg {
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sm90::smem_addr(bar)), "r"(count) : "memory");
 }
 // make the barrier initialisation visible to the async (TMA) proxy
 __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 // arrive (count 1) and arm the barrier with the number of bytes the bulk copies will deliver
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sm90::smem_addr(bar)), "r"(bytes)
+                 : "memory");
+}
+
+// arrive (count 1) without a transaction count
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(sm90::smem_addr(bar)) : "memory");
 }
 
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
@@ -26,7 +32,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
         "selp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
+        : "r"(sm90::smem_addr(bar)), "r"(parity)
         : "memory");
     return ok != 0;
 }
@@ -41,7 +47,7 @@ __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parit
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
         "selp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity), "r"(ns)
+        : "r"(sm90::smem_addr(bar)), "r"(parity), "r"(ns)
         : "memory");
     return ok != 0;
 }
@@ -51,9 +57,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 
 // global -> shared bulk copy; dst/src 16-B aligned, bytes a multiple of 16; completes `bytes` on `bar`
 __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(smem_dst)),
-                 "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(sm90::smem_addr(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(sm90::smem_addr(bar))
                  : "memory");
 }
 
