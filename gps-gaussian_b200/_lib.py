@@ -3,6 +3,7 @@
 There is NO fallback: if the shared library is missing this module raises at import time --
 a product path that silently ran on the CPU oracle or on eager PyTorch would void every parity
 claim.  Build it with `python gps-gaussian_b200/build.py` (or `__graft_entry__.build()`).
+GPSG_LIB_PATH, if set, names another build of the same library to load (an instrumented variant, tools/sort_phases.py).
 """
 import ctypes as C
 import os
@@ -11,7 +12,7 @@ import threading
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib", "libgpsg_sm90.so")
+LIB_PATH = os.environ.get("GPSG_LIB_PATH") or os.path.join(_HERE, "lib", "libgpsg_sm90.so")
 
 
 class GpsgError(RuntimeError):

@@ -3,6 +3,8 @@
     python gps-gaussian_b200/build.py [--force] [--verbose]
 
 Output: gps-gaussian_b200/lib/libgpsg_sm90.so (git-ignored build product).
+build(defines=[...], out=path) compiles the same sources with extra -D macros (instrumented variants such as
+GPSG_SORT_PHASES, see tools/sort_phases.py) into their own object directory and library.
 raster_preprocess.cu is compiled with -fmad=false (see its header): the fp32 op order that decides
 radii / tile rectangles must not be FMA-contracted.  rectify.cu likewise: its fp32 / fp64 op order is what makes
 the rectified images and flow bit-identical to OpenCV.  mesh_render.cu likewise: its fp32 op order is the mesh oracle's.
@@ -63,9 +65,9 @@ def _stale(dst, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def _compile(name, extra, force, verbose):
+def _compile(name, extra, objdir, force, verbose):
     src = os.path.join(CSRC, name)
-    obj = os.path.join(OBJ, name.replace(".cu", ".o"))
+    obj = os.path.join(objdir, name.replace(".cu", ".o"))
     if not force and not _stale(obj, _deps(src)):
         return obj, ""
     cmd = [_nvcc()] + ARCH + COMMON + extra + ["-c", src, "-o", obj]
@@ -80,19 +82,22 @@ def _compile(name, extra, force, verbose):
     return obj, log
 
 
-def build(force=False, verbose=False):
-    os.makedirs(OBJ, exist_ok=True)
-    os.makedirs(LIBDIR, exist_ok=True)
+def build(force=False, verbose=False, defines=(), out=None):
+    objdir = os.path.join(OBJ, "_".join(defines)) if defines else OBJ
+    lib = out or LIB
+    flags = ["-D" + d for d in defines]
+    os.makedirs(objdir, exist_ok=True)
+    os.makedirs(os.path.dirname(lib), exist_ok=True)
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
-        res = list(ex.map(lambda kv: _compile(kv[0], kv[1], force, verbose), SOURCES.items()))
+        res = list(ex.map(lambda kv: _compile(kv[0], kv[1] + flags, objdir, force, verbose), SOURCES.items()))
     objs = [r[0] for r in res]
-    if force or _stale(LIB, objs):
-        cmd = [_nvcc()] + ARCH + ["-shared", "-o", LIB] + objs + ["-Xcompiler", "-fvisibility=hidden", "-cudart",
+    if force or _stale(lib, objs):
+        cmd = [_nvcc()] + ARCH + ["-shared", "-o", lib] + objs + ["-Xcompiler", "-fvisibility=hidden", "-cudart",
                                                                   "static"]
         p = subprocess.run(cmd, capture_output=True, text=True)
         if p.returncode != 0:
             raise RuntimeError(" ".join(cmd) + "\n" + p.stdout + p.stderr)
-    return LIB
+    return lib
 
 
 if __name__ == "__main__":

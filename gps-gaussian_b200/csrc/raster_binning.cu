@@ -6,8 +6,10 @@
 // list with 1-D TMA bulk copies instead of chasing point_list[] indirections, and the backward
 // re-uses the same slabs.  The same pass detects tile boundaries (identifyTileRanges).
 #include <cub/cub.cuh>
+#include <type_traits>
 #include "gpsg_internal.cuh"
 #include "tile_scan.cuh"
+#include "sm90_ptx.cuh"
 
 namespace gpsg {
 
@@ -176,6 +178,34 @@ __device__ __forceinline__ void slab_entry(uint32_t id, const GaussianSrc& src, 
 constexpr int kSortThreads = 512;
 constexpr int kSortCTAsPerSM = 3;
 
+#ifdef GPSG_SORT_PHASES
+// Phase times of the tile sort, both kernels (tools/sort_phases.py builds a library with this macro; the normal build
+// compiles none of it).  Thread 0 of each CTA adds the %globaltimer nanoseconds since its previous mark to
+// g_sort_phase_ns[k]; every mark sits right after a CTA barrier.  Phases: 0 ticket and range, 1 load and min/max,
+// 2 ordering, 3 fix-up and fallback, 4 gather, 5 survivor lists; word 6 counts the tiles.
+__device__ unsigned long long g_sort_phase_ns[8];
+__shared__ unsigned long long s_sort_clock;
+#define SORT_PHASE(k)                                                                                      \
+    do {                                                                                                   \
+        if (threadIdx.x == 0) {                                                                            \
+            const unsigned long long now_ = sm90::globaltimer();                                           \
+            if ((k) >= 0) atomicAdd(&g_sort_phase_ns[(k) < 0 ? 0 : (k)], now_ - s_sort_clock);             \
+            if ((k) == 0) atomicAdd(&g_sort_phase_ns[6], 1ull);                                            \
+            s_sort_clock = now_;                                                                           \
+        }                                                                                                  \
+    } while (0)
+
+extern "C" GPSG_API int gpsg_sort_phases_read(unsigned long long* out) {   // copies the 8 words out and zeroes them
+    GPSG_CUDA(cudaDeviceSynchronize());
+    GPSG_CUDA(cudaMemcpyFromSymbol(out, g_sort_phase_ns, sizeof(g_sort_phase_ns)));
+    const unsigned long long zero[8] = {};
+    GPSG_CUDA(cudaMemcpyToSymbol(g_sort_phase_ns, zero, sizeof(zero)));
+    return GPSG_OK;
+}
+#else
+#define SORT_PHASE(k) do {} while (0)
+#endif
+
 // ---- per-block survivor lists of the compositing forward (raster_render.cu) ------------------------------------------
 // For each of the 8 warp blocks of a tile (fwd_block_origin), the tile-local list positions of the entries whose cull box
 // (slabA: centre +- half-extents) meets the block, in list order.  Positions are 32-bit: tile lists exceed 65535 entries on
@@ -219,31 +249,95 @@ __device__ __forceinline__ void append_block_list(const uint8_t* hits, uint32_t 
     }
 }
 
-// one CTA per tile: radix sort of the tile's bucket inside the CTA (cub::BlockRadixSort, keys in registers), then the
-// parameter slabs (and, on the exact entry point, the sorted keys and point list) and the per-block survivor lists are
-// written -- the sort and the gather never round-trip to HBM.  The CTA picks the smallest items-per-thread variant that
-// fits.  512 threads: a 2048-entry tile needs only 4 keys + 4 ids per thread, so three CTAs (1536 threads, 40 registers)
-// fit per SM without spills.  Not memoising cub's outer scan and keeping the fix-up and gather loops rolled is what
-// keeps the kernel inside 40 registers.
+// one CTA per tile: the tile's bucket is ordered inside the CTA, then the parameter slabs (and, on the exact entry point, the
+// sorted keys and point list) and the per-block survivor lists are written -- the sort and the gather never round-trip to
+// HBM.  The CTA picks the smallest items-per-thread variant that fits.  512 threads: a 2048-entry tile needs only 4 keys +
+// 4 ids per thread, so three CTAs (1536 threads, 40 registers) fit per SM without spills.  Not memoising cub's outer scan
+// and keeping the fix-up and gather loops rolled is what keeps the kernel inside 40 registers.
 constexpr int kBigItems = (int)kMaxTileSort / kSortThreads;   // big-tile kernel: 8 keys per thread
 template <int ITEMS>
 struct TileSort {
     // 32-bit keys (the tile's depth window) carrying the 32-bit Gaussian id
     using BRS = cub::BlockRadixSort<uint32_t, kSortThreads, ITEMS, uint32_t, 4, /*MEMOIZE_OUTER_SCAN=*/false>;
-    union Smem {
-        typename BRS::TempStorage sort;
-        unsigned long long keys[kSortThreads * ITEMS];   // sorted (depth bits << 32 | id), for the equal-depth fix-up
+    // The counting pass (n <= 2048 only; the big-tile kernel keeps the radix sort): 2^kBucketBits buckets over the depth
+    // window, 4 per thread for the scan.
+    static constexpr bool kCounting = ITEMS <= 4;
+    static constexpr int kBucketBits = 11, kBuckets = 1 << kBucketBits;
+    static_assert(kBuckets == 4 * kSortThreads, "the counter scan gives each thread 4 buckets");
+    struct CountingSmem {
+        __align__(16) uint32_t cnt[kBuckets];    // bucket counts, then each bucket's next free position (uint4 access)
+        uint32_t warp_sum[kSortThreads / 32];
+    };
+    struct Smem {
+        union {
+            typename BRS::TempStorage sort;
+            unsigned long long keys[kSortThreads * ITEMS];   // sorted (depth bits << 32 | id)
+        };
+        std::conditional_t<kCounting, CountingSmem, cub::NullType> c;
     };
 
     // Sorts the tile's entries in (depth bits << 32 | id) order and writes slabs (+ keys and point list if b.keys) and the
-    // per-block survivor lists.
-    //  * only the depth window is radix-sorted: 32-bit keys `depth bits - tile minimum`, whose width is the bit length
-    //    of the tile's depth span (block-wide min/max; about 20 bits on real scenes, at most 31 as depth > 0);
-    //  * the Gaussian id rides along as the value and is NOT radix-sorted: equal-depth runs -- the only place it
-    //    matters -- are found after the sort and ordered by id in shared memory.  A run longer than kMaxRun falls back
-    //    to the full (id, then depth) LSD radix sort, so degenerate inputs (thousands of identical depths) stay correct
-    //    and bounded.
+    // per-block survivor lists.  Keys are re-based on the tile's smallest depth word: the window is w = bit_length(max -
+    // min) bits wide (about 20 on real scenes, at most 31 as depth > 0).
+    //  * n <= 2048: one counting pass puts every entry into its bucket, the top (at most) 11 bits of its window offset,
+    //    and one thread per bucket insertion-sorts the bucket on the full 64-bit key.  Buckets are monotone in depth, so
+    //    this is the whole order.  On real scenes no bucket holds more than about 20 entries; a tile with a bucket longer
+    //    than kMaxBucket (a narrow cluster plus far outliers, or many equal depths) takes the radix path below instead.
+    //  * otherwise only the depth window is radix-sorted; the Gaussian id rides along as the value and is NOT
+    //    radix-sorted: equal-depth runs -- the only place it matters -- are found after the sort and ordered by id in
+    //    shared memory.  A run longer than kMaxRun falls back to the full (id, then depth) LSD radix sort, so degenerate
+    //    inputs (thousands of identical depths) stay correct and bounded.
+    static constexpr int kMaxBucket = 32;
     static constexpr int kMaxRun = 16;
+
+    // Counting pass.  Returns false, before it writes sm.keys, if a bucket holds more than kMaxBucket entries.  The
+    // counters were zeroed before the min/max barriers.
+    __device__ static bool count_sort(Smem& sm, uint32_t* flags, const uint32_t (&keys)[ITEMS],
+                                      const uint32_t (&ids)[ITEMS], int n, uint32_t dlo, int w) {
+        CountingSmem& c = sm.c;
+        const int shift = max(0, w - kBucketBits);
+        const int lane = (int)threadIdx.x & 31, warp = (int)threadIdx.x >> 5;
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k)
+            if (k * kSortThreads + (int)threadIdx.x < n) atomicAdd(&c.cnt[(keys[k] - dlo) >> shift], 1u);
+        __syncthreads();
+        // exclusive scan of the counters; thread t owns buckets 4t .. 4t+3
+        const uint4 q = reinterpret_cast<const uint4*>(c.cnt)[threadIdx.x];
+        const uint32_t sum = q.x + q.y + q.z + q.w;
+        uint32_t incl = sum;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+        }
+        if (lane == 31) c.warp_sum[warp] = incl;
+        if (max(max(q.x, q.y), max(q.z, q.w)) > (uint32_t)kMaxBucket) flags[3] = 1u;
+        __syncthreads();
+        const uint32_t base = __reduce_add_sync(0xffffffffu, lane < warp ? c.warp_sum[lane] : 0u) + incl - sum;
+        reinterpret_cast<uint4*>(c.cnt)[threadIdx.x] = make_uint4(base, base + q.x, base + q.x + q.y, base + q.x + q.y + q.z);
+        const bool ok = flags[3] == 0u;
+        __syncthreads();
+        if (!ok) return false;                  // uniform: flags[3] was settled before the barrier above
+        // placement; the order inside a bucket does not matter: it is sorted next.  Afterwards cnt[j] is bucket j's end.
+#pragma unroll
+        for (int k = 0; k < ITEMS; ++k)
+            if (k * kSortThreads + (int)threadIdx.x < n)
+                sm.keys[atomicAdd(&c.cnt[(keys[k] - dlo) >> shift], 1u)] = ((unsigned long long)keys[k] << 32) | ids[k];
+        __syncthreads();
+#pragma unroll 1
+        for (int j = 4 * (int)threadIdx.x; j < 4 * (int)threadIdx.x + 4; ++j) {   // insertion sort of each bucket
+            const int r = j ? (int)c.cnt[j - 1] : 0, e = (int)c.cnt[j];
+            for (int a = r + 1; a < e; ++a) {
+                const unsigned long long v = sm.keys[a];
+                int d = a - 1;
+                while (d >= r && sm.keys[d] > v) { sm.keys[d + 1] = sm.keys[d]; --d; }
+                sm.keys[d + 1] = v;
+            }
+        }
+        __syncthreads();
+        return true;
+    }
+
     __device__ static void run(Smem& sm, uint32_t* flags, uint8_t* hits, const uint2* __restrict__ src, int n, int id_bits,
                                uint32_t tile, int grid_x, size_t out0, const GaussianSrc& src_in, const GeomState& g,
                                const BinningState& b, uint32_t* __restrict__ blk_count) {
@@ -259,14 +353,36 @@ struct TileSort {
         }
         dmin = __reduce_min_sync(0xffffffffu, dmin);
         dmax = __reduce_max_sync(0xffffffffu, dmax);
-        if (threadIdx.x == 0) { flags[0] = ~0u; flags[1] = 0u; flags[2] = 0u; }
+        if (threadIdx.x == 0) { flags[0] = ~0u; flags[1] = 0u; flags[2] = 0u; flags[3] = 0u; }
+        if constexpr (kCounting) reinterpret_cast<uint4*>(sm.c.cnt)[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u);
         __syncthreads();
         if ((threadIdx.x & 31) == 0) { atomicMin(&flags[0], dmin); atomicMax(&flags[1], dmax); }
         __syncthreads();
-        // Keys are re-based on the tile's smallest depth word so that only w = bit_length(max - min) bits need sorting;
-        // padding keys get bit w, i.e. they are strictly greater than every real key and end up at ranks >= n.
+        SORT_PHASE(1);
         const uint32_t dlo = flags[0];
         const int w = 32 - __clz(flags[1] - dlo);                                  // 0..31 (depth bits < 2^31)
+        bool sorted = false;
+        if constexpr (kCounting) sorted = count_sort(sm, flags, keys, ids, n, dlo, w);
+        SORT_PHASE(2);
+        if (!sorted) {
+            if constexpr (kCounting) {          // reloaded (from L2) rather than held in registers through the counting pass
+#pragma unroll
+                for (int k = 0; k < ITEMS; ++k) {
+                    const int i = k * kSortThreads + (int)threadIdx.x;
+                    const uint2 e = i < n ? src[i] : make_uint2(0u, 0u);
+                    ids[k] = e.x;
+                    keys[k] = e.y;
+                }
+            }
+            radix_sort(sm, flags, keys, ids, n, id_bits, dlo, w);
+        }
+        SORT_PHASE(3);
+        gather_and_lists(sm, hits, n, tile, grid_x, out0, src_in, g, b, blk_count);
+    }
+
+    // The radix path: padding keys get bit w, i.e. they are strictly greater than every real key and end up at ranks >= n.
+    __device__ static void radix_sort(Smem& sm, uint32_t* flags, uint32_t (&keys)[ITEMS], uint32_t (&ids)[ITEMS], int n,
+                                      int id_bits, uint32_t dlo, int w) {
         const uint32_t pad = 1u << w;
 #pragma unroll
         for (int k = 0; k < ITEMS; ++k) keys[k] = (k * kSortThreads + (int)threadIdx.x) < n ? keys[k] - dlo : pad;
@@ -331,6 +447,12 @@ struct TileSort {
                 sm.keys[k * kSortThreads + (int)threadIdx.x] = ((unsigned long long)(keys[k] + dlo) << 32) | ids[k];
             __syncthreads();
         }
+    }
+
+    // Reads the sorted sm.keys.
+    __device__ static void gather_and_lists(Smem& sm, uint8_t* hits, int n, uint32_t tile, int grid_x, size_t out0,
+                                            const GaussianSrc& src_in, const GeomState& g, const BinningState& b,
+                                            uint32_t* __restrict__ blk_count) {
         // ---- gather: each thread takes ranks tid, tid + kSortThreads, ... so every store below is coalesced; the block
         // hit mask of each rank goes to shared memory for the list build (cheaper than reading slab A back from L2 and
         // prefixing per-warp counts across the CTA per 512 positions: DESIGN.md, footnote 10) ----
@@ -356,6 +478,7 @@ struct TileSort {
             }
         }
         __syncthreads();
+        SORT_PHASE(4);
         // ---- per-block survivor lists: warp k writes block k's for positions [0, split), warp k + 8 for [split, n), from
         // the masks of the whole tile.  Warp k + 8 starts at the number of block k's survivors in [0, split), which it
         // counts from the masks itself (4 positions per lane and load); split is a multiple of 128 positions for that ----
@@ -388,19 +511,22 @@ __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_s
                                                                             BinningState b, ImageState im, int id_bits,
                                                                             int grid_x, uint32_t tiles) {
     // tiles = length of tile_order, which bounds the ticket walk of BIG = false; BIG = true walks big_tiles instead
-    __shared__ uint32_t flags[4];   // [0..2] TileSort::run, [3] the CTA's current ticket
+    __shared__ uint32_t flags[5];   // [0..3] TileSort::run, [4] the CTA's current ticket
     if (im.totals[2]) return;                   // planned mode overflow
     if constexpr (BIG) {
         __shared__ typename TileSort<kBigItems>::Smem t16;
         __shared__ __align__(16) uint8_t hits[kSortThreads * kBigItems];
         const uint32_t nbig = im.totals[3];
+        SORT_PHASE(-1);
         for (uint32_t k = blockIdx.x; k < nbig; k += gridDim.x) {
             const uint32_t tile = im.big_tiles[k];
             const uint2 range = im.ranges[tile];
             const int n = (int)(range.y - range.x);
+            SORT_PHASE(0);
             TileSort<kBigItems>::run(t16, flags, hits, b.bucket + range.x, n, id_bits, tile, grid_x, range.x, colors, g, b,
                                      im.blk_count);
             __syncthreads();
+            SORT_PHASE(5);
         }
     } else {
         __shared__ union {
@@ -410,22 +536,25 @@ __global__ void __launch_bounds__(kSortThreads, BIG ? 1 : kSortCTAsPerSM) tile_s
             typename TileSort<4>::Smem t4;
         } temp;
         __shared__ __align__(16) uint8_t hits[kSortThreads * 4];
+        SORT_PHASE(-1);
 #pragma unroll 1
         for (;;) {
-            if (threadIdx.x == 0) flags[3] = atomicAdd(&im.totals[kSortTicketWord], 1u);
+            if (threadIdx.x == 0) flags[4] = atomicAdd(&im.totals[kSortTicketWord], 1u);
             __syncthreads();
-            const uint32_t i = flags[3];
+            const uint32_t i = flags[4];
             if (i >= tiles) break;
             const uint32_t tile = im.tile_order[i];
             const uint2 range = im.ranges[tile];
             const int n = (int)(range.y - range.x);
             if (n == 0) break;                                  // this and every later tile of tile_order is empty
             const uint2* __restrict__ src = b.bucket + range.x;
+            SORT_PHASE(0);
             if (n <= 512) TileSort<1>::run(temp.t1, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
             else if (n <= 1024) TileSort<2>::run(temp.t2, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
             else if (n <= 1536) TileSort<3>::run(temp.t3, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
             else if (n <= (int)kBigTile) TileSort<4>::run(temp.t4, flags, hits, src, n, id_bits, tile, grid_x, range.x, colors, g, b, im.blk_count);
-            __syncthreads();                                    // shared memory and flags[3] are reused for the next tile
+            __syncthreads();                                    // shared memory and flags[4] are reused for the next tile
+            SORT_PHASE(5);
         }
     }
 }

@@ -37,6 +37,13 @@ __device__ __forceinline__ uint32_t opaque(uint32_t x) {
     return y;
 }
 
+// the global nanosecond timer (%globaltimer), comparable across SMs
+__device__ __forceinline__ unsigned long long globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
 // shared-memory matrix descriptor (sm_90), no swizzle; start address and offsets in 16-byte units
 __device__ __forceinline__ uint64_t gmma_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
