@@ -225,6 +225,21 @@ lib.gpsg_encoder_stem_workspace_bytes.restype = _sz
 lib.gpsg_encoder_stem_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
 lib.gpsg_encoder_stem_forward.restype = _i
 lib.gpsg_encoder_stem_forward.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _vp, EncoderStemWeights, _vp, _vp]
+# GpsgDecoder1Weights field order (include/gpsg.h)
+DECODER1_PARAMS = tuple(f"b0_{n}" for n in ("conv1_w", "conv1_b", "norm1_w", "norm1_b", "conv2_w", "conv2_b", "norm2_w",
+                                            "norm2_b", "down_w", "down_b", "norm3_w", "norm3_b")) + tuple(
+    f"b1_{n}" for n in ("conv1_w", "conv1_b", "norm1_w", "norm1_b", "conv2_w", "conv2_b", "norm2_w", "norm2_b"))
+
+
+class Decoder1Weights(C.Structure):
+    """GpsgDecoder1Weights (include/gpsg.h), passed by value: the 20 device pointers of decoder1's parameters."""
+    _fields_ = [(n, C.c_void_p) for n in DECODER1_PARAMS]
+
+
+lib.gpsg_decoder1_workspace_bytes.restype = _sz
+lib.gpsg_decoder1_workspace_bytes.argtypes = [_i, _i, _i]
+lib.gpsg_decoder1_forward.restype = _i
+lib.gpsg_decoder1_forward.argtypes = [_i, _vp, _i, _i, _i, _vp, _vp, _vp, Decoder1Weights, _vp, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -249,7 +264,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_jpeg_decode_workspace_bytes", "gpsg_jpeg_decode", "gpsg_jpeg_encode_max_bytes",
             "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode", "gpsg_gs_head_workspace_bytes",
             "gpsg_gs_head_forward", "gpsg_gs_head_backward_workspace_bytes", "gpsg_gs_head_backward",
-            "gpsg_encoder_stem_workspace_bytes", "gpsg_encoder_stem_forward"]
+            "gpsg_encoder_stem_workspace_bytes", "gpsg_encoder_stem_forward", "gpsg_decoder1_workspace_bytes",
+            "gpsg_decoder1_forward"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

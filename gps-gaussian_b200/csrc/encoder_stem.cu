@@ -36,7 +36,7 @@
 //                      inserts its own warpgroup arrives between taps; the MMAs are a small part of the tile's time).
 //                      <TF32,1> 120 / <TF32,2> 120 / <FP16,1> 113 / <FP16,2> 113 registers;
 //                      TF32 85.5 KB, FP16 42.8 KB dynamic smem (halo + packed weights).
-//   stem_gn_finalize   per (sample, group): the tiles' partials (count, mean, M2) merged by Chan's parallel formula in
+//   gn_finalize<32>    per (sample, group): the tiles' partials (count, mean, M2) merged by Chan's parallel formula in
 //                      fp64, in a fixed order (a strided sequential pass per thread, then a fixed tree); var = M2 / n
 //                      (biased), rstd = 1 / sqrt(var + 1e-5), and per channel A = gamma rstd, C = beta - mean A, rounded
 //                      to fp32; the normalized value is fmaf(y, A, C).  48 registers, 6 KB static smem.
@@ -50,6 +50,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "fused_norm.cuh"
 #include "gpsg_internal.cuh"
 #include "sm90_ptx.cuh"
 
@@ -64,9 +65,6 @@ constexpr int kInPx = 256;             // stem_in tile: 256 consecutive output p
 constexpr int kTW = 64, kHX = kTW + 2; // stem_conv tile: 4 rows x 64 columns, halo 6 x 66
 constexpr int kRows = 4, kHY = kRows + 2;
 constexpr int kGIn = 8, kGRes = 4;     // GroupNorm groups of in_ds and of the residual blocks
-constexpr double kEps = 1e-5;
-
-__device__ __forceinline__ float relu(float x) { return x < 0.f ? 0.f : x; }
 
 // precision traits: T is the type of the stored convolution outputs and of the MMA operands
 template <bool kHalf>
@@ -117,39 +115,6 @@ __device__ __forceinline__ uint4 pack(const float (&v)[Prec<H>::kPer]) {
         q = make_uint4(__float_as_uint(v[0]), __float_as_uint(v[1]), __float_as_uint(v[2]), __float_as_uint(v[3]));
     }
     return q;
-}
-
-// Sum over the CTA of v[G] per group, in a fixed order (an xor-shuffle tree per warp, then the 8 warps in order); every
-// thread gets the result.  red: 8 x G doubles of shared memory, res: G doubles.
-template <int G>
-__device__ __forceinline__ void cta_sum(double (&v)[G], double* red, double* res, int tid) {
-#pragma unroll
-    for (int g = 0; g < G; ++g)
-#pragma unroll
-        for (int o = 16; o >= 1; o >>= 1) v[g] += __shfl_xor_sync(0xffffffffu, v[g], o);
-    if ((tid & 31) == 0)
-#pragma unroll
-        for (int g = 0; g < G; ++g) red[(tid >> 5) * G + g] = v[g];
-    __syncthreads();
-    if (tid < G) {
-        double s = 0.0;
-#pragma unroll
-        for (int k = 0; k < kThreads / 32; ++k) s += red[k * G + tid];
-        res[tid] = s;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int g = 0; g < G; ++g) v[g] = res[g];
-    __syncthreads();
-}
-
-// v[tid] for tid < G without indexing a register array by a runtime value
-template <int G>
-__device__ __forceinline__ double pick(const double (&v)[G], int i) {
-    double r = 0.0;
-#pragma unroll
-    for (int g = 0; g < G; ++g) r = g == i ? v[g] : r;
-    return r;
 }
 
 // ---- in_ds -----------------------------------------------------------------------------------------------------------
@@ -421,47 +386,6 @@ stem_conv(int B, int Ho, int Wo, const typename Prec<H>::T* __restrict__ ya, con
     }
 }
 
-// ---- statistics ------------------------------------------------------------------------------------------------------
-struct Moments {
-    double n, m, m2;
-};
-
-// Chan et al.'s merge of two partial (count, mean, M2); a NaN or inf mean or M2 on either side carries into the result
-__device__ __forceinline__ Moments merge(const Moments& a, const Moments& b) {
-    if (b.n == 0.0) return a;
-    if (a.n == 0.0) return b;
-    const double n = a.n + b.n, d = b.m - a.m;
-    return {n, a.m + d * (b.n / n), a.m2 + b.m2 + d * d * (a.n * b.n / n)};
-}
-
-// one CTA per (sample, group): merge the sample's tile partials, then A, C per channel of the group
-__global__ void __launch_bounds__(kThreads)
-stem_gn_finalize(int G, int64_t tps, const double* __restrict__ part, const float* __restrict__ gamma,
-                 const float* __restrict__ beta, float2* __restrict__ prm) {
-    __shared__ Moments sm[kThreads];
-    const int tid = threadIdx.x, b = blockIdx.x / G, grp = blockIdx.x % G;
-    Moments acc{0.0, 0.0, 0.0};
-    for (int64_t t = tid; t < tps; t += kThreads) {
-        const double* q = part + ((size_t)(b * tps + t) * G + grp) * 3;
-        acc = merge(acc, Moments{q[0], q[1], q[2]});
-    }
-    sm[tid] = acc;
-    __syncthreads();
-    for (int s = kThreads / 2; s >= 1; s >>= 1) {
-        if (tid < s) sm[tid] = merge(sm[tid], sm[tid + s]);
-        __syncthreads();
-    }
-    const int cpg = kC / G;
-    if (tid < cpg) {
-        const Moments m = sm[0];
-        const double var = m.m2 / m.n;                      // biased, as torch
-        const double rstd = 1.0 / sqrt(var + kEps);
-        const int c = grp * cpg + tid;
-        const double A = (double)gamma[c] * rstd;
-        prm[b * kC + c] = make_float2((float)A, (float)((double)beta[c] - m.m * A));
-    }
-}
-
 // ---- output ----------------------------------------------------------------------------------------------------------
 template <bool H>
 __global__ void __launch_bounds__(kThreads)
@@ -542,7 +466,7 @@ int run_stem(int device, int B, int Cin, int Hi, int Wi, const float* x, const G
         k<<<(unsigned)(tiles < cap ? tiles : cap), kThreads, 0, stream>>>(B, Hi, Wi, L.Ho, L.Wo, x, wt.in_conv_w,
                                                                           wt.in_conv_b, y[0], part);
         GPSG_LAUNCH_CHECK();
-        stem_gn_finalize<<<B * kGIn, kThreads, 0, stream>>>(kGIn, L.tps_in, part, wt.in_norm_w, wt.in_norm_b, prm[0]);
+        gn_finalize<kC><<<B * kGIn, kGnThreads, 0, stream>>>(kGIn, L.tps_in, part, wt.in_norm_w, wt.in_norm_b, prm[0]);
         GPSG_LAUNCH_CHECK();
     }
     // the four 3x3 convolutions: (input raw, its params, residual raw, its params) -> output i
@@ -568,7 +492,7 @@ int run_stem(int device, int B, int Cin, int Hi, int Wi, const float* x, const G
             stem_conv<H, 1><<<grid, kThreads, smem, stream>>>(B, L.Ho, L.Wo, y[i], prm[i], nullptr, nullptr, cw[i],
                                                               cb[i], y[i + 1], part);
         GPSG_LAUNCH_CHECK();
-        stem_gn_finalize<<<B * kGRes, kThreads, 0, stream>>>(kGRes, L.tps_conv, part, nw[i], nb[i], prm[i + 1]);
+        gn_finalize<kC><<<B * kGRes, kGnThreads, 0, stream>>>(kGRes, L.tps_conv, part, nw[i], nb[i], prm[i + 1]);
         GPSG_LAUNCH_CHECK();
     }
     const int64_t total = (int64_t)B * L.Ho * L.Wo, blocks = (total + kThreads - 1) / kThreads;

@@ -997,6 +997,27 @@ int gpsg_encoder_stem_forward(int device, void* stream_, int B, int Cin, int H, 
                                (cudaStream_t)stream_);
 }
 
+static bool decoder1_shape_ok(int B, int Hs, int Ws) {
+    return B >= 0 && Hs >= 1 && Ws >= 1 && Hs <= 32768 && Ws <= 32768 &&
+           (int64_t)B * (2 * (int64_t)Hs) * (2 * (int64_t)Ws) * 128 < (int64_t(1) << 40);
+}
+
+size_t gpsg_decoder1_workspace_bytes(int B, int Hs, int Ws) {
+    return (B > 0 && decoder1_shape_ok(B, Hs, Ws)) ? decoder1_workspace_bytes(B, Hs, Ws) : 0;
+}
+
+int gpsg_decoder1_forward(int device, void* stream_, int B, int Hs, int Ws, const float* s, const float* img_feat,
+                          const float* depth_feat, GpsgDecoder1Weights weights, float* out, void* workspace) {
+    GPSG_REQUIRE(decoder1_shape_ok(B, Hs, Ws), "decoder1: needs Hs, Ws >= 1 and B >= 0");
+    if (B == 0) return GPSG_OK;
+    GPSG_REQUIRE(s && img_feat && depth_feat && out && workspace, "NULL pointer");
+    const float* const* w = &weights.b0_conv1_w;
+    for (int i = 0; i < 20; ++i) GPSG_REQUIRE(w[i], "decoder1: NULL weight pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 256 == 0, "decoder1: workspace must be 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_decoder1(device, B, Hs, Ws, s, img_feat, depth_feat, weights, out, workspace, (cudaStream_t)stream_);
+}
+
 int gpsg_set_corr_build(int mode) {
     set_corr_build_mode(mode);
     return GPSG_OK;

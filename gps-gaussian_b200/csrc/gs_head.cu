@@ -58,6 +58,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "fused_norm.cuh"
 #include "gpsg_internal.cuh"
 #include "sm90_ptx.cuh"
 
@@ -86,19 +87,6 @@ constexpr int kA2Floats = (kMidC / 4) * kH2Y * kHX * 4;
 constexpr int kW2Floats = 9 * (kMidC / 4) * kHeadN * 4;
 constexpr size_t kSmem2 = (size_t)(2 * kA2Floats + kW2Floats + 8 * kMidC) * sizeof(float);
 static_assert(kSmem1 <= 227 * 1024 && kSmem2 <= 227 * 1024, "shared memory");
-
-__device__ __forceinline__ float relu(float x) { return x < 0.f ? 0.f : x; }
-
-// torch's upsample_bilinear2d source index for scale 2, align_corners=False: (dst + 0.5) * 0.5 - 0.5, clamped at 0;
-// the upper neighbour is clamped to the last row / column.
-__device__ __forceinline__ void bilinear_index(int dst, int n, int& i0, int& i1, float& l0, float& l1) {
-    float s = ((float)dst + 0.5f) * 0.5f - 0.5f;
-    s = s < 0.f ? 0.f : s;
-    i0 = (int)s;
-    i1 = i0 + (i0 < n - 1 ? 1 : 0);
-    l1 = s - (float)i0;
-    l0 = 1.f - l1;
-}
 
 struct Tiles {
     int tiles_x, tiles_y;

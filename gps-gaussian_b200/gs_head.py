@@ -12,7 +12,10 @@ the gradients of the decoder output, the depth and the 14 weights (not the image
 (the inference scripts and the stage-2 evaluation run under `torch.no_grad()`) and `supported(...)` holds; with grad
 enabled (the training step), under autocast, or for inputs the kernels do not cover, it calls `orig`, the reference's
 own method, unchanged.  `make_regresser_forward(orig, train=True)` also sends a grad-enabled call to `gs_head_train`
-when the image does not require grad.  The maps and gradients differ from cuDNN's TF32 convolutions by TF32
+when the image does not require grad.  `make_regresser_forward(orig, tail=..., decoder=True)` also runs `decoder1` on
+the kernels of gps_gaussian_b200.decoder (autograd and autocast off, cudnn.allow_tf32 on); it is the one restatement of
+the regressor's forward for every combination, and with `tail=False` the tail runs on the module's own layers.  The maps
+and gradients differ from cuDNN's TF32 convolutions by TF32
 re-association; see include/gpsg.h for the exact semantics.
 """
 import ctypes as C
@@ -22,6 +25,7 @@ from torch import nn
 from torch.autograd.function import once_differentiable
 
 from . import _lib
+from . import decoder as _decoder
 
 SRC_C, RGB_C, DEPTH_C, HEAD_C = 48, 3, 1, 32
 
@@ -228,24 +232,43 @@ def gs_head_train(up_src, img, depth, regresser):
     return _Tail.apply(up_src, img, depth, *params_of(regresser))
 
 
-def make_regresser_forward(orig, train=False):
-    """`GSRegresser.forward` with the full-resolution tail on the kernels when grad is disabled and the inputs are
-    supported; with `train`, also when grad is enabled and the image does not require grad (`gs_head_train`);
-    otherwise `orig`, the reference's own method."""
+def make_regresser_forward(orig, train=False, tail=True, decoder=False):
+    """`GSRegresser.forward` with parts of it on the kernels; otherwise `orig`, the reference's own method.
+
+    tail: the full-resolution tail runs on the kernels when grad is disabled and the inputs are supported; with `train`,
+    also when grad is enabled and the image does not require grad (`gs_head_train`).
+    decoder: `decoder1` runs on the kernels (gps_gaussian_b200.decoder) when grad and autocast are off, cudnn.allow_tf32
+    is on and `decoder.supported(...)` holds; the tail then runs on the kernels (with `tail`) or on the module's own
+    layers.  With grad enabled decoder1 always stays the module's."""
     def forward(self, img, depth, img_feat):
         grad = torch.is_grad_enabled()
-        if ((grad and not (train and torch.is_tensor(img) and not img.requires_grad)) or torch.is_autocast_enabled()
-                or not supported(self, img, depth, None)):
+        autocast = torch.is_autocast_enabled()
+        on_tail = (tail and not (grad and not (train and torch.is_tensor(img) and not img.requires_grad))
+                   and not autocast and supported(self, img, depth, None))
+        on_dec = (decoder and not grad and not autocast and torch.backends.cudnn.allow_tf32
+                  and _decoder.supported(self, None, img_feat[0], None))
+        if not (on_tail or on_dec):
             return orig(self, img, depth, img_feat)
         img_feat1, img_feat2, img_feat3 = img_feat
         depth_feat1, depth_feat2, depth_feat3 = self.depth_encoder(depth)
         x = self.decoder3(torch.cat([img_feat3, depth_feat3], dim=1))
         x = self.decoder2(torch.cat([self.up(x), img_feat2, depth_feat2], dim=1))
-        x = self.decoder1(torch.cat([self.up(x), img_feat1, depth_feat1], dim=1))
-        if not supported(self, img, depth, x):        # e.g. fp16 image features: the decoders ran in fp16
+        decoded = on_dec and _decoder.supported(self, x, img_feat1, depth_feat1)
+        if decoded:
+            x = _decoder.run(x, img_feat1, depth_feat1, _decoder.params_of(self))
+        else:
+            x = self.decoder1(torch.cat([self.up(x), img_feat1, depth_feat1], dim=1))
+        if on_tail and supported(self, img, depth, x):
+            if grad:
+                return _Tail.apply(x, img, depth, *params_of(self))
+            return run(x, img, depth, params_of(self))
+        if on_tail and not decoded:                   # e.g. fp16 image features: the decoders ran in fp16
             return orig(self, img, depth, img_feat)
-        if grad:
-            return _Tail.apply(x, img, depth, *params_of(self))
-        return run(x, img, depth, params_of(self))
+        # the reference's tail (lib/gs_parm_network.py) on the module's own layers
+        out = self.out_relu(self.out_conv(torch.cat([self.up(x), img, depth], dim=1)))
+        rot_out = torch.nn.functional.normalize(self.rot_head(out), dim=1)
+        scale_out = torch.clamp_max(self.scale_head(out), 0.01)
+        opacity_out = self.opacity_head(out)
+        return rot_out, scale_out, opacity_out
     forward.__doc__ = orig.__doc__
     return forward

@@ -77,6 +77,15 @@ the kernels do not cover, the reference's own forward runs unchanged.  x1 differ
 re-association, which is why the switch is opt-in.  It composes with GPSG_GS_HEAD / GPSG_GS_HEAD_TRAIN, whose rebound
 regressor calls its depth encoder as a module.  Unset or any other value leaves `core.extractor` alone.
 
+`GPSG_DECODER=1`, read once by `install()`, also hooks `lib.gs_parm_network` and rebinds GSRegresser.forward (the same
+method, through the same gs_head.make_regresser_forward) so that with autograd and autocast off and cudnn.allow_tf32
+on, `decoder1` (two ResidualBlocks at half resolution, with the upsample and the concat of its input) runs on the TF32
+kernels of csrc/decoder1.cu (gps_gaussian_b200.decoder).  It composes with GPSG_GS_HEAD / GPSG_GS_HEAD_TRAIN: with
+both, the decoder1 kernels feed the tail kernels directly; alone, the reference's tail runs on the module's own layers.
+With grad enabled decoder1 always stays the module's; in every other case the kernels do not cover, the reference's
+own forward runs.  The output differs from cuDNN's by TF32 re-association, which is why the switch is opt-in.  Unset or
+any other value leaves decoder1 to the module.
+
 `taichi_three` and its submodules always resolve to the stand-in in dropin/taichi_three (the dataset renderer on
 csrc/mesh_render.cu).  `python prepare_data/render_data.py` puts prepare_data/ first on sys.path, where the reference's
 own package, which cannot import without Taichi, would shadow anything on PYTHONPATH.
@@ -97,6 +106,7 @@ _ENCODE = False       # GPSG_ENCODE=1 at install()
 _GS_HEAD = False      # GPSG_GS_HEAD=1 at install()
 _GS_HEAD_TRAIN = False  # GPSG_GS_HEAD_TRAIN=1 at install()
 _ENCODER = False      # GPSG_ENCODER=1 at install()
+_DECODER = False      # GPSG_DECODER=1 at install()
 
 
 def _set(mod, attr, new):
@@ -209,7 +219,8 @@ def _patch_regresser(mod):
     key = (cls, "forward")
     if key not in _ORIG_METHODS:
         _ORIG_METHODS[key] = cls.__dict__["forward"]
-    cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key], train=_GS_HEAD_TRAIN)
+    cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key], train=_GS_HEAD_TRAIN,
+                                                 tail=_GS_HEAD or _GS_HEAD_TRAIN, decoder=_DECODER)
 
 
 def _patch_extractor(mod):
@@ -334,7 +345,7 @@ _ENCODER_TARGETS = {"core.extractor": _patch_extractor}
 
 def _targets():
     return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {}),
-            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD or _GS_HEAD_TRAIN else {}),
+            **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD or _GS_HEAD_TRAIN or _DECODER else {}),
             **(_ENCODER_TARGETS if _ENCODER else {})}
 
 
@@ -385,8 +396,9 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN and GPSG_ENCODER here, once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER
+    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN, GPSG_ENCODER and GPSG_DECODER here,
+    once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER, _DECODER
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
@@ -395,6 +407,7 @@ def install():
     _GS_HEAD = os.environ.get("GPSG_GS_HEAD", "") == "1"
     _GS_HEAD_TRAIN = os.environ.get("GPSG_GS_HEAD_TRAIN", "") == "1"
     _ENCODER = os.environ.get("GPSG_ENCODER", "") == "1"
+    _DECODER = os.environ.get("GPSG_DECODER", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -462,6 +475,11 @@ def gs_head_train():
     """Whether the installed patch also trains the regressor's full-resolution tail on the fused kernels, forward and
     backward (GPSG_GS_HEAD_TRAIN=1 at install())."""
     return _GS_HEAD_TRAIN
+
+
+def decoder():
+    """Whether the installed patch runs the regressor's decoder1 on the fused kernels (GPSG_DECODER=1 at install())."""
+    return _DECODER
 
 
 def encoder():

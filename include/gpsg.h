@@ -615,6 +615,42 @@ GPSG_API int gpsg_encoder_stem_forward(int device, void* stream, int B, int Cin,
                                        const float* input, GpsgEncoderStemWeights weights, float* x1_out,
                                        void* workspace);
 
+/* ---- decoder1 of the Gaussian-parameter regressor (reference lib/gs_parm_network.py, two ResidualBlocks), inference ----
+ * gpsg_decoder1_forward: out [B,48,H,W] (NCHW fp32, H = 2 Hs, W = 2 Ws), the output of `decoder1` on
+ * cat(up2x(s), img_feat, depth_feat), from s [B,64,Hs,Ws] (the decoder2 output), img_feat and depth_feat [B,32,H,W]
+ * (NCHW fp32, contiguous, Hs, Ws >= 1):
+ *   up2x: bilinear x2, align_corners=False, as torch's upsample_bilinear2d: source (d + 0.5) / 2 - 0.5 clamped at 0,
+ *     i0 = floor, i1 = min(i0 + 1, n - 1), evaluated in fp32 as l0y (l0x a + l1x b) + l1y (l0x c + l1x d);
+ *   v = cat(up2x(s), img_feat, depth_feat) [B,128,H,W] (never stored);
+ *   block 0: y1 = conv3x3(v, b0_conv1) ; yd = conv1x1(v, b0_down) ; y2 = conv3x3(relu(GN6(y1)), b0_conv2) ;
+ *            xb = relu(GN6(yd) + relu(GN6(y2)))       (no ReLU on the downsample branch before the add)
+ *   block 1: y3 = conv3x3(xb, b1_conv1) ; y4 = conv3x3(relu(GN6(y3)), b1_conv2) ; out = relu(xb + relu(GN6(y4)))
+ *   every convolution with its bias and zero padding 1 (3x3) or 0 (1x1).
+ *   GN6(y): GroupNorm(6, 48) per sample (8 channels per group), biased variance, eps 1e-5, the channel's weight and bias;
+ *   evaluated as fmaf(y, A, C) with A = w rstd and C = b - mean A rounded to fp32, the statistics in fp64 from the stored
+ *   fp32 y.  A non-finite value in a (sample, group) makes that group NaN; ReLU keeps NaN.
+ *   Precision (cuDNN with allow_tf32): every convolution operand, weights and activations (the interpolated, normalized
+ *   and residual-added values included), rounded to TF32 (round to nearest, ties away); products and sums fp32 in an
+ *   unspecified order; the fp32 bias added after the sum.
+ *   Weights in torch's layouts, fp32 and contiguous: b0_conv1_w [48,128,3,3], b0_down_w [48,128,1,1], the other 3x3
+ *   weights [48,48,3,3], biases and GroupNorm weights / biases [48].
+ *   Bit-reproducible: no floating-point atomics; every sum has a fixed order given the shape and the device's SM count.
+ *   workspace: gpsg_decoder1_workspace_bytes(B, Hs, Ws) bytes, 256-byte aligned.  After the call it starts with the five
+ *   raw convolution outputs y1, yd, y2, y3, y4 in that order (bias included, NHWC [B,H,W,48] fp32), the i-th at byte
+ *   i * S with S = B H W 48 * 4 rounded up to a multiple of 256; then the per-channel A, C, the per-tile GroupNorm
+ *   partials and the TF32-packed weights.  B >= 0 (B = 0 does nothing); Hs, Ws >= 1; NULL pointers are refused.
+ *   Enqueues on `stream` and does not synchronise. */
+typedef struct GpsgDecoder1Weights {
+    const float* b0_conv1_w; const float* b0_conv1_b; const float* b0_norm1_w; const float* b0_norm1_b;
+    const float* b0_conv2_w; const float* b0_conv2_b; const float* b0_norm2_w; const float* b0_norm2_b;
+    const float* b0_down_w; const float* b0_down_b; const float* b0_norm3_w; const float* b0_norm3_b;
+    const float* b1_conv1_w; const float* b1_conv1_b; const float* b1_norm1_w; const float* b1_norm1_b;
+    const float* b1_conv2_w; const float* b1_conv2_b; const float* b1_norm2_w; const float* b1_norm2_b;
+} GpsgDecoder1Weights;
+GPSG_API size_t gpsg_decoder1_workspace_bytes(int B, int Hs, int Ws);
+GPSG_API int gpsg_decoder1_forward(int device, void* stream, int B, int Hs, int Ws, const float* s, const float* img_feat,
+                                   const float* depth_feat, GpsgDecoder1Weights weights, float* out, void* workspace);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.

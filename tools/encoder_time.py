@@ -79,7 +79,7 @@ def _extractor(cin):
     return UnetExtractor(in_channel=cin, encoder_dim=[32, 48, 96]).cuda().eval()
 
 
-_KERNELS = (("stem_in", "stem_in"), ("stem_conv<", "stem_conv"), ("stem_gn_finalize", "stem_gn_finalize"),
+_KERNELS = (("stem_in", "stem_in"), ("stem_conv<", "stem_conv"), ("gn_finalize<", "stem_gn_finalize"),
             ("stem_out", "stem_out"))
 
 
