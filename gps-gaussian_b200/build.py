@@ -39,6 +39,7 @@ SOURCES = {
     "flow_head.cu": [],
     "gs_head.cu": [],
     "encoder_stem.cu": [],
+    "encoder_down.cu": [],
     "decoder1.cu": [],
     "mesh_render.cu": ["-fmad=false"],
     "jpeg_decode.cu": [],

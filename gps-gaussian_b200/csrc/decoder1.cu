@@ -10,7 +10,7 @@
 //
 // Only the raw convolution outputs y1, yd, y2, y3, y4 reach HBM (NHWC fp32); every normalized tensor is recomputed
 // from them where it is read: each convolution applies its input's GroupNorm, affine, ReLU and residual while it stages
-// its input tile, and dec_out does the last one.  Every convolution operand is rounded with cvt.rna.tf32.f32 (the
+// its input tile, and res_out does the last one.  Every convolution operand is rounded with cvt.rna.tf32.f32 (the
 // precision class of cuDNN with allow_tf32); products and sums fp32, the bias added in fp32 after the sum.
 //
 // Kernels (`ptxas -v`, sm_90a, no spills).  Bounds by shape counts at B = 2, 1024^2 input (H = W = 512, 524,288 output
@@ -28,7 +28,7 @@
 //                      so the next chunk (of this tile or the next) is staged while the current one's MMAs run.
 //                      64.4 GFLOP, 369 MB: TF32 bound 0.13 ms, HBM bound 0.11 ms -- bound by the tensor cores.
 //                      Persistent, one CTA per SM.  240 registers, 219 KiB dynamic smem (224,256 B).
-//   dec_conv<S>        one 3x3 convolution 48 -> 48, wgmma m64n48k8, K = 9 taps x 48.  A tile is 2 rows x 64 columns
+//   res_conv<TF32, 48, S>  (fused_conv.cuh, shared with encoder_down.cu) one 3x3 convolution 48 -> 48, wgmma m64n48k8, K = 9 taps x 48.  A tile is 2 rows x 64 columns
 //                      (warpgroup r owns row r); the 4 x 66 x 48 halo (49.5 KiB) is double-buffered beside the resident
 //                      81 KiB of weights, so the next tile is staged while the current one's MMAs run.  S = 1 stages
 //                      relu(GN(y)); S = 2 stages xb = relu(GN(yd) + relu(GN(y2))).  21.7 GFLOP each, 201 MB (S = 1) or
@@ -36,7 +36,7 @@
 //                      Persistent, one CTA per SM.  <1> 124 / <2> 168 registers, 180 KiB dynamic smem.
 //   gn_finalize<48>    per (sample, group): the tiles' partials merged in fp64 in a fixed order (fused_norm.cuh).
 //                      48 registers, 6 KiB static smem.
-//   dec_out            out = relu(xb + relu(GN6(y4))) from yd, y2, y4, written NCHW.  403 MB: HBM bound 0.12 ms.
+//   res_out<TF32, 48>  (fused_conv.cuh) out = relu(xb + relu(GN6(y4))) from yd, y2, y4, written NCHW.  403 MB: HBM bound 0.12 ms.
 //                      48 registers.
 // In all 129.5 GFLOP (0.26 ms at the TF32 rate) and 1.48 GB (0.44 ms at the HBM rate) at B = 2.
 // GroupNorm statistics: every producing kernel reduces its tile's values per group (8 channels: the accumulator's
@@ -46,6 +46,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "fused_conv.cuh"
 #include "fused_norm.cuh"
 #include "gpsg_internal.cuh"
 #include "sm90_ptx.cuh"
@@ -73,28 +74,13 @@ constexpr int kInW1 = kChG * kC * 4;                // [cg][48][4]
 constexpr int kInStage = kInA + kInW3 + kInW1;
 constexpr size_t kSmemIn = (size_t)2 * kInStage * sizeof(float);
 
-// dec_conv: tile 2 x 64, 48 channels; two halo buffers and the resident weights
-constexpr int kCvRows = 2, kCvHY = kCvRows + 2;
-constexpr int kCG = kC / 4;
-constexpr int kCvA = kCG * kCvHY * kHX * 4;         // [cg][4][66][4]
-constexpr int kCvW = 9 * kCG * kC * 4;              // [tap][cg][48][4]
-constexpr size_t kSmemCv = (size_t)(2 * kCvA + kCvW) * sizeof(float);
+// the 48 -> 48 convolutions: fused_conv.cuh's res_conv (tile 2 x 64, resident weights)
+using Cv = ResConv<false, kC>;
+constexpr int kCvRows = Cv::kRows, kCG = Cv::kCG, kCvW = Cv::kW;
+constexpr size_t kSmemCv = Cv::kSmem;
 constexpr int kPackIn = kNChunk * (kInW3 + kInW1);  // dec_in's weights, chunk by chunk as staged
-static_assert(kSmemIn + 1024 <= 227 * 1024 && kSmemCv <= 227 * 1024, "shared memory");
-static_assert((kInA * 4) % 128 == 0 && (kInStage * 4) % 128 == 0 && (kCvA * 4) % 128 == 0, "operand alignment");
-
-struct Tiles {
-    int tx, ty;
-    int64_t tps, n;
-    __host__ __device__ Tiles(int B, int H, int W, int rows)
-        : tx((W + kTW - 1) / kTW), ty((H + rows - 1) / rows), tps((int64_t)tx * ty), n((int64_t)B * tps) {}
-    __device__ void at(int64_t tile, int rows, int& b, int& y0, int& x0) const {
-        b = (int)(tile / tps);
-        const int rem = (int)(tile % tps);
-        y0 = (rem / tx) * rows;
-        x0 = (rem % tx) * kTW;
-    }
-};
+static_assert(kSmemIn + 1024 <= 227 * 1024, "shared memory");
+static_assert((kInA * 4) % 128 == 0 && (kInStage * 4) % 128 == 0, "operand alignment");
 
 // ---- weights -----------------------------------------------------------------------------------------------------
 __global__ void dec_pack(GpsgDecoder1Weights wt, float* __restrict__ pin, float* __restrict__ pcv) {
@@ -111,67 +97,6 @@ __global__ void dec_pack(GpsgDecoder1Weights wt, float* __restrict__ pin, float*
             const int j = q & 3, n = (q >> 2) % kC, cg = (q >> 2) / kC % kCG, tap = (q >> 2) / kC / kCG;
             pcv[k * kCvW + q] = tf32(w[(n * kC + cg * 4 + j) * 9 + tap]);
         }
-    }
-}
-
-// ---- epilogue --------------------------------------------------------------------------------------------------------
-// Bias, the raw NHWC store and the tile's GroupNorm(6) partials (count, mean, M2).  acc[rr] holds row y0 + RW wg + rr of
-// the 2 RW-row tile; in the m64n48 fragment thread (warp q of the warpgroup, lane l) holds d[4j + i] at column
-// 16 q + l / 4 + 8 ((i >> 1) & 1) and channel 8 j + 2 (l % 4) + (i & 1).
-template <int RW>
-__device__ __forceinline__ void emit(float (&acc)[RW][24], const float (&bv)[kNJ][2], float* __restrict__ y,
-                                     double* __restrict__ part, int64_t tile, int b, int y0, int x0, int H, int W,
-                                     int tid, double* red, double* res) {
-    const int lane = tid & 31, wg = tid >> 7, wq = (tid >> 5) & 3, g = lane >> 2, t = lane & 3;
-    const size_t hw = (size_t)H * W;
-    double sg[kG];
-#pragma unroll
-    for (int j = 0; j < kG; ++j) sg[j] = 0.0;
-#pragma unroll
-    for (int rr = 0; rr < RW; ++rr) {
-        const int yy = y0 + RW * wg + rr;
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-            const int xx = x0 + 16 * wq + 8 * hf + g;
-            const bool ok = yy < H && xx < W;
-            float* o = y + ((size_t)b * hw + (size_t)yy * W + xx) * kC + 2 * t;
-#pragma unroll
-            for (int j = 0; j < kNJ; ++j) {
-                const float v0 = acc[rr][4 * j + 2 * hf] + bv[j][0], v1 = acc[rr][4 * j + 2 * hf + 1] + bv[j][1];
-                acc[rr][4 * j + 2 * hf] = v0, acc[rr][4 * j + 2 * hf + 1] = v1;
-                if (ok) {
-                    *reinterpret_cast<float2*>(o + 8 * j) = make_float2(v0, v1);
-                    sg[j] += (double)v0 + (double)v1;
-                }
-            }
-        }
-    }
-    cta_sum<kG>(sg, red, res, tid);
-    const int rows = H - y0 < 2 * RW ? H - y0 : 2 * RW, cols = W - x0 < kTW ? W - x0 : kTW;
-    const double n = (double)rows * cols * 8.0;
-    double m2[kG];
-#pragma unroll
-    for (int j = 0; j < kG; ++j) {
-        sg[j] /= n;
-        m2[j] = 0.0;
-    }
-#pragma unroll
-    for (int rr = 0; rr < RW; ++rr)
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-            if (!(y0 + RW * wg + rr < H && x0 + 16 * wq + 8 * hf + g < W)) continue;
-#pragma unroll
-            for (int j = 0; j < kNJ; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const double d = (double)acc[rr][4 * j + 2 * hf + e] - sg[j];
-                    m2[j] += d * d;
-                }
-        }
-    cta_sum<kG>(m2, red, res, tid);
-    if (tid < kG) {
-        double* q = part + ((size_t)tile * kG + tid) * 3;
-        q[0] = n, q[1] = pick(sg, tid), q[2] = pick(m2, tid);
     }
 }
 
@@ -241,7 +166,7 @@ dec_in(int B, int Hs, int Ws, InArgs a) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) bv1[j][e] = a.b1[8 * j + 2 * t + e], bvd[j][e] = a.bd[8 * j + 2 * t + e];
 
-    const Tiles tl(B, H, W, kInRows);
+    const ConvTiles tl(B, H, W, kInRows);
     const int64_t mine = blockIdx.x < tl.n ? (tl.n - 1 - blockIdx.x) / gridDim.x + 1 : 0;
     const int64_t steps = mine * kNChunk;
     if (steps > 0) {
@@ -303,139 +228,12 @@ dec_in(int B, int Hs, int Ws, InArgs a) {
         if (chunk == kNChunk - 1) {
             int b, y0, x0;
             tl.at(tile, kInRows, b, y0, x0);
-            emit<2>(acc, bv1, a.y1, a.p1, tile, b, y0, x0, H, W, tid, red, res);
-            emit<2>(accd, bvd, a.yd, a.pd, tile, b, y0, x0, H, W, tid, red, res);
+            conv_emit<false, kC, 2>(acc, bv1, a.y1, a.p1, tile, b, y0, x0, H, W, tid, red, res);
+            conv_emit<false, kC, 2>(accd, bvd, a.yd, a.pd, tile, b, y0, x0, H, W, tid, red, res);
         }
         cp_async_wait_all();
         fence_async();
         __syncthreads();                                // the next buffer is complete; this one may be refilled
-    }
-}
-
-// ---- the 48 -> 48 convolutions -----------------------------------------------------------------------------------
-// the 4 x 66 halo at (b, y0 - 1, x0 - 1) of S = 1: relu(GN(yb)), S = 2: relu(GN(yx) + relu(GN(yb))), TF32, zero outside
-// the image, into sA [12][4][66][4]; one work item is 16 channels (four 16-byte loads per tensor) of one halo pixel
-template <int S>
-__device__ __forceinline__ void stage_cv(float* sA, const float* yb, const float2* pb, const float* yx, const float2* px,
-                                         int H, int W, int b, int y0, int x0, int tid) {
-    const size_t hw = (size_t)H * W;
-    for (int i = tid; i < 3 * kCvHY * kHX; i += kThreads) {
-        const int p = i % (kCvHY * kHX), cq = i / (kCvHY * kHX), hy = p / kHX, hx = p % kHX;
-        const int iy = y0 + hy - 1, ix = x0 + hx - 1;
-        const bool in = iy >= 0 && iy < H && ix >= 0 && ix < W;
-        const size_t off = ((size_t)b * hw + (size_t)(in ? iy : 0) * W + (in ? ix : 0)) * kC;
-        float4 qb[4], qx[S == 2 ? 4 : 1];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            qb[c] = in ? __ldg(reinterpret_cast<const float4*>(yb + off) + cq * 4 + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-            if constexpr (S == 2)
-                qx[c] = in ? __ldg(reinterpret_cast<const float4*>(yx + off) + cq * 4 + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const int ch = (cq * 4 + c) * 4;
-            float v[4] = {qb[c].x, qb[c].y, qb[c].z, qb[c].w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 A = __ldg(pb + b * kC + ch + e);
-                v[e] = relu(fmaf(v[e], A.x, A.y));
-            }
-            if constexpr (S == 2) {
-                const float r[4] = {qx[c].x, qx[c].y, qx[c].z, qx[c].w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float2 D = __ldg(px + b * kC + ch + e);
-                    v[e] = relu(fmaf(r[e], D.x, D.y) + v[e]);
-                }
-            }
-#pragma unroll
-            for (int e = 0; e < 4; ++e) v[e] = in ? tf32(v[e]) : 0.f;
-            reinterpret_cast<float4*>(sA)[((cq * 4 + c) * kCvHY + hy) * kHX + hx] = make_float4(v[0], v[1], v[2], v[3]);
-        }
-    }
-}
-
-template <int S>
-__global__ void __launch_bounds__(kThreads, 1)
-dec_conv(int B, int H, int W, const float* __restrict__ yb, const float2* __restrict__ pb, const float* __restrict__ yx,
-         const float2* __restrict__ px, const float* __restrict__ wpack, const float* __restrict__ bias,
-         float* __restrict__ y, double* __restrict__ part) {
-    extern __shared__ __align__(128) float smem[];
-    float* sA = smem;                                    // 2 x [12][4][66][4]
-    float* sW = smem + 2 * kCvA;                         // [tap][12][48][4]
-    __shared__ double red[8 * kG], res[kG];
-    const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7, t = lane & 3;
-    for (int i = tid; i < kCvW / 4; i += kThreads) cp_async16(sW + 4 * i, wpack + 4 * i);
-    float bv[kNJ][2];
-#pragma unroll
-    for (int j = 0; j < kNJ; ++j) bv[j][0] = bias[8 * j + 2 * t], bv[j][1] = bias[8 * j + 2 * t + 1];
-
-    const Tiles tl(B, H, W, kCvRows);
-    if (blockIdx.x < tl.n) {
-        int b, y0, x0;
-        tl.at(blockIdx.x, kCvRows, b, y0, x0);
-        stage_cv<S>(sA, yb, pb, yx, px, H, W, b, y0, x0, tid);
-    }
-    cp_async_wait_all();
-    fence_async();
-    __syncthreads();
-    const uint32_t aBase = smem_addr(sA), wBase = smem_addr(sW);
-    int buf = 0;
-    for (int64_t tile = blockIdx.x; tile < tl.n; tile += gridDim.x, buf ^= 1) {
-        float acc[1][24];
-#pragma unroll
-        for (int i = 0; i < 24; ++i) acc[0][i] = 0.f;
-        fence_acc(acc[0]);
-        const uint32_t aB = opaque(aBase + (uint32_t)(buf * kCvA * 4)), wB = opaque(wBase);
-        wgmma_fence();
-        const uint64_t aD = gmma_desc(aB, kCvHY * kHX * 16, 128), wD = gmma_desc(wB, kC * 16, 128);
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-            const int dy = tap / 3, dx = tap % 3;
-            const uint64_t at = aD + (uint64_t)((wg + dy) * kHX + dx), bt = wD + (uint64_t)(tap * kCG * kC);
-#pragma unroll
-            for (int s = 0; s < kCG / 2; ++s)
-                wgmma_m64n48k8(acc[0], at + (uint64_t)(2 * s * kCvHY * kHX), bt + (uint64_t)(2 * s * kC));
-        }
-        wgmma_commit();
-        if (tile + gridDim.x < tl.n) {                   // stage the next tile while the MMAs run
-            int b, y0, x0;
-            tl.at(tile + gridDim.x, kCvRows, b, y0, x0);
-            stage_cv<S>(sA + (buf ^ 1) * kCvA, yb, pb, yx, px, H, W, b, y0, x0, tid);
-        }
-        wgmma_wait();
-        fence_acc(acc[0]);
-        int b, y0, x0;
-        tl.at(tile, kCvRows, b, y0, x0);
-        emit<1>(acc, bv, y, part, tile, b, y0, x0, H, W, tid, red, res);
-        fence_async();
-        __syncthreads();                                 // the next buffer is complete; this one may be refilled
-    }
-}
-
-// ---- output ----------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads)
-dec_out(int B, int64_t hw, const float* __restrict__ yd, const float2* __restrict__ pd, const float* __restrict__ y2,
-        const float2* __restrict__ p2, const float* __restrict__ y4, const float2* __restrict__ p4, float* __restrict__ out) {
-    const int64_t total = (int64_t)B * hw;
-    for (int64_t q = (int64_t)blockIdx.x * kThreads + threadIdx.x; q < total; q += (int64_t)gridDim.x * kThreads) {
-        const int b = (int)(q / hw);
-        const int64_t p = q % hw;
-        const float4* d = reinterpret_cast<const float4*>(yd + q * kC);
-        const float4* r = reinterpret_cast<const float4*>(y2 + q * kC);
-        const float4* s = reinterpret_cast<const float4*>(y4 + q * kC);
-#pragma unroll
-        for (int c4 = 0; c4 < kC / 4; ++c4) {
-            const float4 a4 = __ldg(d + c4), r4 = __ldg(r + c4), s4 = __ldg(s + c4);
-            const float va[4] = {a4.x, a4.y, a4.z, a4.w}, vr[4] = {r4.x, r4.y, r4.z, r4.w}, vs[4] = {s4.x, s4.y, s4.z, s4.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int c = c4 * 4 + e;
-                const float2 D = __ldg(pd + b * kC + c), R = __ldg(p2 + b * kC + c), Q = __ldg(p4 + b * kC + c);
-                const float xb = relu(fmaf(va[e], D.x, D.y) + relu(fmaf(vr[e], R.x, R.y)));
-                out[((size_t)b * kC + c) * hw + p] = relu(xb + relu(fmaf(vs[e], Q.x, Q.y)));
-            }
-        }
     }
 }
 
@@ -455,7 +253,7 @@ struct Layout {
         const size_t hw = (size_t)H * W;
         raw = align256((size_t)B * hw * kC * sizeof(float));
         prm = align256((size_t)B * kC * sizeof(float2));
-        const int64_t n_in = Tiles(B, H, W, kInRows).n, n_cv = Tiles(B, H, W, kCvRows).n;
+        const int64_t n_in = ConvTiles(B, H, W, kInRows).n, n_cv = ConvTiles(B, H, W, kCvRows).n;
         part = align256((size_t)(n_in > n_cv ? n_in : n_cv) * kG * 3 * sizeof(double));
         pack = align256((size_t)(kPackIn + 3 * kCvW) * sizeof(float));
         total = 5 * raw + 5 * prm + 2 * part + pack;
@@ -495,9 +293,9 @@ int launch_decoder1(int device, int B, int Hs, int Ws, const float* s, const flo
         int occ = 0;
         GPSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dec_in, kThreads, kSmemIn));
         const InArgs a{s, img_feat, depth_feat, pin, wt.b0_conv1_b, wt.b0_down_b, y[0], y[1], part[0], part[1]};
-        dec_in<<<grid_of(Tiles(B, L.H, L.W, kInRows).n, sms, occ), kThreads, kSmemIn, stream>>>(B, Hs, Ws, a);
+        dec_in<<<grid_of(ConvTiles(B, L.H, L.W, kInRows).n, sms, occ), kThreads, kSmemIn, stream>>>(B, Hs, Ws, a);
         GPSG_LAUNCH_CHECK();
-        const int64_t tps = Tiles(1, L.H, L.W, kInRows).tps;
+        const int64_t tps = ConvTiles(1, L.H, L.W, kInRows).tps;
         gn_finalize<kC><<<B * kG, kGnThreads, 0, stream>>>(kG, tps, part[0], wt.b0_norm1_w, wt.b0_norm1_b, prm[0]);
         GPSG_LAUNCH_CHECK();
         gn_finalize<kC><<<B * kG, kGnThreads, 0, stream>>>(kG, tps, part[1], wt.b0_norm3_w, wt.b0_norm3_b, prm[1]);
@@ -505,22 +303,22 @@ int launch_decoder1(int device, int B, int Hs, int Ws, const float* s, const flo
     }
     // the three 48 -> 48 convolutions: y2 from relu(GN(y1)), y3 from xb = relu(GN(yd) + relu(GN(y2))), y4 from
     // relu(GN(y3))
-    GPSG_CUDA(cudaFuncSetAttribute(dec_conv<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCv));
-    GPSG_CUDA(cudaFuncSetAttribute(dec_conv<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCv));
+    GPSG_CUDA(cudaFuncSetAttribute(res_conv<false, kC, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCv));
+    GPSG_CUDA(cudaFuncSetAttribute(res_conv<false, kC, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCv));
     int occ1 = 0, occ2 = 0;
-    GPSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ1, dec_conv<1>, kThreads, kSmemCv));
-    GPSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, dec_conv<2>, kThreads, kSmemCv));
-    const Tiles tc(B, L.H, L.W, kCvRows);
+    GPSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ1, res_conv<false, kC, 1>, kThreads, kSmemCv));
+    GPSG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, res_conv<false, kC, 2>, kThreads, kSmemCv));
+    const ConvTiles tc(B, L.H, L.W, kCvRows);
     const float* nw[3] = {wt.b0_norm2_w, wt.b1_norm1_w, wt.b1_norm2_w};
     const float* nb[3] = {wt.b0_norm2_b, wt.b1_norm1_b, wt.b1_norm2_b};
     const float* cb[3] = {wt.b0_conv2_b, wt.b1_conv1_b, wt.b1_conv2_b};
     for (int k = 0; k < 3; ++k) {
         float* yo = y[2 + k];
         if (k == 1)
-            dec_conv<2><<<grid_of(tc.n, sms, occ2), kThreads, kSmemCv, stream>>>(
+            res_conv<false, kC, 2><<<grid_of(tc.n, sms, occ2), kThreads, kSmemCv, stream>>>(
                 B, L.H, L.W, y[2], prm[2], y[1], prm[1], pcv + k * kCvW, cb[k], yo, part[0]);
         else
-            dec_conv<1><<<grid_of(tc.n, sms, occ1), kThreads, kSmemCv, stream>>>(
+            res_conv<false, kC, 1><<<grid_of(tc.n, sms, occ1), kThreads, kSmemCv, stream>>>(
                 B, L.H, L.W, k == 0 ? y[0] : y[3], k == 0 ? prm[0] : prm[3], nullptr, nullptr, pcv + k * kCvW, cb[k],
                 yo, part[0]);
         GPSG_LAUNCH_CHECK();
@@ -528,7 +326,7 @@ int launch_decoder1(int device, int B, int Hs, int Ws, const float* s, const flo
         GPSG_LAUNCH_CHECK();
     }
     const int64_t total = (int64_t)B * L.H * L.W, blocks = (total + kThreads - 1) / kThreads, cap = (int64_t)sms * 8;
-    dec_out<<<(unsigned)(blocks < cap ? blocks : cap), kThreads, 0, stream>>>(B, (int64_t)L.H * L.W, y[1], prm[1], y[2],
+    res_out<false, kC><<<(unsigned)(blocks < cap ? blocks : cap), kThreads, 0, stream>>>(B, (int64_t)L.H * L.W, y[1], prm[1], y[2],
                                                                               prm[2], y[4], prm[4], out);
     GPSG_LAUNCH_CHECK();
     return GPSG_OK;

@@ -50,6 +50,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "conv_prec.cuh"
 #include "fused_norm.cuh"
 #include "gpsg_internal.cuh"
 #include "sm90_ptx.cuh"
@@ -65,57 +66,6 @@ constexpr int kInPx = 256;             // stem_in tile: 256 consecutive output p
 constexpr int kTW = 64, kHX = kTW + 2; // stem_conv tile: 4 rows x 64 columns, halo 6 x 66
 constexpr int kRows = 4, kHY = kRows + 2;
 constexpr int kGIn = 8, kGRes = 4;     // GroupNorm groups of in_ds and of the residual blocks
-
-// precision traits: T is the type of the stored convolution outputs and of the MMA operands
-template <bool kHalf>
-struct Prec;
-template <>
-struct Prec<false> {
-    using T = float;
-    static constexpr int kPer = 4;                           // elements per 16-byte chunk
-    __device__ static float op(float x) { return tf32(x); }  // operand rounding
-    __device__ static float bias(float x) { return x; }      // the bias is added in fp32
-    __device__ static float out(float x) { return x; }       // the output stays fp32
-    __device__ static float to_f(T v) { return v; }
-    __device__ static T from_f(float v) { return v; }
-};
-template <>
-struct Prec<true> {
-    using T = __half;
-    static constexpr int kPer = 8;
-    __device__ static float op(float x) { return __half2float(__float2half_rn(x)); }
-    __device__ static float bias(float x) { return __half2float(__float2half_rn(x)); }
-    __device__ static float out(float x) { return __half2float(__float2half_rn(x)); }
-    __device__ static float to_f(T v) { return __half2float(v); }
-    __device__ static T from_f(float v) { return __float2half_rn(v); }
-};
-
-// 16 bytes of T as floats
-template <bool H>
-__device__ __forceinline__ void unpack(const uint4& q, float (&v)[Prec<H>::kPer]) {
-    if constexpr (H) {
-        const __half2* h = reinterpret_cast<const __half2*>(&q);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 f = __half22float2(h[i]);
-            v[2 * i] = f.x, v[2 * i + 1] = f.y;
-        }
-    } else {
-        v[0] = __uint_as_float(q.x), v[1] = __uint_as_float(q.y), v[2] = __uint_as_float(q.z), v[3] = __uint_as_float(q.w);
-    }
-}
-template <bool H>
-__device__ __forceinline__ uint4 pack(const float (&v)[Prec<H>::kPer]) {
-    uint4 q;
-    if constexpr (H) {
-        __half2* h = reinterpret_cast<__half2*>(&q);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    } else {
-        q = make_uint4(__float_as_uint(v[0]), __float_as_uint(v[1]), __float_as_uint(v[2]), __float_as_uint(v[3]));
-    }
-    return q;
-}
 
 // ---- in_ds -----------------------------------------------------------------------------------------------------------
 template <int CIN, bool H>

@@ -997,6 +997,31 @@ int gpsg_encoder_stem_forward(int device, void* stream_, int B, int Cin, int H, 
                                (cudaStream_t)stream_);
 }
 
+static bool encoder_down_shape_ok(int B, int Cin, int C, int H, int W, int precision) {
+    return B >= 0 && H >= 1 && W >= 1 && H <= 65536 && W <= 65536 && ((Cin == 32 && C == 48) || (Cin == 48 && C == 96)) &&
+           (precision == GPSG_ENCODER_STEM_TF32 || precision == GPSG_ENCODER_STEM_FP16) &&
+           (int64_t)B * H * W * Cin < (int64_t(1) << 40);
+}
+
+size_t gpsg_encoder_down_workspace_bytes(int B, int Cin, int C, int H, int W, int precision) {
+    return (B > 0 && encoder_down_shape_ok(B, Cin, C, H, W, precision))
+               ? encoder_down_workspace_bytes(B, Cin, C, H, W, precision) : 0;
+}
+
+int gpsg_encoder_down_forward(int device, void* stream_, int B, int Cin, int C, int H, int W, int precision,
+                              const float* input, GpsgEncoderDownWeights weights, float* out, void* workspace) {
+    GPSG_REQUIRE(encoder_down_shape_ok(B, Cin, C, H, W, precision),
+                 "encoder_down: needs (Cin, C) = (32, 48) or (48, 96), H, W >= 1, B >= 0 and a known precision");
+    if (B == 0) return GPSG_OK;
+    GPSG_REQUIRE(input && out && workspace, "NULL pointer");
+    const float* const* w = &weights.b0_conv1_w;
+    for (int i = 0; i < 20; ++i) GPSG_REQUIRE(w[i], "encoder_down: NULL weight pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 256 == 0, "encoder_down: workspace must be 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_encoder_down(device, B, Cin, C, H, W, precision, input, weights, out, workspace,
+                               (cudaStream_t)stream_);
+}
+
 static bool decoder1_shape_ok(int B, int Hs, int Ws) {
     return B >= 0 && Hs >= 1 && Ws >= 1 && Hs <= 32768 && Ws <= 32768 &&
            (int64_t)B * (2 * (int64_t)Hs) * (2 * (int64_t)Ws) * 128 < (int64_t(1) << 40);

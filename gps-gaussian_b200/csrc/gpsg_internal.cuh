@@ -281,6 +281,10 @@ int launch_gs_head_bwd(int device, int B, int H, int W, const float* src, const 
 size_t encoder_stem_workspace_bytes(int B, int Cin, int H, int W, int precision);
 int launch_encoder_stem(int device, int B, int Cin, int H, int W, int precision, const float* x,
                         const GpsgEncoderStemWeights& wt, float* x1, void* workspace, cudaStream_t stream);
+// encoder_down.cu
+size_t encoder_down_workspace_bytes(int B, int Cin, int C, int H, int W, int precision);
+int launch_encoder_down(int device, int B, int Cin, int C, int H, int W, int precision, const float* x,
+                        const GpsgEncoderDownWeights& wt, float* out, void* workspace, cudaStream_t stream);
 // decoder1.cu
 size_t decoder1_workspace_bytes(int B, int Hs, int Ws);
 int launch_decoder1(int device, int B, int Hs, int Ws, const float* s, const float* img_feat, const float* depth_feat,

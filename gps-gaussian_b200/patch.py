@@ -77,6 +77,12 @@ the kernels do not cover, the reference's own forward runs unchanged.  x1 differ
 re-association, which is why the switch is opt-in.  It composes with GPSG_GS_HEAD / GPSG_GS_HEAD_TRAIN, whose rebound
 regressor calls its depth encoder as a module.  Unset or any other value leaves `core.extractor` alone.
 
+`GPSG_ENCODER_DEEP=1`, read once by `install()`, takes effect together with GPSG_ENCODER=1 (alone it does nothing): the
+method is rebound with `encoder.make_extractor_forward(orig, deep=True)`, so that where the stem runs on the kernels
+and res2 / res3 are the reference's stages with encoder_dims [32, 48, 96], x2 and x3 run on the kernels of
+csrc/encoder_down.cu too, in the stem's precision.  x2 and x3 differ from cuDNN's by TF32 or fp16 re-association,
+which is why this switch is opt-in as well.  It composes with GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN and GPSG_DECODER.
+
 `GPSG_DECODER=1`, read once by `install()`, also hooks `lib.gs_parm_network` and rebinds GSRegresser.forward (the same
 method, through the same gs_head.make_regresser_forward) so that with autograd and autocast off and cudnn.allow_tf32
 on, `decoder1` (two ResidualBlocks at half resolution, with the upsample and the concat of its input) runs on the TF32
@@ -107,6 +113,7 @@ _GS_HEAD = False      # GPSG_GS_HEAD=1 at install()
 _GS_HEAD_TRAIN = False  # GPSG_GS_HEAD_TRAIN=1 at install()
 _ENCODER = False      # GPSG_ENCODER=1 at install()
 _DECODER = False      # GPSG_DECODER=1 at install()
+_ENCODER_DEEP = False  # GPSG_ENCODER=1 and GPSG_ENCODER_DEEP=1 at install()
 
 
 def _set(mod, attr, new):
@@ -229,7 +236,7 @@ def _patch_extractor(mod):
     key = (cls, "forward")
     if key not in _ORIG_METHODS:
         _ORIG_METHODS[key] = cls.__dict__["forward"]
-    cls.forward = encoder.make_extractor_forward(_ORIG_METHODS[key])
+    cls.forward = encoder.make_extractor_forward(_ORIG_METHODS[key], deep=_ENCODER_DEEP)
 
 
 _JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
@@ -396,9 +403,9 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN, GPSG_ENCODER and GPSG_DECODER here,
-    once."""
-    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER, _DECODER
+    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN, GPSG_ENCODER, GPSG_ENCODER_DEEP and
+    GPSG_DECODER here, once."""
+    global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER, _DECODER, _ENCODER_DEEP
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
@@ -408,6 +415,7 @@ def install():
     _GS_HEAD_TRAIN = os.environ.get("GPSG_GS_HEAD_TRAIN", "") == "1"
     _ENCODER = os.environ.get("GPSG_ENCODER", "") == "1"
     _DECODER = os.environ.get("GPSG_DECODER", "") == "1"
+    _ENCODER_DEEP = _ENCODER and os.environ.get("GPSG_ENCODER_DEEP", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -486,3 +494,9 @@ def encoder():
     """Whether the installed patch runs the UnetExtractor's half-resolution stem on the fused kernels (GPSG_ENCODER=1 at
     install())."""
     return _ENCODER
+
+
+def encoder_deep():
+    """Whether the installed patch also runs the UnetExtractor's res2 and res3 on the fused kernels (GPSG_ENCODER=1 and
+    GPSG_ENCODER_DEEP=1 at install())."""
+    return _ENCODER_DEEP

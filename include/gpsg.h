@@ -651,6 +651,39 @@ GPSG_API size_t gpsg_decoder1_workspace_bytes(int B, int Hs, int Ws);
 GPSG_API int gpsg_decoder1_forward(int device, void* stream, int B, int Hs, int Ws, const float* s, const float* img_feat,
                                    const float* depth_feat, GpsgDecoder1Weights weights, float* out, void* workspace);
 
+/* ---- stride-2 residual stages of the UnetExtractor (reference core/extractor.py: res2, res3), inference -------------
+ * gpsg_encoder_down_forward: out [B,C,Ho,Wo] (NCHW fp32, Ho = ceil(H/2), Wo = ceil(W/2)), the output of one stage of
+ * two ResidualBlocks (the first with stride 2 and a 1x1 downsample) on input [B,Cin,H,W] (NCHW fp32, H, W >= 1);
+ * (Cin, C) is (32, 48) (res2 of encoder_dims [32, 48, 96]) or (48, 96) (res3), any other pair is refused:
+ *   block 0: ya = conv3x3(input, b0_conv1; stride 2, padding 1) ; yd = conv1x1(input, b0_down; stride 2, padding 0) ;
+ *            yb = conv3x3(relu(GN(ya)), b0_conv2) ; xb = relu(GN(yd) + relu(GN(yb)))   (no ReLU on the downsample)
+ *   block 1: yc = conv3x3(xb, b1_conv1) ; ye = conv3x3(relu(GN(yc)), b1_conv2) ; out = relu(xb + relu(GN(ye)))
+ *   every convolution with its bias; the 3x3 ones of block 1 and conv2 with stride 1, padding 1.
+ *   GN(y): GroupNorm(C/8, C) per sample with its own weight and bias (norm1, norm2, norm3 in order of use), biased
+ *   variance, eps 1e-5, evaluated as fmaf(y, A, C) with A = w rstd and C = b - mean A rounded to fp32, the statistics in
+ *   fp64.  A non-finite value in a (sample, group) makes that group NaN; ReLU keeps NaN.
+ *   precision GPSG_ENCODER_STEM_TF32 / _FP16 with gpsg_encoder_stem_forward's semantics: TF32 operands (the input, each
+ *   normalized input, the weights) and fp32 outputs, or fp16 operands and biases with each convolution's output, bias
+ *   included, rounded to fp16; GroupNorm, ReLU and the residual adds in fp32 in both.
+ *   Weights in torch's layouts, fp32 and contiguous: b0_conv1_w [C,Cin,3,3], b0_down_w [C,Cin,1,1], the other 3x3 weights
+ *   [C,C,3,3], biases and GroupNorm weights / biases [C]; the field order is GpsgDecoder1Weights'.
+ *   Bit-reproducible: no floating-point atomics; every sum has a fixed order given the shape and the device's SM count.
+ *   workspace: gpsg_encoder_down_workspace_bytes(B, Cin, C, H, W, precision) bytes, 256-byte aligned.  After the call it
+ *   starts with the five raw convolution outputs ya, yd, yb, yc, ye in that order (bias included, NHWC [B,Ho,Wo,C], fp32
+ *   in TF32 mode, fp16 in FP16 mode), the i-th at byte i * S with S = B Ho Wo C sizeof(element) rounded up to a multiple
+ *   of 256; then the per-channel A, C, the per-tile GroupNorm partials and the packed weights.  B >= 0 (B = 0 does
+ *   nothing); NULL pointers are refused.  Enqueues on `stream` and does not synchronise. */
+typedef struct GpsgEncoderDownWeights {
+    const float* b0_conv1_w; const float* b0_conv1_b; const float* b0_norm1_w; const float* b0_norm1_b;
+    const float* b0_conv2_w; const float* b0_conv2_b; const float* b0_norm2_w; const float* b0_norm2_b;
+    const float* b0_down_w; const float* b0_down_b; const float* b0_norm3_w; const float* b0_norm3_b;
+    const float* b1_conv1_w; const float* b1_conv1_b; const float* b1_norm1_w; const float* b1_norm1_b;
+    const float* b1_conv2_w; const float* b1_conv2_b; const float* b1_norm2_w; const float* b1_norm2_b;
+} GpsgEncoderDownWeights;
+GPSG_API size_t gpsg_encoder_down_workspace_bytes(int B, int Cin, int C, int H, int W, int precision);
+GPSG_API int gpsg_encoder_down_forward(int device, void* stream, int B, int Cin, int C, int H, int W, int precision,
+                                       const float* input, GpsgEncoderDownWeights weights, float* out, void* workspace);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.

@@ -37,9 +37,9 @@ def work(B, Hs=256, Ws=256):
     f3 = 2 * px * 48 * 48 * 9
     return {
         "dec_in": dict(flop=2 * px * 48 * 128 * 10, bytes=B * 64 * Hs * Ws * 4 + px * 64 * 4 + 2 * raw),
-        "dec_conv<1>": dict(flop=f3, bytes=2 * raw),       # y2 and y4 (two launches)
-        "dec_conv<2>": dict(flop=f3, bytes=3 * raw),       # y3 from yd and y2
-        "dec_out": dict(flop=0, bytes=4 * raw),
+        "res_conv<false, 48, 1>": dict(flop=f3, bytes=2 * raw),       # y2 and y4 (two launches)
+        "res_conv<false, 48, 2>": dict(flop=f3, bytes=3 * raw),       # y3 from yd and y2
+        "res_out<false, 48>": dict(flop=0, bytes=4 * raw),
     }
 
 
@@ -79,8 +79,8 @@ def _regresser():
     return GSRegresser(cfg).cuda().eval()
 
 
-_KERNELS = ("dec_pack", "dec_in", "dec_conv<1>", "dec_conv<2>", "gn_finalize<", "dec_out")
-_PER_CALL = {"dec_conv<1>": 2, "gn_finalize<": 5}
+_KERNELS = ("dec_pack", "dec_in", "res_conv<false, 48, 1>", "res_conv<false, 48, 2>", "gn_finalize<", "res_out<false, 48>")
+_PER_CALL = {"res_conv<false, 48, 1>": 2, "gn_finalize<": 5}
 
 
 def _per_kernel(prof, w, calls):
@@ -133,9 +133,9 @@ def _decoder1(seconds, rounds):
             torch.cuda.synchronize()
         w = work(B)
         row["kernels"] = _per_kernel(prof, w, 10)
-        row["bytes_total"] = w["dec_in"]["bytes"] + 2 * w["dec_conv<1>"]["bytes"] + w["dec_conv<2>"]["bytes"] \
-            + w["dec_out"]["bytes"]
-        row["flop_total"] = w["dec_in"]["flop"] + 3 * w["dec_conv<1>"]["flop"]
+        row["bytes_total"] = w["dec_in"]["bytes"] + 2 * w["res_conv<false, 48, 1>"]["bytes"] + w["res_conv<false, 48, 2>"]["bytes"] \
+            + w["res_out<false, 48>"]["bytes"]
+        row["flop_total"] = w["dec_in"]["flop"] + 3 * w["res_conv<false, 48, 1>"]["flop"]
         res[f"B{B}"] = row
         del s, fi, fd
         torch.cuda.empty_cache()
