@@ -13,6 +13,8 @@ comes from autograd rather than from a hand-written backward:
 are well defined: their window lies wholly outside the row and the output is 0.  Callers pass the fp32 coordinate the
 kernels see; `.double()` of it is exact, and so is the division by 2^l, so `dx` is the kernels' `dx`.
 
+Tensors are created on the device of the inputs: CPU by default, the GPU where a check is too large for the CPU.
+
 `amp=True` rounds to fp16 at the reference's op boundaries under autocast (einsum result, the division, each pooled
 level): the pyramid the reference holds when it is handed fp16 feature maps.  The rounding is straight-through (the
 gradient is the fp64 derivative of the unrounded op), so gradients are the same with and without it.
@@ -66,10 +68,10 @@ def sample(vol, x, r):
     fl = torch.floor(x)
     dx = (x - fl).unsqueeze(-1)                                           # exact: x and floor(x) share a binade
     xf = torch.nan_to_num(fl, nan=0.0).clamp(-2.0 ** 62, 2.0 ** 62).to(torch.int64)
-    k = xf.unsqueeze(-1) - r + torch.arange(2 * r + 2, dtype=torch.int64)  # taps xf-r .. xf+r+1, [B,H,W1,2r+2]
+    k = xf.unsqueeze(-1) - r + torch.arange(2 * r + 2, dtype=torch.int64, device=vol.device)  # taps xf-r .. xf+r+1, [B,H,W1,2r+2]
     inside = (k >= 0) & (k < W2)
     if W2 == 0:
-        taps = torch.zeros(k.shape, dtype=F64) + 0.0 * vol.sum()
+        taps = torch.zeros(k.shape, dtype=F64, device=vol.device) + 0.0 * vol.sum()
     else:
         taps = torch.where(inside, torch.gather(vol, 3, k.clamp(0, W2 - 1)), torch.zeros((), dtype=F64))
     out = taps[..., :-1] * (1.0 - dx) + taps[..., 1:] * dx
@@ -87,7 +89,7 @@ def lookup(levels, coords_x, r):
 
 def level_grads(shapes, coords_x, r, grad_out):
     """d<lookup(levels, coords_x, r), grad_out>/d level, by autograd: one fp64 tensor per shape in `shapes`."""
-    lv = [torch.zeros(s, dtype=F64, requires_grad=True) for s in shapes]
+    lv = [torch.zeros(s, dtype=F64, device=grad_out.device, requires_grad=True) for s in shapes]
     out = lookup(lv, coords_x, r)
     return list(torch.autograd.grad(out, lv, grad_out.to(F64), allow_unused=True))
 
@@ -100,7 +102,7 @@ def fold(grads, W2):
         if gl is None:
             continue
         if g is None:
-            g = torch.zeros(tuple(gl.shape[:3]) + (W2,), dtype=F64)
+            g = torch.zeros(tuple(gl.shape[:3]) + (W2,), dtype=F64, device=gl.device)
         n = gl.shape[-1]
         g[..., :n << l] += (gl.to(F64) / 2 ** l).repeat_interleave(1 << l, dim=-1)
     return g
