@@ -252,6 +252,24 @@ lib.gpsg_encoder_down_workspace_bytes.restype = _sz
 lib.gpsg_encoder_down_workspace_bytes.argtypes = [_i, _i, _i, _i, _i, _i]
 lib.gpsg_encoder_down_forward.restype = _i
 lib.gpsg_encoder_down_forward.argtypes = [_i, _vp, _i, _i, _i, _i, _i, _i, _vp, EncoderDownWeights, _vp, _vp]
+UPDATE_PARAMS = ("convc1_w", "convc1_b", "convc2_w", "convc2_b", "convf1_w", "convf1_b", "convf2_w", "convf2_b",
+                 "conv_w", "conv_b", "convz_w", "convz_b", "convr_w", "convr_b", "convq_w", "convq_b",
+                 "fh_conv1_w", "fh_conv1_b", "fh_conv2_w", "fh_conv2_b", "mask0_w", "mask0_b", "mask2_w", "mask2_b")
+
+
+class UpdateWeights(C.Structure):
+    """GpsgUpdateWeights (include/gpsg.h), passed by value: the 24 device pointers of the update block's parameters."""
+    _fields_ = [(n, C.c_void_p) for n in UPDATE_PARAMS]
+
+
+lib.gpsg_update_workspace_bytes.restype = _sz
+lib.gpsg_update_workspace_bytes.argtypes = [_i, _i, _i]
+lib.gpsg_update_packed_bytes.restype = _sz
+lib.gpsg_update_packed_bytes.argtypes = []
+lib.gpsg_update_pack.restype = _i
+lib.gpsg_update_pack.argtypes = [_i, _vp, UpdateWeights, _vp]
+lib.gpsg_update_step.restype = _i
+lib.gpsg_update_step.argtypes = [_i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp]
 lib.gpsg_profile_enable.restype = _i
 lib.gpsg_profile_enable.argtypes = [_i]
 lib.gpsg_profile_read.restype = _i
@@ -277,7 +295,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode", "gpsg_gs_head_workspace_bytes",
             "gpsg_gs_head_forward", "gpsg_gs_head_backward_workspace_bytes", "gpsg_gs_head_backward",
             "gpsg_encoder_stem_workspace_bytes", "gpsg_encoder_stem_forward", "gpsg_decoder1_workspace_bytes",
-            "gpsg_decoder1_forward", "gpsg_encoder_down_workspace_bytes", "gpsg_encoder_down_forward"]
+            "gpsg_decoder1_forward", "gpsg_encoder_down_workspace_bytes", "gpsg_encoder_down_forward",
+            "gpsg_update_workspace_bytes", "gpsg_update_packed_bytes", "gpsg_update_pack", "gpsg_update_step"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)
 FWD_ANTIALIAS = 1         # GPSG_FWD_ANTIALIAS (include/gpsg.h)

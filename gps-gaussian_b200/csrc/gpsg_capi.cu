@@ -1043,6 +1043,38 @@ int gpsg_decoder1_forward(int device, void* stream_, int B, int Hs, int Ws, cons
     return launch_decoder1(device, B, Hs, Ws, s, img_feat, depth_feat, weights, out, workspace, (cudaStream_t)stream_);
 }
 
+static bool update_shape_ok(int B, int H, int W) {
+    return B >= 1 && H >= 1 && W >= 1 && H <= 65536 && W <= 65536 && (int64_t)B * H * W * 576 < (int64_t(1) << 40);
+}
+
+size_t gpsg_update_workspace_bytes(int B, int H, int W) {
+    return update_shape_ok(B, H, W) ? update_workspace_bytes(B, H, W) : 0;
+}
+
+size_t gpsg_update_packed_bytes(void) { return update_packed_bytes(); }
+
+int gpsg_update_pack(int device, void* stream_, GpsgUpdateWeights weights, void* packed) {
+    const float* const* w = &weights.convc1_w;
+    for (int i = 0; i < 24; ++i) GPSG_REQUIRE(w[i], "update: NULL weight pointer");
+    GPSG_REQUIRE(packed && (uintptr_t)packed % 256 == 0, "update: packed must be non-NULL and 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_update_pack(device, weights, packed, (cudaStream_t)stream_);
+}
+
+int gpsg_update_step(int device, void* stream_, int B, int H, int W, int corr_dtype, const void* corr, float* coords1,
+                     const void* net, const void* czrq, int64_t czrq_batch_stride, void* mask_out, const void* packed,
+                     void* workspace) {
+    GPSG_REQUIRE(update_shape_ok(B, H, W), "update: needs B, H, W >= 1");
+    GPSG_REQUIRE(corr_dtype == 0 || corr_dtype == 1, "update: corr_dtype must be 0 (fp32) or 1 (fp16)");
+    GPSG_REQUIRE(corr && coords1 && czrq && packed && workspace, "update: NULL pointer");
+    GPSG_REQUIRE(czrq_batch_stride >= (int64_t)288 * H * W || B == 1, "update: czrq_batch_stride below 288 H W");
+    GPSG_REQUIRE((uintptr_t)packed % 256 == 0 && (uintptr_t)workspace % 256 == 0,
+                 "update: packed and workspace must be 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_update_step(device, B, H, W, corr_dtype, corr, coords1, net, czrq, czrq_batch_stride, mask_out,
+                              packed, workspace, (cudaStream_t)stream_);
+}
+
 int gpsg_set_corr_build(int mode) {
     set_corr_build_mode(mode);
     return GPSG_OK;

@@ -285,6 +285,13 @@ int launch_encoder_stem(int device, int B, int Cin, int H, int W, int precision,
 size_t encoder_down_workspace_bytes(int B, int Cin, int C, int H, int W, int precision);
 int launch_encoder_down(int device, int B, int Cin, int C, int H, int W, int precision, const float* x,
                         const GpsgEncoderDownWeights& wt, float* out, void* workspace, cudaStream_t stream);
+// update_block.cu
+size_t update_workspace_bytes(int B, int H, int W);
+size_t update_packed_bytes();
+int launch_update_pack(int device, const GpsgUpdateWeights& wt, void* packed, cudaStream_t stream);
+int launch_update_step(int device, int B, int H, int W, int corr_dtype, const void* corr, float* coords1,
+                       const void* net, const void* czrq, int64_t czrq_bs, void* mask_out, const void* packed,
+                       void* workspace, cudaStream_t stream);
 // decoder1.cu
 size_t decoder1_workspace_bytes(int B, int Hs, int Ws);
 int launch_decoder1(int device, int B, int Hs, int Ws, const float* s, const float* img_feat, const float* depth_feat,

@@ -92,6 +92,19 @@ With grad enabled decoder1 always stays the module's; in every other case the ke
 own forward runs.  The output differs from cuDNN's by TF32 re-association, which is why the switch is opt-in.  Unset or
 any other value leaves decoder1 to the module.
 
+`GPSG_UPDATE=1`, read once by `install()`, also hooks `core.raft_stereo_human` and rebinds
+
+    FlowUpdateModule.forward -> update.make_update_forward (a class method, kept in _ORIG_METHODS)
+
+so that with autograd off and `args.mixed_precision` set (the stage-2 eval forward: test_view_interp.py,
+test_real_data.py, train_stage2.py's run_eval) every RAFT iteration's update block (motion encoder, ConvGRU, flow and
+mask heads) runs on the fp16 wgmma kernels of csrc/update_block.cu (gps_gaussian_b200.update).  The corr block is still
+built through the module's own corr class and the flow upsampled by `self.upsample_flow`, so the switch composes with
+the rebound CorrBlockFast1D and with GPSG_FLOW_HEAD.  With grad enabled, stage 1's fp32 eval, another GRU / hidden /
+corr / downsample configuration or inputs the kernels do not cover, the reference's own forward runs unchanged.  The
+flow differs from cuDNN's by fp16 re-association compounded over the iterations through the lookup, which is why the
+switch is opt-in.  Unset or any other value leaves FlowUpdateModule.forward alone.
+
 `taichi_three` and its submodules always resolve to the stand-in in dropin/taichi_three (the dataset renderer on
 csrc/mesh_render.cu).  `python prepare_data/render_data.py` puts prepare_data/ first on sys.path, where the reference's
 own package, which cannot import without Taichi, would shadow anything on PYTHONPATH.
@@ -114,6 +127,7 @@ _GS_HEAD_TRAIN = False  # GPSG_GS_HEAD_TRAIN=1 at install()
 _ENCODER = False      # GPSG_ENCODER=1 at install()
 _DECODER = False      # GPSG_DECODER=1 at install()
 _ENCODER_DEEP = False  # GPSG_ENCODER=1 and GPSG_ENCODER_DEEP=1 at install()
+_UPDATE = False       # GPSG_UPDATE=1 at install()
 
 
 def _set(mod, attr, new):
@@ -239,6 +253,23 @@ def _patch_extractor(mod):
     cls.forward = encoder.make_extractor_forward(_ORIG_METHODS[key], deep=_ENCODER_DEEP)
 
 
+def _patch_update(mod):
+    from gps_gaussian_b200 import update
+    cls = mod.FlowUpdateModule
+    key = (cls, "forward")
+    if key not in _ORIG_METHODS:
+        _ORIG_METHODS[key] = cls.__dict__["forward"]
+    cls.forward = update.make_update_forward(_ORIG_METHODS[key])
+
+
+def _patch_raft(mod):
+    """core.raft_stereo_human under GPSG_FLOW_HEAD and / or GPSG_UPDATE."""
+    if _FLOW_HEAD:
+        _patch_upsample(mod)
+    if _UPDATE:
+        _patch_update(mod)
+
+
 _JPEG_EXTS = (".jpg", ".jpeg", ".jpe")
 _JPEG_SAMPLING = {0x111111: "444", 0x211111: "422", 0x221111: "420"}   # cv2.IMWRITE_JPEG_SAMPLING_FACTOR_444/422/420
 _IMWRITE_JPEG_QUALITY, _IMWRITE_JPEG_SAMPLING_FACTOR = 1, 7
@@ -344,7 +375,7 @@ def original(mod, attr):
 
 _TARGETS = {"core.corr": _patch_corr, "lib.GaussianRender": _patch_render}
 _RECTIFY_TARGETS = {"lib.human_loader": _patch_loader}
-_FLOW_HEAD_TARGETS = {"core.raft_stereo_human": _patch_upsample, "lib.loss": _patch_loss}
+_FLOW_HEAD_TARGETS = {"lib.loss": _patch_loss}
 _ENCODE_TARGETS = {"cv2": _patch_cv2}
 _GS_HEAD_TARGETS = {"lib.gs_parm_network": _patch_regresser}
 _ENCODER_TARGETS = {"core.extractor": _patch_extractor}
@@ -353,7 +384,8 @@ _ENCODER_TARGETS = {"core.extractor": _patch_extractor}
 def _targets():
     return {**_TARGETS, **(_RECTIFY_TARGETS if _RECTIFY else {}), **(_FLOW_HEAD_TARGETS if _FLOW_HEAD else {}),
             **(_ENCODE_TARGETS if _ENCODE else {}), **(_GS_HEAD_TARGETS if _GS_HEAD or _GS_HEAD_TRAIN or _DECODER else {}),
-            **(_ENCODER_TARGETS if _ENCODER else {})}
+            **(_ENCODER_TARGETS if _ENCODER else {}),
+            **({"core.raft_stereo_human": _patch_raft} if _FLOW_HEAD or _UPDATE else {})}
 
 
 class _PatchingLoader(importlib.abc.Loader):
@@ -403,9 +435,10 @@ _FINDER = _Finder()
 
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
-    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN, GPSG_ENCODER, GPSG_ENCODER_DEEP and
-    GPSG_DECODER here, once."""
+    GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN, GPSG_ENCODER, GPSG_ENCODER_DEEP,
+    GPSG_DECODER and GPSG_UPDATE here, once."""
     global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER, _DECODER, _ENCODER_DEEP
+    global _UPDATE
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
@@ -416,6 +449,7 @@ def install():
     _ENCODER = os.environ.get("GPSG_ENCODER", "") == "1"
     _DECODER = os.environ.get("GPSG_DECODER", "") == "1"
     _ENCODER_DEEP = _ENCODER and os.environ.get("GPSG_ENCODER_DEEP", "") == "1"
+    _UPDATE = os.environ.get("GPSG_UPDATE", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
     for name, hook in _targets().items():
@@ -500,3 +534,8 @@ def encoder_deep():
     """Whether the installed patch also runs the UnetExtractor's res2 and res3 on the fused kernels (GPSG_ENCODER=1 and
     GPSG_ENCODER_DEEP=1 at install())."""
     return _ENCODER_DEEP
+
+
+def update():
+    """Whether the installed patch runs the RAFT update block on the fp16 kernels (GPSG_UPDATE=1 at install())."""
+    return _UPDATE

@@ -684,6 +684,48 @@ GPSG_API size_t gpsg_encoder_down_workspace_bytes(int B, int Cin, int C, int H, 
 GPSG_API int gpsg_encoder_down_forward(int device, void* stream, int B, int Cin, int C, int H, int W, int precision,
                                        const float* input, GpsgEncoderDownWeights weights, float* out, void* workspace);
 
+/* ---- disparity update block (reference core/update.py: BasicMultiUpdateBlock, n_gru_layers = 1), inference --------
+ * One RAFT iteration of FlowUpdateModule.forward under CUDA autocast in fp16, at 1/8 resolution [H,W], hidden dims 96,
+ * corr_levels 4, corr_radius 4, n_downsample 3.  With flow = fp16(coords1 - coords0) (coords0 the pixel grid, x then y):
+ *   cor = relu(convc2(relu(convc1(corr))))  flo = relu(convf2(relu(convf1(flow))))   (1x1 36->64, 3x3, 7x7 2->64, 3x3)
+ *   x = [relu(conv([cor, flo])), flow]  (3x3 128->126, then the two fp16 flow channels)
+ *   z = sigmoid(convz([h, x]) + cz)   r = sigmoid(convr([h, x]) + cr)   q = tanh(convq([r*h, x]) + cq)
+ *   h = (1 - z) h + z q
+ *   delta = flow_head.conv2(relu(flow_head.conv1(h)))   coords1[:, 0] += delta[:, 0] (fp32; channel 1 is zeroed)
+ *   mask = .25 * mask[2](relu(mask[0](h)))               (only when mask_out is not NULL)
+ *   Every convolution takes fp16 operands and an fp16 bias and accumulates in fp32; its output is rounded to fp16, then
+ *   the bias added and rounded again (cuDNN's convolution followed by the bias add).  Each elementwise op above rounds
+ *   to fp16 as autocast's fp16 tensors do: the + cz / cr / cq adds, sigmoid, tanh, r*h, 1-z, (1-z) h, z q, their sum and
+ *   the .25 scale.  ReLU keeps NaN.
+ * gpsg_update_pack: the 24 fp32 weights (contiguous, torch's layouts) rounded to fp16 (to nearest even) into `packed`,
+ *   gpsg_update_packed_bytes() bytes, 256-byte aligned.  Enqueues on `stream`.
+ * gpsg_update_step: one iteration.  corr [B,36,H,W] NCHW contiguous, fp16 (corr_dtype 1) or fp32 (corr_dtype 0, rounded
+ *   to fp16 at the convolution input); coords1 [B,2,H,W] fp32 contiguous, updated in place; czrq points at cz of the
+ *   [B,288,H,W] fp16 context tensor (cz, cr, cq its channels 0-95, 96-191, 192-287, each plane H*W contiguous, sample i
+ *   at czrq + i * czrq_batch_stride elements); mask_out NULL or [B,576,H,W] fp16 NCHW.  The hidden state h lives in the
+ *   workspace as NHWC [B,H,W,96] fp16 and is updated in place; `net` non-NULL ([B,96,H,W] fp16 NCHW contiguous) loads it
+ *   first (the first iteration), NULL continues from the workspace's h.  workspace: gpsg_update_workspace_bytes(B, H, W)
+ *   bytes, 256-byte aligned; after the call it holds, each at a 256-byte-aligned offset in this order, NHWC fp16:
+ *   h [96], x [128], cf1 = [relu(convc1), relu(convf1)] [128], cf2 = [cor, flo] [128], z [96], r*h [96],
+ *   [relu(flow_head.conv1), relu(mask[0])] [512] (the mask half only when mask_out is set) and delta [2] (channel 1 not
+ *   zeroed).  B >= 1, H, W >= 1.  Bit-reproducible; no floating-point atomics.  Enqueues on `stream` and does not
+ *   synchronise. */
+typedef struct GpsgUpdateWeights {
+    const float* convc1_w; const float* convc1_b; const float* convc2_w; const float* convc2_b;
+    const float* convf1_w; const float* convf1_b; const float* convf2_w; const float* convf2_b;
+    const float* conv_w; const float* conv_b;
+    const float* convz_w; const float* convz_b; const float* convr_w; const float* convr_b;
+    const float* convq_w; const float* convq_b;
+    const float* fh_conv1_w; const float* fh_conv1_b; const float* fh_conv2_w; const float* fh_conv2_b;
+    const float* mask0_w; const float* mask0_b; const float* mask2_w; const float* mask2_b;
+} GpsgUpdateWeights;
+GPSG_API size_t gpsg_update_workspace_bytes(int B, int H, int W);
+GPSG_API size_t gpsg_update_packed_bytes(void);
+GPSG_API int gpsg_update_pack(int device, void* stream, GpsgUpdateWeights weights, void* packed);
+GPSG_API int gpsg_update_step(int device, void* stream, int B, int H, int W, int corr_dtype, const void* corr,
+                              float* coords1, const void* net, const void* czrq, int64_t czrq_batch_stride,
+                              void* mask_out, const void* packed, void* workspace);
+
 /* ---- fused photometric loss on the rendered image (SURVEY.md 8f-4)-----------------------------------------------
  * replaces  0.8 * l1_loss(img, gt) + 0.2 * (1 - ssim(img, gt))  (train_stage2.py:70-72; lib/loss.py:35-72: 11x11 Gaussian
  * window sigma 1.5, zero padding, C1 = 0.01^2, C2 = 0.03^2, means over all planes*H*W elements) and its autograd.
