@@ -242,6 +242,22 @@ lib.gpsg_decoder1_forward.restype = _i
 lib.gpsg_decoder1_forward.argtypes = [_i, _vp, _i, _i, _i, _vp, _vp, _vp, Decoder1Weights, _vp, _vp]
 
 
+class Decoder23Weights(C.Structure):
+    """GpsgDecoder23Weights (include/gpsg.h), passed by value: the 20 device pointers of decoder3's or decoder2's
+    parameters, in GpsgDecoder1Weights' field order (`DECODER1_PARAMS`)."""
+    _fields_ = [(n, C.c_void_p) for n in DECODER1_PARAMS]
+
+
+lib.gpsg_decoder3_workspace_bytes.restype = _sz
+lib.gpsg_decoder3_workspace_bytes.argtypes = [_i, _i, _i]
+lib.gpsg_decoder3_forward.restype = _i
+lib.gpsg_decoder3_forward.argtypes = [_i, _vp, _i, _i, _i, _vp, _vp, Decoder23Weights, _vp, _vp]
+lib.gpsg_decoder2_workspace_bytes.restype = _sz
+lib.gpsg_decoder2_workspace_bytes.argtypes = [_i, _i, _i]
+lib.gpsg_decoder2_forward.restype = _i
+lib.gpsg_decoder2_forward.argtypes = [_i, _vp, _i, _i, _i, _vp, _vp, _vp, Decoder23Weights, _vp, _vp]
+
+
 class EncoderDownWeights(C.Structure):
     """GpsgEncoderDownWeights (include/gpsg.h), passed by value: the 20 device pointers of one down stage (res2 or res3),
     in GpsgDecoder1Weights' field order (`DECODER1_PARAMS`)."""
@@ -295,7 +311,8 @@ EXPORTED = ["gpsg_last_error", "gpsg_version", "gpsg_rasterize_forward", "gpsg_r
             "gpsg_jpeg_encode_workspace_bytes", "gpsg_jpeg_encode", "gpsg_gs_head_workspace_bytes",
             "gpsg_gs_head_forward", "gpsg_gs_head_backward_workspace_bytes", "gpsg_gs_head_backward",
             "gpsg_encoder_stem_workspace_bytes", "gpsg_encoder_stem_forward", "gpsg_decoder1_workspace_bytes",
-            "gpsg_decoder1_forward", "gpsg_encoder_down_workspace_bytes", "gpsg_encoder_down_forward",
+            "gpsg_decoder1_forward", "gpsg_decoder3_workspace_bytes", "gpsg_decoder3_forward",
+            "gpsg_decoder2_workspace_bytes", "gpsg_decoder2_forward", "gpsg_encoder_down_workspace_bytes", "gpsg_encoder_down_forward",
             "gpsg_update_workspace_bytes", "gpsg_update_packed_bytes", "gpsg_update_pack", "gpsg_update_step"]
 
 BWD_DETERMINISTIC = 1     # GPSG_BWD_DETERMINISTIC (include/gpsg.h)

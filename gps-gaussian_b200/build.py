@@ -41,6 +41,7 @@ SOURCES = {
     "encoder_stem.cu": [],
     "encoder_down.cu": [],
     "decoder1.cu": [],
+    "decoder23.cu": [],
     "update_block.cu": [],
     "mesh_render.cu": ["-fmad=false"],
     "jpeg_decode.cu": [],

@@ -29,7 +29,7 @@
 //                      shifted descriptor of a dense row.  The 1x1 downsample is the centre tap (even[j], middle
 //                      row) against its own weights, into a second accumulator.  5 x 129 pixel halo per chunk.
 //                      S = 1: stride 1, stages relu(GN(y)).  S = 2: stride 1, stages xb = relu(GN(yd) + relu(GN(y))).
-//                      Persistent, one CTA per SM.
+//                      Persistent, one CTA per SM.  (fused_conv.cuh, shared with decoder23.cu.)
 //   res_conv<P,48,S>   res2's three 48 -> 48 convolutions with resident weights (fused_conv.cuh, shared with decoder1).
 //   gn_finalize<C>     per (sample, group): the tiles' partials merged in fp64 in a fixed order (fused_norm.cuh).
 //   res_out<P,C>       out = relu(xb + relu(GN(ye))) from yd, yb, ye, written NCHW (fused_conv.cuh).
@@ -55,34 +55,13 @@ namespace {
 using namespace sm90;
 
 constexpr int kThreads = kFcThreads;
-constexpr int kTW = kFcTW;                 // tile: 2 output rows x 64 columns
-constexpr int kRows = 2;
-constexpr int kKC = 16;                    // input channels per K chunk
+constexpr int kRows = kFcDownRows;         // tile: 2 output rows x 64 columns
+constexpr int kKC = kFcKC;                 // input channels per K chunk
 
 // the C -> C convolutions of res2 (C = 48) keep all their weights in shared memory (fused_conv.cuh's res_conv, shared
 // with decoder1); res3's (C = 96, 332 KB in TF32) run on down_conv in K chunks
 template <int C>
 constexpr bool kResident = C == 48;
-
-constexpr int align128(int n) { return (n + 127) / 128 * 128; }
-
-// shared-memory layout of one stage buffer: [halo][3x3 weights][1x1 weights (S = 0)], each 128-byte aligned
-template <bool H, int C, int S>
-struct Shape {
-    using T = typename Prec<H>::T;
-    static constexpr int kPer = Prec<H>::kPer;
-    static constexpr int kNCG = kKC / kPer;                          // 16-byte channel groups per chunk: 4 / 2
-    static constexpr int kHY = S == 0 ? 2 * kRows + 1 : kRows + 2;   // halo rows
-    static constexpr int kHX = S == 0 ? 2 * kTW + 1 : kTW + 2;       // halo pixels per row (S = 0: even then odd)
-    static constexpr int kABytes = align128(kNCG * kHY * kHX * 16);  // [cg][hy][hx][kPer]
-    static constexpr int kW3 = 9 * kKC * C;                          // elements: [tap][cg][n][kPer]
-    static constexpr int kW1 = S == 0 ? kKC * C : 0;                 // elements: [cg][n][kPer]
-    static constexpr int kWBytes = (kW3 + kW1) * (int)sizeof(T);
-    static constexpr int kStage = kABytes + kWBytes;
-    static constexpr size_t kSmem = (size_t)2 * kStage;
-    static_assert(kWBytes % 128 == 0, "operand alignment");
-    static_assert(kSmem + 4096 <= 227 * 1024, "shared memory");
-};
 
 // ---- weights -------------------------------------------------------------------------------------------------------
 // Packed per convolution, chunk by chunk as staged: conv k's chunk q holds [tap][cg][n][kPer] of its 3x3 weights for
@@ -109,160 +88,6 @@ __global__ void down_pack(GpsgEncoderDownWeights wt, typename Prec<H>::T* __rest
             v = w[(n * C + chunk * kCh + cg * kPer + e) * 9 + tap];
         }
         out[i] = P::from_f(P::op(v));
-    }
-}
-
-// ---- convolutions ----------------------------------------------------------------------------------------------------
-template <bool H>
-struct ConvArgs {
-    using T = typename Prec<H>::T;
-    const float* x;           // S = 0: the stage input v [B,Cin,Hi,Wi] NCHW fp32
-    const T* yb;              // S = 1, 2: the raw input [B,Hi,Wi,Cin] NHWC and its GroupNorm's A, C
-    const float2* pb;
-    const T* yx;              // S = 2: the downsample branch's raw yd and its GroupNorm's A, C
-    const float2* px;
-    const T* wpack;           // this convolution's packed weights
-    const float* bias;
-    const float* bias_d;      // S = 0: the downsample's bias
-    T* y;
-    T* yd;                    // S = 0: the downsample's raw output
-    double* part;
-    double* part_d;
-};
-
-// one step = (tile, chunk): the chunk's packed weights by cp.async and its input halo, rounded to the operand type,
-// zero outside the image, into stage buffer `st`
-template <bool H, int CIN, int C, int S>
-__device__ __forceinline__ void stage(unsigned char* st, const ConvArgs<H>& a, int Hi, int Wi, int b, int y0, int x0,
-                                      int chunk, int tid) {
-    using P = Prec<H>;
-    using Sh = Shape<H, C, S>;
-    constexpr int kPer = P::kPer, kNCG = Sh::kNCG;
-    const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(a.wpack) + (size_t)chunk * Sh::kWBytes;
-    for (int i = tid; i < Sh::kWBytes / 16; i += kThreads) cp_async16(st + Sh::kABytes + 16 * i, wsrc + 16 * i);
-    uint4* sA = reinterpret_cast<uint4*>(st);
-    if constexpr (S == 0) {
-        // row hy is input row 2 y0 - 1 + hy; pixel p < 64 is input column 2 (x0 + p), p >= 64 is 2 (x0 + p - 64) - 1
-        const size_t plane = (size_t)Hi * Wi;
-        for (int i = tid; i < kNCG * Sh::kHY * Sh::kHX; i += kThreads) {
-            const int p = i % Sh::kHX, hy = i / Sh::kHX % Sh::kHY, cg = i / (Sh::kHX * Sh::kHY);
-            const int iy = 2 * y0 - 1 + hy, ix = p < kTW ? 2 * (x0 + p) : 2 * (x0 + p - kTW) - 1;
-            const bool in = iy >= 0 && iy < Hi && ix >= 0 && ix < Wi;
-            float v[kPer];
-            const float* src = a.x + ((size_t)b * CIN + chunk * kKC + cg * kPer) * plane + (size_t)(in ? iy : 0) * Wi +
-                               (in ? ix : 0);
-#pragma unroll
-            for (int e = 0; e < kPer; ++e) v[e] = in ? P::op(__ldg(src + e * plane)) : 0.f;
-            sA[(cg * Sh::kHY + hy) * Sh::kHX + p] = pack<H>(v);
-        }
-    } else {
-        // one work item is one 16-byte channel group of one halo pixel, the groups of a pixel in consecutive threads
-        const size_t hw = (size_t)Hi * Wi;
-        for (int i = tid; i < kNCG * Sh::kHY * Sh::kHX; i += kThreads) {
-            const int cg = i % kNCG, px = i / kNCG, hx = px % Sh::kHX, hy = px / Sh::kHX;
-            const int iy = y0 + hy - 1, ix = x0 + hx - 1;
-            const bool in = iy >= 0 && iy < Hi && ix >= 0 && ix < Wi;
-            const int ch = chunk * kKC + cg * kPer;
-            const size_t off = ((size_t)b * hw + (size_t)(in ? iy : 0) * Wi + (in ? ix : 0)) * CIN + ch;
-            float v[kPer];
-            unpack<H>(in ? __ldg(reinterpret_cast<const uint4*>(a.yb + off)) : make_uint4(0, 0, 0, 0), v);
-#pragma unroll
-            for (int e = 0; e < kPer; ++e) {
-                const float2 A = __ldg(a.pb + b * CIN + ch + e);
-                v[e] = relu(fmaf(v[e], A.x, A.y));
-            }
-            if constexpr (S == 2) {
-                float r[kPer];
-                unpack<H>(in ? __ldg(reinterpret_cast<const uint4*>(a.yx + off)) : make_uint4(0, 0, 0, 0), r);
-#pragma unroll
-                for (int e = 0; e < kPer; ++e) {
-                    const float2 D = __ldg(a.px + b * CIN + ch + e);
-                    v[e] = relu(fmaf(r[e], D.x, D.y) + v[e]);
-                }
-            }
-#pragma unroll
-            for (int e = 0; e < kPer; ++e) v[e] = in ? P::op(v[e]) : 0.f;
-            sA[(cg * Sh::kHY + hy) * Sh::kHX + hx] = pack<H>(v);
-        }
-    }
-}
-
-template <bool H, int CIN, int C, int S>
-__global__ void __launch_bounds__(kThreads, 1)
-down_conv(int B, int Hi, int Wi, int Ho, int Wo, ConvArgs<H> a) {
-    using Sh = Shape<H, C, S>;
-    constexpr int kNCG = Sh::kNCG, kNChunk = CIN / kKC, kG = C / 8;
-    constexpr bool kDown = S == 0;
-    extern __shared__ __align__(128) unsigned char smem[];  // 2 x [halo][3x3 weights][1x1 weights]
-    __shared__ double red[8 * kG], res[kG];
-    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 3;
-
-    const ConvTiles tl(B, Ho, Wo, kRows);
-    const int64_t mine = blockIdx.x < tl.n ? (tl.n - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-    const int64_t steps = mine * kNChunk;
-    if (steps > 0) {
-        int b, y0, x0;
-        tl.at(blockIdx.x, kRows, b, y0, x0);
-        stage<H, CIN, C, S>(smem, a, Hi, Wi, b, y0, x0, 0, tid);
-    }
-    cp_async_wait_all();
-    fence_async();
-    __syncthreads();
-    const uint32_t base = smem_addr(smem);
-    float acc[1][C / 2], accd[1][kDown ? C / 2 : 1];
-    for (int64_t q = 0; q < steps; ++q) {
-        const int chunk = (int)(q % kNChunk), buf = (int)(q & 1);
-        const int64_t tile = blockIdx.x + (q / kNChunk) * gridDim.x;
-        if (chunk == 0) {
-#pragma unroll
-            for (int i = 0; i < C / 2; ++i) acc[0][i] = 0.f;
-            if constexpr (kDown)
-#pragma unroll
-                for (int i = 0; i < C / 2; ++i) accd[0][i] = 0.f;
-        }
-        fence_acc(acc[0]);
-        if constexpr (kDown) fence_acc(accd[0]);
-        // made opaque so that the descriptors are not hoisted out of the step loop and kept live in registers
-        const uint32_t sb = opaque(base + (uint32_t)(buf * Sh::kStage));
-        wgmma_fence();
-        const uint64_t aD = gmma_desc(sb, Sh::kHY * Sh::kHX * 16, 128), wD = gmma_desc(sb + Sh::kABytes, C * 16, 128);
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-            const int dy = tap / 3, dx = tap % 3;
-            // a descriptor advances by its 16-byte offset added to the start-address field (addresses < 256 KB: no carry)
-            const int px = kDown ? (2 * wg + dy) * Sh::kHX + (dx == 0 ? kTW : (dx == 1 ? 0 : kTW + 1))
-                                 : (wg + dy) * Sh::kHX + dx;
-            const uint64_t at = aD + (uint64_t)px, bt = wD + (uint64_t)(tap * kNCG * C);
-#pragma unroll
-            for (int s = 0; s < kNCG / 2; ++s)
-                conv_mma<H, C>(acc[0], at + (uint64_t)(2 * s * Sh::kHY * Sh::kHX), bt + (uint64_t)(2 * s * C));
-        }
-        if constexpr (kDown) {
-            // the 1x1 downsample: the centre tap (middle row, even columns) against the 1x1 weights
-            const uint64_t at = aD + (uint64_t)((2 * wg + 1) * Sh::kHX), dD = wD + (uint64_t)(9 * kNCG * C);
-#pragma unroll
-            for (int s = 0; s < kNCG / 2; ++s)
-                conv_mma<H, C>(accd[0], at + (uint64_t)(2 * s * Sh::kHY * Sh::kHX), dD + (uint64_t)(2 * s * C));
-        }
-        wgmma_commit();
-        if (q + 1 < steps) {                            // stage the next chunk while the MMAs run
-            int b, y0, x0;
-            tl.at(blockIdx.x + ((q + 1) / kNChunk) * gridDim.x, kRows, b, y0, x0);
-            stage<H, CIN, C, S>(smem + (buf ^ 1) * Sh::kStage, a, Hi, Wi, b, y0, x0, (int)((q + 1) % kNChunk), tid);
-        }
-        wgmma_wait();
-        fence_acc(acc[0]);
-        if constexpr (kDown) fence_acc(accd[0]);
-        if (chunk == kNChunk - 1) {
-            int b, y0, x0;
-            tl.at(tile, kRows, b, y0, x0);
-            conv_emit<H, C, 1>(acc, LdgBias{a.bias + 2 * t}, a.y, a.part, tile, b, y0, x0, Ho, Wo, tid, red, res);
-            if constexpr (kDown)
-                conv_emit<H, C, 1>(accd, LdgBias{a.bias_d + 2 * t}, a.yd, a.part_d, tile, b, y0, x0, Ho, Wo, tid, red, res);
-        }
-        cp_async_wait_all();
-        fence_async();
-        __syncthreads();                                // the next buffer is complete; this one may be refilled
     }
 }
 
@@ -295,7 +120,7 @@ unsigned grid_of(int64_t tiles, int sms, int occ) {
 
 template <bool H, int CIN, int C, int S>
 int launch_conv(int B, int Hi, int Wi, int Ho, int Wo, const ConvArgs<H>& a, int sms, cudaStream_t stream) {
-    constexpr size_t smem = Shape<H, C, S>::kSmem;
+    constexpr size_t smem = DownShape<H, C, S>::kSmem;
     auto k = down_conv<H, CIN, C, S>;
     GPSG_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;

@@ -1,5 +1,5 @@
-// fused_conv.cuh -- the GroupNorm-fused pieces of a ResidualBlock chain shared by decoder1.cu (TF32, C = 48) and
-// encoder_down.cu (res2: TF32 and fp16, C = 48; res3's C = 96 epilogue and output):
+// fused_conv.cuh -- the GroupNorm-fused pieces of a ResidualBlock chain shared by decoder1.cu (TF32, C = 48),
+// encoder_down.cu (res2: TF32 and fp16, C = 48; res3: C = 96) and decoder23.cu (TF32, C = 96 and 64):
 //   ConvTiles          the tile walk: `rows` output rows x 64 columns of one sample per tile.
 //   conv_emit          the epilogue of an m64nC accumulator: bias, output rounding, the raw NHWC store and the tile's
 //                      GroupNorm partials (count, mean, M2) per group of 8 channels.
@@ -7,7 +7,18 @@
 //                      weights resident in shared memory.  A tile is 2 rows x 64 columns (warpgroup r owns row r); the
 //                      4 x 66 x C halo is double-buffered, so the next tile is staged while the current one's MMAs run.
 //                      S = 1 stages relu(GN(y)); S = 2 stages xb = relu(GN(yd) + relu(GN(y))).  Persistent, one CTA per
-//                      SM.  The weights fit for C = 48 (81 KiB TF32, 40.5 KiB fp16), not for C = 96.
+//                      SM.  The weights fit for C = 48 (81 KiB TF32, 40.5 KiB fp16), not for C = 64 or 96.
+//   down_conv<P, Cin, C, S>  a 3x3 convolution Cin -> C as an implicit GEMM whose K dimension (9 taps x Cin) runs in
+//                      chunks of 16 input channels, for weights that do not fit in shared memory.  A tile is 2 output
+//                      rows x 64 columns (warpgroup r owns row r); a chunk's stage buffer holds its input halo and its
+//                      packed weights (cp.async, re-read from L2 per tile), and two buffers let the next (tile, chunk)
+//                      be staged while the current one's MMAs run.  Persistent, one CTA per SM.  Staging modes:
+//                      S = 0  stride 2 from an NCHW fp32 input, with the 1x1 / stride-2 downsample into a second
+//                             accumulator (polyphase halo, see encoder_down.cu);
+//                      S = 1  stride 1, stages relu(GN(y));  S = 2  stride 1, stages xb = relu(GN(yd) + relu(GN(y)));
+//                      S = 3  stride 1 from cat(x', x1, x2) of two or three NCHW fp32 sources, x' optionally the
+//                             bilinear x2 of x (torch's upsample_bilinear2d indexing), with the 1x1 downsample as the
+//                             centre tap of the same halo into a second accumulator.
 //   res_out<P, C>      out = relu(xb + relu(GN(ye))) with xb = relu(GN(yd) + relu(GN(yb))), written NCHW fp32.
 // P is the precision (conv_prec.cuh).  The GroupNorm statistics are fused_norm.cuh's.
 #pragma once
@@ -41,11 +52,14 @@ struct ConvTiles {
 // D[64 x N] += A B on the precision's wgmma: TF32 k8 or f16 k16 (two 16-byte K core matrices either way)
 template <bool H, int N>
 __device__ __forceinline__ void conv_mma(float (&d)[N / 2], uint64_t a, uint64_t b) {
+    static_assert(N == 48 || N == 64 || N == 96, "conv_mma: N = 48, 64 or 96");
     if constexpr (H) {
         if constexpr (N == 48) sm90::wgmma_m64n48k16_f16(d, a, b);
+        else if constexpr (N == 64) sm90::wgmma_m64n64k16_f16(d, a, b);
         else sm90::wgmma_m64n96k16_f16(d, a, b);
     } else {
         if constexpr (N == 48) sm90::wgmma_m64n48k8(d, a, b);
+        else if constexpr (N == 64) sm90::wgmma_m64n64k8(d, a, b);
         else sm90::wgmma_m64n96k8(d, a, b);
     }
 }
@@ -250,6 +264,231 @@ res_conv(int B, int Hh, int W, const typename Prec<H>::T* __restrict__ yb, const
         conv_emit<H, C, 1>(acc, bv, y, part, tile, b, y0, x0, Hh, W, tid, red, res);
         sm90::fence_async();
         __syncthreads();                                 // the next buffer is complete; this one may be refilled
+    }
+}
+
+// ---- down_conv: a K-chunked 3x3 convolution ------------------------------------------------------------------------
+constexpr int kFcKC = 16;                  // input channels per K chunk
+constexpr int kFcDownRows = 2;             // tile: 2 output rows x 64 columns
+
+constexpr int fc_align128(int n) { return (n + 127) / 128 * 128; }
+
+// shared-memory layout of one down_conv stage buffer: [halo][3x3 weights][1x1 weights (S = 0, 3)], each 128-byte aligned
+template <bool H, int C, int S>
+struct DownShape {
+    using T = typename Prec<H>::T;
+    static constexpr int kPer = Prec<H>::kPer;
+    static constexpr bool kDown = S == 0 || S == 3;                         // with the 1x1 downsample
+    static constexpr int kNCG = kFcKC / kPer;                               // 16-byte channel groups per chunk: 4 / 2
+    static constexpr int kHY = S == 0 ? 2 * kFcDownRows + 1 : kFcDownRows + 2;  // halo rows
+    static constexpr int kHX = S == 0 ? 2 * kFcTW + 1 : kFcTW + 2;          // halo pixels per row (S = 0: even, odd)
+    static constexpr int kABytes = fc_align128(kNCG * kHY * kHX * 16);      // [cg][hy][hx][kPer]
+    static constexpr int kW3 = 9 * kFcKC * C;                               // elements: [tap][cg][n][kPer]
+    static constexpr int kW1 = kDown ? kFcKC * C : 0;                       // elements: [cg][n][kPer]
+    static constexpr int kWBytes = (kW3 + kW1) * (int)sizeof(T);
+    static constexpr int kStage = kABytes + kWBytes;
+    static constexpr size_t kSmem = (size_t)2 * kStage;
+    static_assert(kWBytes % 128 == 0, "operand alignment");
+    static_assert(kSmem + 4096 <= 227 * 1024, "shared memory");
+};
+
+template <bool H>
+struct ConvArgs {
+    using T = typename Prec<H>::T;
+    const float* x;           // S = 0: the stage input v [B,Cin,Hi,Wi] NCHW fp32; S = 3: v's first source
+    const T* yb;              // S = 1, 2: the raw input [B,Hi,Wi,Cin] NHWC and its GroupNorm's A, C
+    const float2* pb;
+    const T* yx;              // S = 2: the downsample branch's raw yd and its GroupNorm's A, C
+    const float2* px;
+    const T* wpack;           // this convolution's packed weights
+    const float* bias;
+    const float* bias_d;      // S = 0, 3: the downsample's bias
+    T* y;
+    T* yd;                    // S = 0, 3: the downsample's raw output
+    double* part;
+    double* part_d;
+    // S = 3: v = cat(x', x1, x2) [B,Cin,Hi,Wi] from NCHW fp32 sources of n0, n1 and Cin - n0 - n1 channels (multiples of
+    // 16, so every chunk comes from one source); x' = x [B,n0,Hi,Wi], or with up2 its bilinear x2 from x [B,n0,Hi/2,Wi/2]
+    const float* x1;
+    const float* x2;
+    int n0, n1, up2;
+};
+
+// one step = (tile, chunk): the chunk's packed weights by cp.async and its input halo, rounded to the operand type,
+// zero outside the image, into stage buffer `st`
+template <bool H, int CIN, int C, int S>
+__device__ __forceinline__ void stage_down(unsigned char* st, const ConvArgs<H>& a, int Hi, int Wi, int b, int y0,
+                                           int x0, int chunk, int tid) {
+    using P = Prec<H>;
+    using Sh = DownShape<H, C, S>;
+    constexpr int kPer = P::kPer, kNCG = Sh::kNCG;
+    const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(a.wpack) + (size_t)chunk * Sh::kWBytes;
+    for (int i = tid; i < Sh::kWBytes / 16; i += kFcThreads) sm90::cp_async16(st + Sh::kABytes + 16 * i, wsrc + 16 * i);
+    uint4* sA = reinterpret_cast<uint4*>(st);
+    if constexpr (S == 0) {
+        // row hy is input row 2 y0 - 1 + hy; pixel p < 64 is input column 2 (x0 + p), p >= 64 is 2 (x0 + p - 64) - 1
+        const size_t plane = (size_t)Hi * Wi;
+        for (int i = tid; i < kNCG * Sh::kHY * Sh::kHX; i += kFcThreads) {
+            const int p = i % Sh::kHX, hy = i / Sh::kHX % Sh::kHY, cg = i / (Sh::kHX * Sh::kHY);
+            const int iy = 2 * y0 - 1 + hy, ix = p < kFcTW ? 2 * (x0 + p) : 2 * (x0 + p - kFcTW) - 1;
+            const bool in = iy >= 0 && iy < Hi && ix >= 0 && ix < Wi;
+            float v[kPer];
+            const float* src = a.x + ((size_t)b * CIN + chunk * kFcKC + cg * kPer) * plane + (size_t)(in ? iy : 0) * Wi +
+                               (in ? ix : 0);
+#pragma unroll
+            for (int e = 0; e < kPer; ++e) v[e] = in ? P::op(__ldg(src + e * plane)) : 0.f;
+            sA[(cg * Sh::kHY + hy) * Sh::kHX + p] = pack<H>(v);
+        }
+    } else if constexpr (S == 3) {
+        // the chunk's source and its first channel there; the halo pixel of row hy, column hx is (y0 + hy - 1, x0 + hx - 1)
+        const int c0 = chunk * kFcKC;
+        const bool up = c0 < a.n0 && a.up2;
+        const float* src;
+        int cs, nc;
+        if (c0 < a.n0) src = a.x, cs = c0, nc = a.n0;
+        else if (c0 < a.n0 + a.n1) src = a.x1, cs = c0 - a.n0, nc = a.n1;
+        else src = a.x2, cs = c0 - a.n0 - a.n1, nc = CIN - a.n0 - a.n1;
+        const int Hs = up ? Hi / 2 : Hi, Ws = up ? Wi / 2 : Wi;
+        const size_t plane = (size_t)Hs * Ws;
+        for (int i = tid; i < kNCG * Sh::kHY * Sh::kHX; i += kFcThreads) {
+            const int hx = i % Sh::kHX, hy = i / Sh::kHX % Sh::kHY, cg = i / (Sh::kHX * Sh::kHY);
+            const int iy = y0 + hy - 1, ix = x0 + hx - 1;
+            float v[kPer];
+#pragma unroll
+            for (int e = 0; e < kPer; ++e) v[e] = 0.f;
+            if (iy >= 0 && iy < Hi && ix >= 0 && ix < Wi) {
+                const float* sb = src + ((size_t)b * nc + cs + cg * kPer) * plane;
+                if (up) {
+                    int ya, yb, xa, xb;
+                    float ly0, ly1, lx0, lx1;
+                    bilinear_index(iy, Hs, ya, yb, ly0, ly1);
+                    bilinear_index(ix, Ws, xa, xb, lx0, lx1);
+#pragma unroll
+                    for (int e = 0; e < kPer; ++e) {
+                        const float* p = sb + e * plane;
+                        const float v00 = __ldg(p + (size_t)ya * Ws + xa), v01 = __ldg(p + (size_t)ya * Ws + xb);
+                        const float v10 = __ldg(p + (size_t)yb * Ws + xa), v11 = __ldg(p + (size_t)yb * Ws + xb);
+                        v[e] = P::op(ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11));
+                    }
+                } else {
+                    const size_t px = (size_t)iy * Ws + ix;
+#pragma unroll
+                    for (int e = 0; e < kPer; ++e) v[e] = P::op(__ldg(sb + e * plane + px));
+                }
+            }
+            sA[(cg * Sh::kHY + hy) * Sh::kHX + hx] = pack<H>(v);
+        }
+    } else {
+        // one work item is one 16-byte channel group of one halo pixel, the groups of a pixel in consecutive threads
+        const size_t hw = (size_t)Hi * Wi;
+        for (int i = tid; i < kNCG * Sh::kHY * Sh::kHX; i += kFcThreads) {
+            const int cg = i % kNCG, px = i / kNCG, hx = px % Sh::kHX, hy = px / Sh::kHX;
+            const int iy = y0 + hy - 1, ix = x0 + hx - 1;
+            const bool in = iy >= 0 && iy < Hi && ix >= 0 && ix < Wi;
+            const int ch = chunk * kFcKC + cg * kPer;
+            const size_t off = ((size_t)b * hw + (size_t)(in ? iy : 0) * Wi + (in ? ix : 0)) * CIN + ch;
+            float v[kPer];
+            unpack<H>(in ? __ldg(reinterpret_cast<const uint4*>(a.yb + off)) : make_uint4(0, 0, 0, 0), v);
+#pragma unroll
+            for (int e = 0; e < kPer; ++e) {
+                const float2 A = __ldg(a.pb + b * CIN + ch + e);
+                v[e] = relu(fmaf(v[e], A.x, A.y));
+            }
+            if constexpr (S == 2) {
+                float r[kPer];
+                unpack<H>(in ? __ldg(reinterpret_cast<const uint4*>(a.yx + off)) : make_uint4(0, 0, 0, 0), r);
+#pragma unroll
+                for (int e = 0; e < kPer; ++e) {
+                    const float2 D = __ldg(a.px + b * CIN + ch + e);
+                    v[e] = relu(fmaf(r[e], D.x, D.y) + v[e]);
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < kPer; ++e) v[e] = in ? P::op(v[e]) : 0.f;
+            sA[(cg * Sh::kHY + hy) * Sh::kHX + hx] = pack<H>(v);
+        }
+    }
+}
+
+template <bool H, int CIN, int C, int S>
+__global__ void __launch_bounds__(kFcThreads, 1)
+down_conv(int B, int Hi, int Wi, int Ho, int Wo, ConvArgs<H> a) {
+    using Sh = DownShape<H, C, S>;
+    constexpr int kNCG = Sh::kNCG, kNChunk = CIN / kFcKC, kG = C / 8, kRows = kFcDownRows;
+    constexpr bool kDown = Sh::kDown;
+    static_assert(CIN % kFcKC == 0, "K chunks");
+    extern __shared__ __align__(128) unsigned char smem_dc[];  // 2 x [halo][3x3 weights][1x1 weights]
+    __shared__ double red[8 * kG], res[kG];
+    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 3;
+
+    const ConvTiles tl(B, Ho, Wo, kRows);
+    const int64_t mine = blockIdx.x < tl.n ? (tl.n - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+    const int64_t steps = mine * kNChunk;
+    if (steps > 0) {
+        int b, y0, x0;
+        tl.at(blockIdx.x, kRows, b, y0, x0);
+        stage_down<H, CIN, C, S>(smem_dc, a, Hi, Wi, b, y0, x0, 0, tid);
+    }
+    sm90::cp_async_wait_all();
+    sm90::fence_async();
+    __syncthreads();
+    const uint32_t base = sm90::smem_addr(smem_dc);
+    float acc[1][C / 2], accd[1][kDown ? C / 2 : 1];
+    for (int64_t q = 0; q < steps; ++q) {
+        const int chunk = (int)(q % kNChunk), buf = (int)(q & 1);
+        const int64_t tile = blockIdx.x + (q / kNChunk) * gridDim.x;
+        if (chunk == 0) {
+#pragma unroll
+            for (int i = 0; i < C / 2; ++i) acc[0][i] = 0.f;
+            if constexpr (kDown)
+#pragma unroll
+                for (int i = 0; i < C / 2; ++i) accd[0][i] = 0.f;
+        }
+        sm90::fence_acc(acc[0]);
+        if constexpr (kDown) sm90::fence_acc(accd[0]);
+        // made opaque so that the descriptors are not hoisted out of the step loop and kept live in registers
+        const uint32_t sb = sm90::opaque(base + (uint32_t)(buf * Sh::kStage));
+        sm90::wgmma_fence();
+        const uint64_t aD = sm90::gmma_desc(sb, Sh::kHY * Sh::kHX * 16, 128),
+                       wD = sm90::gmma_desc(sb + Sh::kABytes, C * 16, 128);
+#pragma unroll 1
+        for (int tap = 0; tap < 9; ++tap) {
+            const int dy = tap / 3, dx = tap % 3;
+            // a descriptor advances by its 16-byte offset added to the start-address field (addresses < 256 KB: no carry)
+            const int px = S == 0 ? (2 * wg + dy) * Sh::kHX + (dx == 0 ? kFcTW : (dx == 1 ? 0 : kFcTW + 1))
+                                  : (wg + dy) * Sh::kHX + dx;
+            const uint64_t at = aD + (uint64_t)px, bt = wD + (uint64_t)(tap * kNCG * C);
+#pragma unroll
+            for (int s = 0; s < kNCG / 2; ++s)
+                conv_mma<H, C>(acc[0], at + (uint64_t)(2 * s * Sh::kHY * Sh::kHX), bt + (uint64_t)(2 * s * C));
+        }
+        if constexpr (kDown) {
+            // the 1x1 downsample: the centre tap (S = 0: middle row, even columns) against the 1x1 weights
+            const int pc = S == 0 ? (2 * wg + 1) * Sh::kHX : (wg + 1) * Sh::kHX + 1;
+            const uint64_t at = aD + (uint64_t)pc, dD = wD + (uint64_t)(9 * kNCG * C);
+#pragma unroll
+            for (int s = 0; s < kNCG / 2; ++s)
+                conv_mma<H, C>(accd[0], at + (uint64_t)(2 * s * Sh::kHY * Sh::kHX), dD + (uint64_t)(2 * s * C));
+        }
+        sm90::wgmma_commit();
+        if (q + 1 < steps) {                            // stage the next chunk while the MMAs run
+            int b, y0, x0;
+            tl.at(blockIdx.x + ((q + 1) / kNChunk) * gridDim.x, kRows, b, y0, x0);
+            stage_down<H, CIN, C, S>(smem_dc + (buf ^ 1) * Sh::kStage, a, Hi, Wi, b, y0, x0, (int)((q + 1) % kNChunk), tid);
+        }
+        sm90::wgmma_wait();
+        sm90::fence_acc(acc[0]);
+        if constexpr (kDown) sm90::fence_acc(accd[0]);
+        if (chunk == kNChunk - 1) {
+            int b, y0, x0;
+            tl.at(tile, kRows, b, y0, x0);
+            conv_emit<H, C, 1>(acc, LdgBias{a.bias + 2 * t}, a.y, a.part, tile, b, y0, x0, Ho, Wo, tid, red, res);
+            if constexpr (kDown)
+                conv_emit<H, C, 1>(accd, LdgBias{a.bias_d + 2 * t}, a.yd, a.part_d, tile, b, y0, x0, Ho, Wo, tid, red, res);
+        }
+        sm90::cp_async_wait_all();
+        sm90::fence_async();
+        __syncthreads();                                // the next buffer is complete; this one may be refilled
     }
 }
 

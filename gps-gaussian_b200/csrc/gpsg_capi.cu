@@ -1043,6 +1043,47 @@ int gpsg_decoder1_forward(int device, void* stream_, int B, int Hs, int Ws, cons
     return launch_decoder1(device, B, Hs, Ws, s, img_feat, depth_feat, weights, out, workspace, (cudaStream_t)stream_);
 }
 
+static bool decoder3_shape_ok(int B, int H, int W) {
+    return B >= 0 && H >= 1 && W >= 1 && H <= 65536 && W <= 65536 && (int64_t)B * H * W * 192 < (int64_t(1) << 40);
+}
+
+size_t gpsg_decoder3_workspace_bytes(int B, int H, int W) {
+    return (B > 0 && decoder3_shape_ok(B, H, W)) ? decoder3_workspace_bytes(B, H, W) : 0;
+}
+
+int gpsg_decoder3_forward(int device, void* stream_, int B, int H, int W, const float* img_feat, const float* depth_feat,
+                          GpsgDecoder23Weights weights, float* out, void* workspace) {
+    GPSG_REQUIRE(decoder3_shape_ok(B, H, W), "decoder3: needs H, W >= 1 and B >= 0");
+    if (B == 0) return GPSG_OK;
+    GPSG_REQUIRE(img_feat && depth_feat && out && workspace, "NULL pointer");
+    const float* const* w = &weights.b0_conv1_w;
+    for (int i = 0; i < 20; ++i) GPSG_REQUIRE(w[i], "decoder3: NULL weight pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 256 == 0, "decoder3: workspace must be 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_decoder3(device, B, H, W, img_feat, depth_feat, weights, out, workspace, (cudaStream_t)stream_);
+}
+
+static bool decoder2_shape_ok(int B, int Hs, int Ws) {
+    return B >= 0 && Hs >= 1 && Ws >= 1 && Hs <= 32768 && Ws <= 32768 &&
+           (int64_t)B * (2 * (int64_t)Hs) * (2 * (int64_t)Ws) * 192 < (int64_t(1) << 40);
+}
+
+size_t gpsg_decoder2_workspace_bytes(int B, int Hs, int Ws) {
+    return (B > 0 && decoder2_shape_ok(B, Hs, Ws)) ? decoder2_workspace_bytes(B, Hs, Ws) : 0;
+}
+
+int gpsg_decoder2_forward(int device, void* stream_, int B, int Hs, int Ws, const float* s, const float* img_feat,
+                          const float* depth_feat, GpsgDecoder23Weights weights, float* out, void* workspace) {
+    GPSG_REQUIRE(decoder2_shape_ok(B, Hs, Ws), "decoder2: needs Hs, Ws >= 1 and B >= 0");
+    if (B == 0) return GPSG_OK;
+    GPSG_REQUIRE(s && img_feat && depth_feat && out && workspace, "NULL pointer");
+    const float* const* w = &weights.b0_conv1_w;
+    for (int i = 0; i < 20; ++i) GPSG_REQUIRE(w[i], "decoder2: NULL weight pointer");
+    GPSG_REQUIRE((uintptr_t)workspace % 256 == 0, "decoder2: workspace must be 256-byte aligned");
+    GPSG_CUDA(cudaSetDevice(device));
+    return launch_decoder2(device, B, Hs, Ws, s, img_feat, depth_feat, weights, out, workspace, (cudaStream_t)stream_);
+}
+
 static bool update_shape_ok(int B, int H, int W) {
     return B >= 1 && H >= 1 && W >= 1 && H <= 65536 && W <= 65536 && (int64_t)B * H * W * 576 < (int64_t(1) << 40);
 }

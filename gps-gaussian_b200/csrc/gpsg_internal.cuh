@@ -296,6 +296,14 @@ int launch_update_step(int device, int B, int H, int W, int corr_dtype, const vo
 size_t decoder1_workspace_bytes(int B, int Hs, int Ws);
 int launch_decoder1(int device, int B, int Hs, int Ws, const float* s, const float* img_feat, const float* depth_feat,
                     const GpsgDecoder1Weights& wt, float* out, void* workspace, cudaStream_t stream);
+
+// decoder23.cu
+size_t decoder3_workspace_bytes(int B, int H, int W);
+size_t decoder2_workspace_bytes(int B, int Hs, int Ws);
+int launch_decoder3(int device, int B, int H, int W, const float* img_feat, const float* depth_feat,
+                    const GpsgDecoder23Weights& wt, float* out, void* workspace, cudaStream_t stream);
+int launch_decoder2(int device, int B, int Hs, int Ws, const float* s, const float* img_feat, const float* depth_feat,
+                    const GpsgDecoder23Weights& wt, float* out, void* workspace, cudaStream_t stream);
 int launch_sequence_loss_fwd(const GpsgSeqLossArgs& a, float* stats, void* workspace, cudaStream_t stream);
 int launch_sequence_loss_bwd(const GpsgSeqLossArgs& a, const float* grad_loss, const float* stats, cudaStream_t stream);
 // corr.cu

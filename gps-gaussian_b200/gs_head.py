@@ -232,14 +232,17 @@ def gs_head_train(up_src, img, depth, regresser):
     return _Tail.apply(up_src, img, depth, *params_of(regresser))
 
 
-def make_regresser_forward(orig, train=False, tail=True, decoder=False):
+def make_regresser_forward(orig, train=False, tail=True, decoder=False, deep=False):
     """`GSRegresser.forward` with parts of it on the kernels; otherwise `orig`, the reference's own method.
 
     tail: the full-resolution tail runs on the kernels when grad is disabled and the inputs are supported; with `train`,
     also when grad is enabled and the image does not require grad (`gs_head_train`).
     decoder: `decoder1` runs on the kernels (gps_gaussian_b200.decoder) when grad and autocast are off, cudnn.allow_tf32
     is on and `decoder.supported(...)` holds; the tail then runs on the kernels (with `tail`) or on the module's own
-    layers.  With grad enabled decoder1 always stays the module's."""
+    layers.  With grad enabled decoder1 always stays the module's.
+    deep: under the same conditions `decoder3` and `decoder2` run on the kernels (`decoder.run3`, `decoder.run2`) where
+    `decoder.deep_supported(...)` holds; their output feeds decoder1 (kernels or module) as it is.  Otherwise they run
+    on the module's own layers."""
     def forward(self, img, depth, img_feat):
         grad = torch.is_grad_enabled()
         autocast = torch.is_autocast_enabled()
@@ -247,12 +250,18 @@ def make_regresser_forward(orig, train=False, tail=True, decoder=False):
                    and not autocast and supported(self, img, depth, None))
         on_dec = (decoder and not grad and not autocast and torch.backends.cudnn.allow_tf32
                   and _decoder.supported(self, None, img_feat[0], None))
-        if not (on_tail or on_dec):
+        on_deep = (deep and not grad and not autocast and torch.backends.cudnn.allow_tf32 and torch.is_tensor(img_feat[2])
+                   and img_feat[2].is_cuda and _decoder._deep_module_supported(self))
+        if not (on_tail or on_dec or on_deep):
             return orig(self, img, depth, img_feat)
         img_feat1, img_feat2, img_feat3 = img_feat
         depth_feat1, depth_feat2, depth_feat3 = self.depth_encoder(depth)
-        x = self.decoder3(torch.cat([img_feat3, depth_feat3], dim=1))
-        x = self.decoder2(torch.cat([self.up(x), img_feat2, depth_feat2], dim=1))
+        if on_deep and _decoder.deep_supported(self, img_feat3, depth_feat3, img_feat2, depth_feat2):
+            p3, p2 = _decoder.deep_params_of(self)
+            x = _decoder.run2(_decoder.run3(img_feat3, depth_feat3, p3), img_feat2, depth_feat2, p2)
+        else:
+            x = self.decoder3(torch.cat([img_feat3, depth_feat3], dim=1))
+            x = self.decoder2(torch.cat([self.up(x), img_feat2, depth_feat2], dim=1))
         decoded = on_dec and _decoder.supported(self, x, img_feat1, depth_feat1)
         if decoded:
             x = _decoder.run(x, img_feat1, depth_feat1, _decoder.params_of(self))

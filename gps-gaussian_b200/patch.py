@@ -92,6 +92,13 @@ With grad enabled decoder1 always stays the module's; in every other case the ke
 own forward runs.  The output differs from cuDNN's by TF32 re-association, which is why the switch is opt-in.  Unset or
 any other value leaves decoder1 to the module.
 
+`GPSG_DECODER_DEEP=1`, read once by `install()`, takes effect together with GPSG_DECODER=1 (alone it does nothing): the
+method is rebound with `make_regresser_forward(..., deep=True)`, so that under the same conditions `decoder3` and
+`decoder2` (the 1/8- and 1/4-resolution ResidualBlock pairs, with the upsample and the concats of their inputs) run on
+the TF32 kernels of csrc/decoder23.cu too, where they are the reference's stage-2 layers (decoder_dims [48, 64, 96],
+encoder dims [32, 48, 96], GroupNorm).  Their output feeds decoder1's kernels as it is.  It differs from cuDNN's by TF32
+re-association, which is why this switch is opt-in as well.
+
 `GPSG_UPDATE=1`, read once by `install()`, also hooks `core.raft_stereo_human` and rebinds
 
     FlowUpdateModule.forward -> update.make_update_forward (a class method, kept in _ORIG_METHODS)
@@ -127,6 +134,7 @@ _GS_HEAD_TRAIN = False  # GPSG_GS_HEAD_TRAIN=1 at install()
 _ENCODER = False      # GPSG_ENCODER=1 at install()
 _DECODER = False      # GPSG_DECODER=1 at install()
 _ENCODER_DEEP = False  # GPSG_ENCODER=1 and GPSG_ENCODER_DEEP=1 at install()
+_DECODER_DEEP = False  # GPSG_DECODER=1 and GPSG_DECODER_DEEP=1 at install()
 _UPDATE = False       # GPSG_UPDATE=1 at install()
 
 
@@ -240,8 +248,9 @@ def _patch_regresser(mod):
     key = (cls, "forward")
     if key not in _ORIG_METHODS:
         _ORIG_METHODS[key] = cls.__dict__["forward"]
+    kw = {"deep": True} if _DECODER_DEEP else {}      # passed only when on: a factory without `deep` keeps working
     cls.forward = gs_head.make_regresser_forward(_ORIG_METHODS[key], train=_GS_HEAD_TRAIN,
-                                                 tail=_GS_HEAD or _GS_HEAD_TRAIN, decoder=_DECODER)
+                                                 tail=_GS_HEAD or _GS_HEAD_TRAIN, decoder=_DECODER, **kw)
 
 
 def _patch_extractor(mod):
@@ -436,9 +445,9 @@ _FINDER = _Finder()
 def install():
     """Hook future imports and patch what is already imported. Idempotent.  Reads GPSG_ANTIALIAS, GPSG_RECTIFY,
     GPSG_FLOW_HEAD, GPSG_DECODE, GPSG_ENCODE, GPSG_GS_HEAD, GPSG_GS_HEAD_TRAIN, GPSG_ENCODER, GPSG_ENCODER_DEEP,
-    GPSG_DECODER and GPSG_UPDATE here, once."""
+    GPSG_DECODER, GPSG_DECODER_DEEP and GPSG_UPDATE here, once."""
     global _ANTIALIAS, _RECTIFY, _FLOW_HEAD, _DECODE, _ENCODE, _GS_HEAD, _GS_HEAD_TRAIN, _ENCODER, _DECODER, _ENCODER_DEEP
-    global _UPDATE
+    global _UPDATE, _DECODER_DEEP
     _ANTIALIAS = os.environ.get("GPSG_ANTIALIAS", "") == "1"
     _RECTIFY = os.environ.get("GPSG_RECTIFY", "") == "1"
     _FLOW_HEAD = os.environ.get("GPSG_FLOW_HEAD", "") == "1"
@@ -449,6 +458,7 @@ def install():
     _ENCODER = os.environ.get("GPSG_ENCODER", "") == "1"
     _DECODER = os.environ.get("GPSG_DECODER", "") == "1"
     _ENCODER_DEEP = _ENCODER and os.environ.get("GPSG_ENCODER_DEEP", "") == "1"
+    _DECODER_DEEP = _DECODER and os.environ.get("GPSG_DECODER_DEEP", "") == "1"
     _UPDATE = os.environ.get("GPSG_UPDATE", "") == "1"
     if _FINDER not in sys.meta_path:
         sys.meta_path.insert(0, _FINDER)
@@ -522,6 +532,12 @@ def gs_head_train():
 def decoder():
     """Whether the installed patch runs the regressor's decoder1 on the fused kernels (GPSG_DECODER=1 at install())."""
     return _DECODER
+
+
+def decoder_deep():
+    """Whether the installed patch also runs the regressor's decoder3 and decoder2 on the fused kernels (GPSG_DECODER=1
+    and GPSG_DECODER_DEEP=1 at install())."""
+    return _DECODER_DEEP
 
 
 def encoder():

@@ -651,6 +651,46 @@ GPSG_API size_t gpsg_decoder1_workspace_bytes(int B, int Hs, int Ws);
 GPSG_API int gpsg_decoder1_forward(int device, void* stream, int B, int Hs, int Ws, const float* s, const float* img_feat,
                                    const float* depth_feat, GpsgDecoder1Weights weights, float* out, void* workspace);
 
+/* ---- decoder3 and decoder2 of the Gaussian-parameter regressor (reference lib/gs_parm_network.py), inference ----------
+ * gpsg_decoder3_forward: out [B,96,H,W] (NCHW fp32), the output of `decoder3` on cat(img_feat, depth_feat), from
+ * img_feat and depth_feat [B,96,H,W] (img_feat3, depth_feat3; NCHW fp32, contiguous, H, W >= 1).  GN: GroupNorm(12, 96).
+ * gpsg_decoder2_forward: out [B,64,H,W] (H = 2 Hs, W = 2 Ws), the output of `decoder2` on
+ * cat(up2x(s), img_feat, depth_feat), from s [B,96,Hs,Ws] (the decoder3 output), img_feat and depth_feat [B,48,H,W]
+ * (img_feat2, depth_feat2; Hs, Ws >= 1).  up2x is gpsg_decoder1_forward's.  GN: GroupNorm(8, 64).
+ * In both, with v the concatenated input [B,192,H,W] (never stored) and C the output channels:
+ *   block 0: ya = conv3x3(v, b0_conv1) ; yd = conv1x1(v, b0_down) ; yb = conv3x3(relu(GN(ya)), b0_conv2) ;
+ *            xb = relu(GN(yd) + relu(GN(yb)))       (no ReLU on the downsample branch before the add)
+ *   block 1: yc = conv3x3(xb, b1_conv1) ; ye = conv3x3(relu(GN(yc)), b1_conv2) ; out = relu(xb + relu(GN(ye)))
+ *   every convolution with its bias and zero padding 1 (3x3) or 0 (1x1).
+ *   GN(y): GroupNorm(C/8, C) per sample (8 channels per group) with its own weight and bias (norm1, norm2, norm3 in
+ *   order of use), biased variance, eps 1e-5, evaluated as fmaf(y, A, C) with A = w rstd and C = b - mean A rounded to
+ *   fp32, the statistics in fp64 from the stored fp32 y.  A non-finite value in a (sample, group) makes that group NaN;
+ *   ReLU keeps NaN.
+ *   Precision (cuDNN with allow_tf32): every convolution operand, weights and activations (the interpolated, normalized
+ *   and residual-added values included), rounded to TF32 (round to nearest, ties away); products and sums fp32 in an
+ *   unspecified order; the fp32 bias added after the sum.
+ *   Weights in torch's layouts, fp32 and contiguous, in GpsgDecoder1Weights' field order: b0_conv1_w [C,192,3,3],
+ *   b0_down_w [C,192,1,1], the other 3x3 weights [C,C,3,3], biases and GroupNorm weights / biases [C].
+ *   Bit-reproducible: no floating-point atomics; every sum has a fixed order given the shape and the device's SM count.
+ *   workspace: gpsg_decoder3_workspace_bytes(B, H, W) / gpsg_decoder2_workspace_bytes(B, Hs, Ws) bytes, 256-byte
+ *   aligned.  After the call it starts with the five raw convolution outputs ya, yd, yb, yc, ye in that order (bias
+ *   included, NHWC [B,H,W,C] fp32), the i-th at byte i * S with S = B H W C * 4 rounded up to a multiple of 256; then the
+ *   per-channel A, C, the per-tile GroupNorm partials and the TF32-packed weights.  B >= 0 (B = 0 does nothing); sizes
+ *   >= 1; NULL pointers are refused.  Enqueues on `stream` and does not synchronise. */
+typedef struct GpsgDecoder23Weights {
+    const float* b0_conv1_w; const float* b0_conv1_b; const float* b0_norm1_w; const float* b0_norm1_b;
+    const float* b0_conv2_w; const float* b0_conv2_b; const float* b0_norm2_w; const float* b0_norm2_b;
+    const float* b0_down_w; const float* b0_down_b; const float* b0_norm3_w; const float* b0_norm3_b;
+    const float* b1_conv1_w; const float* b1_conv1_b; const float* b1_norm1_w; const float* b1_norm1_b;
+    const float* b1_conv2_w; const float* b1_conv2_b; const float* b1_norm2_w; const float* b1_norm2_b;
+} GpsgDecoder23Weights;
+GPSG_API size_t gpsg_decoder3_workspace_bytes(int B, int H, int W);
+GPSG_API int gpsg_decoder3_forward(int device, void* stream, int B, int H, int W, const float* img_feat,
+                                   const float* depth_feat, GpsgDecoder23Weights weights, float* out, void* workspace);
+GPSG_API size_t gpsg_decoder2_workspace_bytes(int B, int Hs, int Ws);
+GPSG_API int gpsg_decoder2_forward(int device, void* stream, int B, int Hs, int Ws, const float* s, const float* img_feat,
+                                   const float* depth_feat, GpsgDecoder23Weights weights, float* out, void* workspace);
+
 /* ---- stride-2 residual stages of the UnetExtractor (reference core/extractor.py: res2, res3), inference -------------
  * gpsg_encoder_down_forward: out [B,C,Ho,Wo] (NCHW fp32, Ho = ceil(H/2), Wo = ceil(W/2)), the output of one stage of
  * two ResidualBlocks (the first with stride 2 and a 1x1 downsample) on input [B,Cin,H,W] (NCHW fp32, H, W >= 1);
