@@ -16,8 +16,16 @@ sum to fp16 and then the bias add to fp16, every elementwise op's result to fp16
 result is therefore a monotone function f of the exact fp64 convolution sums v, and the only freedom the kernels have
 is the fp32 accumulation error e of v.  `stage_checks` gives, per element, want = f(v) and the bound
 max |f(v +- e) - f(v)|: zero wherever e cannot move a rounding, one fp16 step where it can.  `emulate` chains the same
-stages on the CPU; its `mutant` argument swaps in one deliberate error (MUTANTS) so the tests can show that each breaks
-a check.
+stages on the CPU; its `mutant` argument swaps in one deliberate error so the tests can show that each breaks a check.
+MUTANTS are rounding and formula mistakes.  INDEX_MUTANTS have the shape of the bugs a persistent tiled GEMM tends to
+have (tiles of 2 rows x 64 columns of one sample, csrc/update_block.cu): a halo line of every tile read as zero
+(`seam_column_zero`: the column left and right of each 64-column tile, `halo_row_below_zero`: the row below each 2-row
+tile, both in every 3x3 GEMM convolution), convf1's 7x7 window clipped to 5x5, cz / cr / cq of sample b read at the
+packed stride 288 H W from the start of a wider context (`czrq_packed_stride`), two carried-state mistakes that need
+the previous iteration (`emulate(..., prev=)`): the GRU reading that iteration's hidden state (`h_stale`) and x's flow
+channels from its coords (`x_flow_stale`), and mask[2]'s N-block nb written at channel offset ((nb + 1) mod 3) 192
+(`mask_nblock_offset`).  Each moves some element by far more than the ACC K sum|a w| envelope at B = 2, H = 5,
+W = 130 (tests/test_update_cpu.py); none slips under it.
 """
 import torch
 import torch.nn.functional as F
@@ -27,6 +35,10 @@ from oracle.encoder_torch64 import F64, conv, ratio, relu  # noqa: F401  (ratio 
 HID = 96
 KEYS = ("cf1", "cf2", "x", "z", "rh", "h", "fh1", "m1", "delta", "mask", "coords1")
 MUTANTS = ("flow_unrounded", "bias_fp32", "sigmoid_unrounded_sum", "delta_y_kept", "mask_unscaled", "z_r_swapped")
+INDEX_MUTANTS = ("seam_column_zero", "halo_row_below_zero", "convf1_5x5", "czrq_packed_stride", "h_stale",
+                 "x_flow_stale", "mask_nblock_offset")
+TILE_H, TILE_W = 2, 64
+MASK_NB = 192         # mask[2]'s N-block: 576 channels in three
 # fp32 accumulation of K products on the tensor cores: 4 K units of 2^-24 of sum |a w| (room for the truncating adds)
 ACC = 2.0 ** -22
 # expf / tanhf in fp32 before the fp16 rounding: a few fp32 ulps
@@ -130,11 +142,35 @@ def loop64(params, fmap1, fmap2, net, czrq, iters, flow_init=None, test_mode=Tru
 
 # ---- the fp16 route: stages as monotone functions of the exact sums ----------------------------------------------------
 
-def _sum(a, w, pad=None):
-    """(v, e): the exact fp64 sum conv(a, w) of fp16-exact operands and the kernels' accumulation error bound."""
+def _sum(a, w, pad=None, mutant=None):
+    """(v, e): the exact fp64 sum conv(a, w) of fp16-exact operands and the kernels' accumulation error bound.  The tile
+    mutants replace v of a 3x3 convolution by `_halo_dropped`'s."""
     K = w[0].numel()
     v = conv(a, w, pad=pad)
+    if mutant in ("seam_column_zero", "halo_row_below_zero") and w.shape[-1] == 3:
+        v = _halo_dropped(a, w, mutant)
     return v, ACC * K * conv(a.abs(), w.abs(), pad=pad)
+
+
+def _halo_dropped(a, w, mutant):
+    """The 3x3 zero-padded conv(a, w) computed tile by tile with one halo line of each tile read as zero: the columns
+    left and right of every TILE_W-column tile, or the row below every TILE_H-row tile."""
+    B, _, H, W = a.shape
+    ap = F.pad(a, (1, 1, 1, 1))
+    out = torch.empty(B, w.shape[0], H, W, dtype=a.dtype, device=a.device)
+    if mutant == "seam_column_zero":
+        for x0 in range(0, W, TILE_W):
+            s = ap[..., x0:x0 + TILE_W + 2].clone()
+            s[..., 0] = 0
+            s[..., -1] = 0
+            out[..., x0:x0 + TILE_W] = conv(s, w, pad=0)
+    else:
+        for y0 in range(0, H, TILE_H):
+            s = ap[:, :, y0:y0 + TILE_H + 2].clone()
+            if s.shape[2] == TILE_H + 2:
+                s[:, :, -1] = 0
+            out[:, :, y0:y0 + TILE_H] = conv(s, w, pad=0)
+    return out
 
 
 def _envelope(f, v, e):
@@ -170,12 +206,21 @@ def _sfu(fn, v, e):
 
 def stages(params, inp, mutant=None):
     """Every stage of one iteration from its own fp16 inputs in `inp` (h_in, corr, coords1_in, czrq and the stored
-    cf1, cf2, x, z, rh, h, fh1, m1, delta): {key: (want, bound)}.  `mutant` in MUTANTS injects one error."""
-    assert mutant is None or mutant in MUTANTS, mutant
+    cf1, cf2, x, z, rh, h, fh1, m1, delta): {key: (want, bound)}.  `mutant` in MUTANTS or INDEX_MUTANTS injects one
+    error; h_stale and x_flow_stale read inp's h_stale / coords1_stale."""
+    assert mutant is None or mutant in MUTANTS + INDEX_MUTANTS, mutant
     W = [(r16(w.to(inp["h_in"].device)), b.to(inp["h_in"].device)) for w, b in _split(params)]
     (c1, c2, f1, f2, cv, cwz, cwr, cwq, fh1, fh2, m0, m2) = W
+    B, _, H, Wd = inp["coords1_in"].shape
+    if mutant == "czrq_packed_stride":
+        c = inp["czrq"]
+        inp = {**inp, "czrq": torch.as_strided(c, c.shape, (3 * HID * H * Wd, H * Wd, Wd, 1), c.storage_offset())}
+    if mutant == "convf1_5x5":
+        f1 = (f1[0].clone(), f1[1])
+        f1[0][..., (0, 6), :] = 0
+        f1[0][..., :, (0, 6)] = 0
     g = {k: v.to(F64) if torch.is_tensor(v) else v for k, v in inp.items()}
-    B, _, H, Wd = g["coords1_in"].shape
+    S = lambda a, w, pad=None: _sum(a, w, pad, mutant)
     bf = mutant == "bias_fp32"
     out = {}
     # motion encoder: convc1 on the fp16 corr, convf1 on the fp16 flow
@@ -183,17 +228,20 @@ def stages(params, inp, mutant=None):
     flow32 = (g["coords1_in"].to(torch.float32) - grid(B, H, Wd, dev).to(torch.float32)).to(F64)
     flow = flow32 if mutant == "flow_unrounded" else r16(flow32)
     relu_out = lambda b: (lambda v: relu(_conv_out(b, bf)(v)))
-    a = _envelope(relu_out(c1[1]), *_sum(r16(g["corr"]), c1[0]))
-    b = _envelope(relu_out(f1[1]), *_sum(flow, f1[0]))
+    a = _envelope(relu_out(c1[1]), *S(r16(g["corr"]), c1[0]))
+    b = _envelope(relu_out(f1[1]), *S(flow, f1[0]))
     out["cf1"] = (torch.cat([a[0], b[0]], 1), torch.cat([a[1], b[1]], 1))
     cf1 = g["cf1"]
-    a = _envelope(relu_out(c2[1]), *_sum(cf1[:, :64], c2[0]))
-    b = _envelope(relu_out(f2[1]), *_sum(cf1[:, 64:], f2[0]))
+    a = _envelope(relu_out(c2[1]), *S(cf1[:, :64], c2[0]))
+    b = _envelope(relu_out(f2[1]), *S(cf1[:, 64:], f2[0]))
     out["cf2"] = (torch.cat([a[0], b[0]], 1), torch.cat([a[1], b[1]], 1))
-    a = _envelope(relu_out(cv[1]), *_sum(g["cf2"], cv[0]))
-    out["x"] = (torch.cat([a[0], flow], 1), torch.cat([a[1], torch.zeros_like(flow)], 1))
+    a = _envelope(relu_out(cv[1]), *S(g["cf2"], cv[0]))
+    xf = flow
+    if mutant == "x_flow_stale":
+        xf = r16((g["coords1_stale"].to(torch.float32) - grid(B, H, Wd, dev).to(torch.float32)).to(F64))
+    out["x"] = (torch.cat([a[0], xf], 1), torch.cat([a[1], torch.zeros_like(flow)], 1))
     # GRU
-    h, x = g["h_in"], g["x"]
+    h, x = g["h_stale" if mutant == "h_stale" else "h_in"], g["x"]
     cz, cr, cq = g["czrq"].split(HID, 1)
     hx = torch.cat([h, x], 1)
     if mutant == "z_r_swapped":
@@ -201,21 +249,23 @@ def stages(params, inp, mutant=None):
     pre = lambda b, c: (lambda v: r16(_conv_out(b, bf)(v) + c))
     if mutant == "sigmoid_unrounded_sum":
         pre = lambda b, c: (lambda v: _conv_out(b, bf)(v) + c)
-    vz, ez = _sum(hx, cwz[0])
-    vr, er = _sum(hx, cwr[0])
+    vz, ez = S(hx, cwz[0])
+    vr, er = S(hx, cwr[0])
     out["z"] = _sfu(lambda v, s: _sig(pre(cwz[1], cz)(v), s), vz, ez)
     out["rh"] = _sfu(lambda v, s: r16(_sig(pre(cwr[1], cr)(v), s) * h), vr, er)
     # rh is monotone in v with the sign of h: the envelope's max over both ends holds either way
-    vq, eq = _sum(torch.cat([g["rh"], x], 1), cwq[0])
+    vq, eq = S(torch.cat([g["rh"], x], 1), cwq[0])
     z = g["z"]
     upd = lambda v, s: r16(r16(r16(1 - z) * h) + r16(z * _tanh(pre(cwq[1], cq)(v), s)))
     out["h"] = _sfu(upd, vq, eq)
     # heads from the new h
-    out["fh1"] = _envelope(relu_out(fh1[1]), *_sum(g["h"], fh1[0]))
-    out["m1"] = _envelope(relu_out(m0[1]), *_sum(g["h"], m0[0]))
-    out["delta"] = _envelope(_conv_out(fh2[1], bf), *_sum(g["fh1"], fh2[0]))
+    out["fh1"] = _envelope(relu_out(fh1[1]), *S(g["h"], fh1[0]))
+    out["m1"] = _envelope(relu_out(m0[1]), *S(g["h"], m0[0]))
+    out["delta"] = _envelope(_conv_out(fh2[1], bf), *S(g["fh1"], fh2[0]))
     scale = 1.0 if mutant == "mask_unscaled" else .25
-    out["mask"] = _envelope(lambda v: r16(scale * _conv_out(m2[1], bf)(v)), *_sum(g["m1"], m2[0], pad=0))
+    out["mask"] = _envelope(lambda v: r16(scale * _conv_out(m2[1], bf)(v)), *S(g["m1"], m2[0], pad=0))
+    if mutant == "mask_nblock_offset":
+        out["mask"] = tuple(t.roll(MASK_NB, 1) for t in out["mask"])
     d = g["delta"].clone()
     if mutant != "delta_y_kept":
         d[:, 1] = 0
@@ -224,10 +274,13 @@ def stages(params, inp, mutant=None):
     return out
 
 
-def emulate(params, corr, coords1, net, czrq, mutant=None):
+def emulate(params, corr, coords1, net, czrq, mutant=None, prev=None):
     """One iteration of the fp16 route on the CPU, each stage from the previous stages' emulated outputs: a dict with
-    the inputs (h_in, corr, coords1_in, czrq) and every key of KEYS.  `mutant` in MUTANTS injects one error."""
+    the inputs (h_in, corr, coords1_in, czrq) and every key of KEYS.  `mutant` in MUTANTS or INDEX_MUTANTS injects one
+    error; prev, the previous iteration's emulate() dict, holds the stale state h_stale and x_flow_stale read."""
     g = dict(h_in=net.to(F64), corr=corr.to(F64), coords1_in=coords1.to(F64), czrq=czrq.to(F64))
+    if prev is not None:
+        g.update(h_stale=prev["h_in"], coords1_stale=prev["coords1_in"])
     order = ("cf1", "cf2", "x", "z", "rh", "h", "fh1", "m1", "delta", "mask", "coords1")
     for k in order:
         g[k] = _stage(params, g, k, mutant)

@@ -1,7 +1,9 @@
 """CPU: the update-block entry points are exported and declared, the workspace and packed sizes, refusals, the parameter
 order against the reference's own BasicMultiUpdateBlock, the `supported` truth table for every fallback condition, the
 GPSG_UPDATE switch (alone without GPSG_PATCH it does nothing; it composes with the other switches), and every mutant of
-the fp16-route emulation caught by a stage check."""
+the fp16-route emulation caught by a stage check: the rounding mutants at 2 x 9 x 7, the index mutants (tile halos, the
+convf1 window, the context stride, stale carried state, the mask's N-block offset) on a second iteration at B = 2,
+H = 5, W = 130, whose two full 64-column tiles, partial third and three 2-row tiles put a seam in every direction."""
 import os
 import re
 import subprocess
@@ -271,3 +273,38 @@ def test_every_mutant_caught(mutant_case, mutant):
         g = ut.emulate(ps, inp["corr"], inp["coords1"], inp["net"], inp["czrq"], mutant=mutant)
         worst = max(worst, max(_worst(ps, g).values()))
     assert worst > 1.0, mutant
+
+
+# ---- the emulation's index mutants: two column tiles and a partial third, three row tiles ------------------------------
+
+@pytest.fixture(scope="module")
+def index_case():
+    """The second iteration at B = 2, H = 5, W = 130, from the emulated first, with cz / cr / cq split from channels
+    32 .. 319 of a [B,384,H,W] context."""
+    B, H, W = 2, 5, 130
+    inp = uc.inputs(B, H, W)
+    outer = uc.inputs(B, H, W, seed=7)["czrq"]
+    wide = torch.cat([outer[:, :32], inp["czrq"], outer[:, 32:96]], 1)
+    czrq = wide[:, 32:320]
+    ps = _off_fp16(uc.params(0))
+    first = ut.emulate(ps, inp["corr"], inp["coords1"], inp["net"], czrq)
+    return ps, inp["corr"], first, czrq
+
+
+def _second(case, mutant=None):
+    ps, corr, first, czrq = case
+    return ut.emulate(ps, corr, first["coords1"], first["h"], czrq, mutant=mutant, prev=first)
+
+
+def test_emulation_passes_its_checks_on_tiles(index_case):
+    ps, _, first, _ = index_case
+    assert max(_worst(ps, first).values()) == 0.0
+    assert max(_worst(ps, _second(index_case)).values()) == 0.0
+
+
+@pytest.mark.parametrize("mutant", ut.INDEX_MUTANTS)
+def test_every_index_mutant_caught(index_case, mutant):
+    ps = index_case[0]
+    worst = _worst(ps, _second(index_case, mutant))
+    print(f"{mutant}: {worst}")
+    assert max(worst.values()) > 1.0, (mutant, worst)

@@ -4,7 +4,8 @@ and the fp16-route stage bounds (oracle/update_torch64.py).
 Every stage of one iteration is checked per element from the kernels' own stored inputs to it: the fp16 route is a
 monotone function of the exact convolution sums, so the bound is zero wherever the fp32 accumulation error cannot move
 a rounding.  Sizes: the 1/8-resolution maps of a 1024^2 pair at B = 2 and 4, odd shapes down to 1 x 1 and widths that
-are not a multiple of the 64-column tile, corr in fp16 and fp32, and the golden inputs.  Three test-mode and three
+are not a multiple of the 64-column tile, corr in fp16 and fp32, and the golden inputs; the outputs and the workspace
+are NaN before each launch.  Three test-mode and three
 training-mode iterations through `make_update_forward` on the reference's own FlowUpdateModule: the kernel route's error
 against the fp64 loop is at most twice that of the module's own autocast route.  flow_init, non-finite inputs, repeats,
 every fallback bit for bit, and with the staged reference the RtStereoHumanModel eval forward with GPSG_UPDATE on and
@@ -26,6 +27,24 @@ from oracle import update_torch64 as ut
 pytestmark = pytest.mark.gpu
 needs_ref = pytest.mark.skipif(harness.staged_reference() is None, reason="oracle/_ref not staged")
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "update_golden.npz")
+
+
+@pytest.fixture(autouse=True)
+def poisoned_outputs(monkeypatch):
+    """torch.empty inside update returns NaN-filled floating buffers and 0xFF-filled bytes (NaN in every fp16 view of
+    the workspace), so an element the kernels skip shows."""
+    def nan(fn):
+        def make(*a, **k):
+            t = fn(*a, **k)
+            if t.is_floating_point():
+                t.fill_(float("nan"))
+            elif t.dtype == torch.uint8:
+                t.fill_(0xFF)
+            return t
+        return make
+    fake = types.SimpleNamespace(**{n: getattr(torch, n) for n in dir(torch) if not n.startswith("__")})
+    fake.empty, fake.empty_like = nan(torch.empty), nan(torch.empty_like)
+    monkeypatch.setattr(update, "torch", fake)
 
 
 def params(seed):
